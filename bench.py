@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- rows/sec of the scoring hot path at batch = 65 536 x 23 features (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--model gbdt100d6|rf100d6]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--model gbdt100d6|rf100d6] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 One "step" = one pass of the hot path over one 65 536-row batch of synthetic credit-default rows
@@ -18,6 +18,11 @@ Printed by rank 0: ONE JSON line.
   roofline   algorithmic bytes (100 B/row: 92 B features in, 4 B probability + 4 B label out) / the average
              per-launch device time measured live in the timed region, against the measured HBM peak.
   cpu_baseline  the reference-style sklearn pipeline's predict_proba on this box's host cores (rank 0, N=1).
+  device     the GPU's name and power limit: both are part of every time above.
+
+--dump-outputs DIR (rank 0) writes what the timed paths computed in their last step: value_proba1.npy / value_label.npy
+(the device-resident leg's last batch) and e2e_predictions.npy (the last B200Model.predict call).  The inputs are seeded,
+so two builds run with the same arguments can be compared output for output.
 
 --impl reference times that CPU path alone (all host cores, process pool) and prints the same line shape.
 """
@@ -30,6 +35,7 @@ import os
 import statistics
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -48,7 +54,7 @@ def emit(obj) -> None:
     os.write(_REAL_STDOUT, (json.dumps(obj) + "\n").encode())
 
 BATCH = 65536
-POOL = 32  # distinct device-resident batches: 32 * 6.29 MB = 201 MB > 126 MB L2
+POOL = 32  # distinct device-resident batches: 32 * 6.29 MB = 201 MB of 96-byte rows > 50 MB L2
 ALG_BYTES_PER_ROW = 100  # SURVEY.md section 8(d): 92 B in + 4 B proba + 4 B label
 MOM_BYTES_PER_ROW = 92
 METRIC = "rows/sec at batch=65536x23f"
@@ -135,7 +141,7 @@ def get_pipeline(name: str, dist: Dist):
     from databricks_kubernetes_mlops_poc_b200 import training
 
     kind, params = MODELS[name]
-    cache_dir = os.environ.get("B2F_BENCH_CACHE", "/tmp/b2f_bench_cache")
+    cache_dir = os.environ.get("B2F_BENCH_CACHE", os.path.join(tempfile.gettempdir(), f"b2f_bench_cache_{os.getuid()}"))
     os.makedirs(cache_dir, exist_ok=True)
     n_train = N_TRAIN_BY_MODEL.get(name, N_TRAIN)
     path = os.path.join(cache_dir, f"{name}_n{n_train}_s{TRAIN_SEED}_sk{sklearn.__version__}.joblib")
@@ -217,19 +223,26 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s at 700 W)"
 
 
-def ncu_traffic(model_name: str):
-    """dram bytes per launch from the committed ncu capture, if one exists for this model."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        try:
-            v = json.load(open(p)).get(model_name, {})
-            return v.get("dram_bytes_per_launch") if isinstance(v, dict) else None
-        except Exception:
-            return None
-    return None
+def device_record(index: int) -> dict:
+    """Name and power limit of the GPU the numbers were measured on (read-only nvidia-smi query)."""
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
+        return {"name": out[0], "power_limit_w": float(out[1]), "sm_max_mhz": float(out[2])}
+    except (OSError, ValueError, IndexError, subprocess.TimeoutExpired):
+        return {"name": None, "power_limit_w": None, "sm_max_mhz": None}
+
+
+def dump_outputs(path: str, arrays: dict) -> None:
+    """Write each array as <path>/<name>.npy (float32 / float64 only)."""
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(path, f"{name}.npy"), a)
 
 
 # ----------------------------------------------------------------------------- CPU baseline
@@ -284,8 +297,8 @@ def cpu_port_rate(pipe, codes, nums, repeats: int):
 
 
 def cpu_bandwidth() -> float:
-    """CPUs the container may burn (cgroup CFS quota / period), 0.0 when unlimited.  The B200 boxes give a 128-CPU host a quota
-    of 16: more busy workers than that (forked sklearn processes, polling encoder threads) get the whole cgroup throttled."""
+    """CPUs the container may burn (cgroup CFS quota / period), 0.0 when unlimited.  A container's quota can be far below the
+    host's CPU count: more busy workers than that (forked sklearn processes, polling encoder threads) get the whole cgroup throttled."""
     try:
         q, per = open("/sys/fs/cgroup/cpu.max").read().split()[:2]
         return 0.0 if q == "max" else float(q) / float(per)
@@ -354,8 +367,7 @@ def host_thread_share(dist: Dist) -> int:
     """Encoder threads for this rank.  One rank: the library's default (the GPU's NUMA node, capped by the container's CPU
     bandwidth -- `b2f_host_threads_default`).  Under torchrun the ranks share the host: a rank takes the physical cores of its
     GPU's NUMA node divided by the ranks whose GPUs sit on that node, plus two, and never more than its share of the CPU
-    quota.  (Measured on the 8-GPU box, 2 x 32 cores, quota 96: 8 ranks x 10 threads 548 M rows/s, x 7: 489 M, x 13: 502 M;
-    4 ranks -- all four GPUs on node 0 -- x 10: 368 M, x 14: 306 M, x 22: 256 M.)"""
+    quota."""
     env = os.environ.get("B200_HOST_THREADS")
     if env:
         return int(env)
@@ -371,7 +383,7 @@ def host_thread_share(dist: Dist) -> int:
     my_node = lib.b2f_device_numa_node(dist.local_rank, ctypes.byref(ncpu))
     if my_node >= 0 and ncpu.value > 0:
         on_my_node = sum(1 for r in range(local_world) if lib.b2f_device_numa_node(r, None) == my_node)
-        share = (ncpu.value // 2) // max(1, on_my_node) + 2  # two hyper-threads per core on the B200 hosts
+        share = (ncpu.value // 2) // max(1, on_my_node) + 2  # assumes two hyper-threads per core
     else:
         share = (os.cpu_count() or 2) // 2 // max(1, local_world) + 2
     limit = float(lib.b2f_host_cpu_limit())
@@ -389,7 +401,7 @@ def run_b200(args, dist: Dist):
 
     K, W = args.steps, max(args.warmup, 3)
     # one process per GPU: live on the GPU's socket (the DataFrame the encoder threads read, the Python heap the response lists
-    # are built in and the pinned staging then share a NUMA node; on the 8-GPU box ranks 4-7 serve GPUs of node 1)
+    # are built in and the pinned staging then share a NUMA node; on a two-socket host half of the ranks serve GPUs of node 1)
     bound_cpus = 0
     lib0 = _cabi.load_library()
     if os.environ.get("B200_BIND_CALLER", "1") != "0" and (dist.world > 1 or lib0.b2f_device_count() == 1):
@@ -431,6 +443,14 @@ def run_b200(args, dist: Dist):
     l0 = eng.info()["launches"]
     _, ms_total = eng.predict_stream_timed(d_rows, BATCH, POOL, d_proba, False, d_label, K, fmt=fmt, per_launch=False)
     launches_value = eng.info()["launches"] - l0
+    dumps = {}
+    if args.dump_outputs and dist.rank == 0:  # the last timed launch scored batch (K - 1) % POOL
+        b_last = (K - 1) % POOL
+        last_p = np.empty(BATCH, dtype=np.float32)
+        last_l = np.empty(BATCH, dtype=np.int32)
+        eng.d2h(last_p, d_proba + b_last * BATCH * 4)
+        eng.d2h(last_l, d_label + b_last * BATCH * 4)
+        dumps = {"value_proba1": last_p, "value_label": last_l.astype(np.float32)}
     dist.barrier()
     ms_total_max = dist.max(ms_total)
     value = dist.world * BATCH * K / (ms_total_max * 1e-3)
@@ -518,6 +538,9 @@ def run_b200(args, dist: Dist):
         stages.append(model.last_timing)
     plugin_s = time.perf_counter() - t0
     launches_plugin = eng.info()["launches"] - l0
+    if args.dump_outputs and dist.rank == 0:
+        dumps["e2e_predictions"] = np.asarray(out0["predictions"], dtype=np.float64)
+        dump_outputs(args.dump_outputs, dumps)
     dist.barrier()
     plugin_value = dist.world * BATCH * K / dist.max(plugin_s)
     st = [s for s in stages if s]
@@ -641,7 +664,7 @@ def run_b200(args, dist: Dist):
             "workload": workload_label(args.model),
             "forest": args.model, "trees": info0["n_trees"], "depth": info0["max_depth"], "nodes": flat.total_nodes, "batch": BATCH,
             "parallelism": f"dp{dist.world} (rows sharded, forest replicated, no collective)",
-            "l2": f"inputs rotate over {POOL} distinct batches ({POOL * BATCH * row_bytes / 1e6:.0f} MB of rows + {POOL * BATCH * 8 / 1e6:.0f} MB of results > 126 MB L2)",
+            "l2": f"inputs rotate over {POOL} distinct batches ({POOL * BATCH * row_bytes / 1e6:.0f} MB of rows + {POOL * BATCH * 8 / 1e6:.0f} MB of results > 50 MB L2)",
             "walk": info0["walk"], "row_format": f"{fmt_name}: {row_bytes}-byte encoded rows",
             "kernel": kernel_used,
         },
@@ -661,12 +684,13 @@ def run_b200(args, dist: Dist):
                       "pcie_h2d_gbs_one_batch": h2d_gbs},
         "gpu_launches": int(launches_value),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": ncu_traffic(args.model), "peak_source": peak_src, "kernel": kernel_used,
+                     "peak_source": peak_src, "kernel": kernel_used,
                      "alg_bytes_per_launch": ALG_BYTES_PER_ROW * BATCH, "avg_launch_ms": avg_launch_ms,
                      "how": "timed region / launches (back-to-back launches overlap head and tail: programmatic dependent launch)",
                      "isolated_launch_ms": float(np.mean(iso_ms)), "isolated_launch_min_ms": float(np.min(iso_ms)),
                      "actual_bytes_per_launch": BATCH * (row_bytes + 8)},
         "clocks": clocks,
+        "device": device_record(dist.local_rank),
         "sustained_rows_per_s": sustained,
         "parity_max_abs_dp_vs_sklearn_2048rows_all_ranks": parity, "parity_labels_equal_all_ranks": labels_equal,
     }
@@ -979,7 +1003,9 @@ def run_stream(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=200,
+                    help="timed steps K of value, e2e, e2e_c_abi (synchronous and pipelined) and the outlier-forest leg; the isolated-launch "
+                         "timing takes min(K, 100); the moments, drift and latency-sweep legs use fixed call counts")
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--model", default="gbdt100d6", choices=sorted(MODELS))
@@ -999,7 +1025,10 @@ def main():
     ap.add_argument("--stream-rows", type=int, default=10_000_000)
     ap.add_argument("--quick", action="store_true", help="only the timed value / e2e legs (no sweep, stream, cpu baseline, outliers, drift)")
     ap.add_argument("--stream-gpus", type=int, default=0, help="GPUs used by --stream (0 = all visible)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     if args.quick:
         args.no_sweep = args.no_stream = args.no_cpu = args.no_outliers = args.no_drift = args.no_gib = True
 

@@ -1,9 +1,9 @@
-"""b200-forest-serve: B200-native scoring engine for the credit-default service.
+"""b200-forest-serve: H100-native scoring engine for the credit-default service.
 
 Drop-in for the hot path of nfmoore/databricks-kubernetes-mlops-poc:
 ``POST /predict`` -> ``model.predict(DataFrame) -> dict`` (reference ``app/main.py:42-86``,
 ``databricks/src/02-register-model.ipynb:330-353``), with the sklearn pipeline arithmetic replaced by
-hand-written sm_100a CUDA kernels behind a C ABI (``include/b2f.h``).  No CPU fallback.
+hand-written sm_90a CUDA kernels behind a C ABI (``include/b2f.h``).  No CPU fallback.
 """
 
 from .flatten import FlatForest, flatten_pipeline  # noqa: F401

@@ -33,11 +33,11 @@
 #include "json_rows.h"
 #include "row_encoder.h"
 
-#define B2F_VERSION_STR "b200forest 0.1.0 (sm_100a)"
+#define B2F_VERSION_STR "b200forest 0.1.0 (sm_90a)"
 #define B2F_STREAMS 4
 #define B2F_TICKETS 256
 #define B2F_CHUNK_ROWS 16384
-#define B2F_FLUSH_BYTES (256ull << 20) /* > 126 MB L2 */
+#define B2F_FLUSH_BYTES (256ull << 20) /* > 50 MB L2 */
 
 /* ------------------------------------------------------------------ errors */
 static thread_local char g_err[512] = "";
@@ -538,8 +538,8 @@ static int model_init_cuda(b2f_model *m, const uint8_t *blob, size_t nbytes) {
     CUDA_TRY(cudaSetDevice(m->device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, m->device));
-    if (prop.major < 10)
-        return set_err(B2F_ENODEV, "device %d is sm_%d%d; this library is built for sm_100a (B200) only", m->device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return set_err(B2F_ENODEV, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", m->device, prop.major, prop.minor);
     m->sm_count = prop.multiProcessorCount;
     CUDA_TRY(cudaDeviceGetAttribute(&m->max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, m->device));
 
@@ -590,7 +590,10 @@ static int model_init_cuda(b2f_model *m, const uint8_t *blob, size_t nbytes) {
     }
     const char *cr = getenv("B2F_CHUNK_ROWS"); /* tuning hook: rows per pipelined H2D/kernel/D2H chunk */
     if (cr && atoll(cr) >= 1024) m->chunk_rows = atoll(cr);
-    m->chunk_plan = {768}; /* measured best on B200 for 65 536-row batches: 3/4 of the batch, then the rest */
+    /* 65 536-row batches: 3/4 of the batch, then the rest.  tools/chunk_plan_sweep.py on an H100 80GB HBM3 (700 W): the best of
+     * nine plans for both row formats -- 88 us p50 per ranked-row call against 108 us in one chunk, 145 us against 158 us with
+     * 64-byte rows */
+    m->chunk_plan = {768};
     if (const char *pl = getenv("B2F_CHUNK_PLAN")) {
         m->chunk_plan.clear();
         for (const char *q = pl; *q;) {
@@ -600,11 +603,11 @@ static int model_init_cuda(b2f_model *m, const uint8_t *blob, size_t nbytes) {
         }
     }
     /* latency kernel: while rows x groups warps still fit about two waves of the chip */
-    /* the latency form (one CTA per 2 rows, warp = tree group) hands over to the warp-per-row kernel at 3 072 rows: measured on
-     * B200 (profiles/r02_split_threshold.json, synchronous 64-byte-row calls) it is never slower below that -- GBDT 500 x d8:
-     * 35 vs 60 us at 1 024 rows, 59 vs 71 at 3 072, equal at 4 096; GBDT 100 x d6: equal from 512 rows up.  (Round 1 scaled the
-     * threshold with the number of tree groups: 592 rows for 500 trees, which left 768..3 072-row requests on the slower kernel.) */
-    m->split_max_rows = 3072;
+    /* the latency form (one CTA per 2 rows, warp = tree group) hands over to the warp-per-row kernel at 2 048 rows: below that
+     * the warp-per-row kernel leaves most SMs idle while the latency form spreads one row's trees over a CTA's warps.
+     * tools/split_threshold.py on an H100 80GB HBM3 (700 W), synchronous 64-byte-row calls, GBDT 500 x d8: 38 vs 64 us at 512
+     * rows, 72 vs 80 at 2 048, 89 vs 79 at 3 072; GBDT 100 x d6: within ~5 us of each other at every size up to 4 096. */
+    m->split_max_rows = 2048;
     if (const char *sp = getenv("B2F_SPLIT_MAX_ROWS")) m->split_max_rows = atoll(sp);
     if (kn_env_is("warp") || kn_env_is("tile")) m->split_max_rows = 0; /* tests pin one kernel */
     if (kn_env_is("split")) m->split_max_rows = INT64_MAX;
@@ -670,8 +673,8 @@ static int model_init_cuda(b2f_model *m, const uint8_t *blob, size_t nbytes) {
             CUDA_TRY(cudaFuncSetAttribute(k_forest_predict_tile<true, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, m->tile_smem_bytes));
             CUDA_TRY(cudaFuncSetAttribute(k_forest_predict_tile<true, double>, cudaFuncAttributeMaxDynamicSharedMemorySize, m->tile_smem_bytes));
             m->tile_ok = true;
-            /* crossover measured on B200 (tools/ksweep.py): a resident forest ties with the warp kernel from
-             * 65 536 rows up (and sums in sklearn's tree order); a streamed forest wins from ~24k rows */
+            /* crossover chosen on the previous GPU generation and kept, not re-measured on the H100: a resident forest ties
+             * with the warp kernel from 65 536 rows up (and sums in sklearn's tree order); a streamed forest wins from ~24k rows */
             m->tile_min_rows = (tp.n_pieces <= tp.n_slots) ? 65536 : 24576;
             if (tm && atoll(tm) >= 0) m->tile_min_rows = atoll(tm);
             if (kn && !strcmp(kn, "tile")) m->tile_min_rows = 1;

@@ -62,7 +62,7 @@ static int drift_init(b2f_drift *d, const double *ref_sorted, const int32_t *cat
     CUDA_TRY(cudaSetDevice(d->device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, d->device));
-    if (prop.major < 10) return set_err(B2F_ENODEV, "device %d is sm_%d%d; this library is built for sm_100a (B200) only", d->device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return set_err(B2F_ENODEV, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", d->device, prop.major, prop.minor);
     d->sm_count = prop.multiProcessorCount;
     d->cat_off.assign(d->n_cat + 1, 0);
     for (int c = 0; c < d->n_cat; ++c) {

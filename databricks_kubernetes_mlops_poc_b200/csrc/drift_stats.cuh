@@ -325,8 +325,11 @@ __device__ __forceinline__ double sweep_block(const SweepConst &c, int tid, int 
  * Rows live in a global scratch (L2), element i at (i mod CH) * NT + i / CH so that thread t owns the CH consecutive
  * columns [t CH, (t+1) CH) and every load / store of a pass is coalesced; row j is scaled by 2^-E_j, E_j the exponent of
  * its largest binomial, so nothing overflows.  Sums run in a fixed order (deterministic).  p = W(m,n) / C(m+n, n). */
-#define B2F_DRIFT_ROWSCAN_MAX 48       /* global-scratch form: ~20 us per row, the sweep is faster beyond */
-#define B2F_DRIFT_ROWSCAN_SMEM_MAX 448  /* shared-memory form: ~3.5 us per row; the sweep (2.0 ms at 30 000 reference rows) wins beyond ~480 */
+/* Limits measured with tools/drift_time.py against 30 000 reference rows on an H100 80GB HBM3 (700 W), device ms per request:
+ * global-scratch row scan 1.11 at 48 rows vs the sweep's 1.76; shared-memory row scan 1.31 at 320 rows, 2.38 at 512 vs the
+ * sweep's 2.15 / 2.17 -- the crossover lies between 320 and 512 rows. */
+#define B2F_DRIFT_ROWSCAN_MAX 48       /* global-scratch form: two dependent L2 trips per row, the sweep is faster beyond */
+#define B2F_DRIFT_ROWSCAN_SMEM_MAX 448  /* shared-memory form: cost grows per row, the sweep's is flat in n */
 #define B2F_DRIFT_ROWSCAN_SMEM_LIMIT 1024 /* what B2F_DRIFT_ROWSCAN_SMEM may raise it to (32 factors per lane in the binomial products) */
 #define B2F_DRIFT_ROWSCAN_CAP 28672     /* doubles of the shared-memory row ring (224 KB of the 227 KB a CTA may have) */
 /* doubles per scratch row: the transposed layout (i mod CH) * NT + i / CH spans CH * NT >= m + 1 slots */
@@ -462,15 +465,15 @@ __device__ double rows_scan(const SweepConst &c, double *buf0, double *buf1, int
 }
 
 /* ---- the row-scan with the row RESIDENT IN SHARED MEMORY ---------------------------------------------------------------
- * The global-scratch form above pays two dependent trips to L2 per row (~20 us per row measured: it loses to the sweep beyond
- * ~48 rows).  A row only ever needs its in-band cells [lo_j, hi_j], at most 2h/ng + 1 of them, and the interval only moves
+ * The global-scratch form above pays two dependent trips to L2 per row (it loses to the sweep beyond
+ * B2F_DRIFT_ROWSCAN_MAX rows).  A row only ever needs its in-band cells [lo_j, hi_j], at most 2h/ng + 1 of them, and the interval only moves
  * right: cell i lives in slot i mod cap of a shared-memory ring of `cap` doubles (cap >= the widest row, checked by the caller),
  * updated IN PLACE.  Thread t owns the L consecutive cells lo_j + tL .. (L odd: the float64 accesses of a half-warp then fall
  * into 16 different bank pairs), adds them up, the block scans the 1024 partial sums (two shuffle scans, fixed order), and a
  * second pass writes the running sums.  The binomials a row needs -- its scale, its seed, and the cells the previous row had
  * outside the band -- are products of up to j factors; they are computed by GROUPS of G lanes (G = 1, 8 or 32 by j), each lane
  * a strided share of the factors, combined by a butterfly of multiplies on (mantissa, exponent) pairs: warp 0 the scale, warp 1
- * the seed, warps 2.. the cells, all at the same time.  ~1-2 us per row instead of ~20. */
+ * the seed, warps 2.. the cells, all at the same time. */
 /* frexp / ldexp for the values that occur here (positive, normal): two integer operations instead of the library routines */
 __device__ __forceinline__ double frexp_pos(double x, int &e) {
     int hi = __double2hiint(x);
@@ -656,8 +659,8 @@ __global__ void __launch_bounds__(B2F_DRIFT_THREADS) k_drift_finish(DriftParams 
     /* ---- (1) K-S numerator: max over reference points of |n*(#ref <= r) - m0*(#batch <= r)| and the left limits.
      *      Running counts over the m0 + 1 histogram bins: warp w owns a contiguous segment, lanes read consecutive bins
      *      (coalesced), pass 1 adds the segment up, one barrier, pass 2 walks it again 32 bins at a time with shuffle scans.
-     *      (Round 1 gave each THREAD a contiguous run of 30 bins: every load of a warp touched 32 different lines, and the
-     *      1024 partial sums were scanned by one thread -- most of the 0.11 ms a single-row request took.) */
+     *      (Giving each THREAD a contiguous run of 30 bins instead makes every load of a warp touch 32 different lines, and
+     *      leaves the 1024 partial sums to be scanned by one thread.) */
     const int64_t m0 = p.n_ref, n0 = p.n;
     const uint32_t *ha = p.hist_a + (int64_t)f * (m0 + 1);
     const uint32_t *hb = p.hist_b + (int64_t)f * (m0 + 1);

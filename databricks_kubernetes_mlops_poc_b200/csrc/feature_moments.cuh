@@ -1,5 +1,5 @@
 /*
- * feature_moments.cuh -- K2: per-feature (count, mean, M2) over N encoded rows, sm_100a.
+ * feature_moments.cuh -- K2: per-feature (count, mean, M2) over N encoded rows, sm_90a.
  *
  * BASELINE config 5 ("drift-monitor path: per-feature mean/var reduction").  The reference has no
  * mean/var computation; the nearest call on its path is `self.drift.predict(df[all].values)`
@@ -13,10 +13,10 @@
  * (float32, NaN = missing) is WARP-UNIFORM and compiled in (consume_slabs<NC>): no per-word type select,
  * no NaN test on integer words, and the missing-value case is a predicate on the three accumulations
  * instead of selects.  (Round 1 gave thread t vector t mod 6: every word went through both conversions
- * and a select chain, 83 instructions per vector, issue-bound at 0.53 of the HBM roofline.)
+ * and a select chain, 83 instructions per vector: issue-bound, not memory-bound.)
  * Memory-level parallelism comes from the ring (3 CTAs x 3 stages x 24 KB = 216 KB in flight per SM),
  * not from registers: a first version that relied on unrolled LDG.128 got one or two loads in flight
- * per warp from ptxas and stalled on the long scoreboard at 2.7 TB/s.
+ * per warp from ptxas and stalled on the long scoreboard.
  * Arithmetic: shifted float64 sums sum(x-K), sum((x-K)^2) and an integer count per word (K = the word's
  * value in row 0; the shift removes the cancellation of the raw sum-of-squares form).  Block partials are
  * reduced through shared memory in a fixed order, written to global memory, and the last block to finish

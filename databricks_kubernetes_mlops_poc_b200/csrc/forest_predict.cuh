@@ -1,6 +1,6 @@
 /*
  * forest_predict.cuh -- K1: fused impute -> one-hot-as-equality -> tree walk -> aggregate kernel
- * for sm_100a.  No tensor cores: the path is a branchy pointer walk, not a contraction.
+ * for sm_90a.  No tensor cores: the path is a branchy pointer walk, not a contraction.
  *
  * Replaces, on the GPU, what `classifier.predict_proba(df[all_features])[:, 1]` computes on the CPU
  * (reference databricks/src/02-register-model.ipynb:335-337; pipeline definition

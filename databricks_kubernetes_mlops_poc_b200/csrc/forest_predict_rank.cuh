@@ -1,21 +1,21 @@
 /*
- * forest_predict_rank.cuh -- K1c: the rank-quantised form of the fused scoring kernel (sm_100a), for forests that stay
+ * forest_predict_rank.cuh -- K1c: the rank-quantised form of the fused scoring kernel (sm_90a), for forests that stay
  * resident in shared memory.  Same arithmetic as k_forest_predict / k_forest_predict_tile -- it replaces
  * `classifier.predict_proba(df[all_features])[:, 1]` (reference databricks/src/02-register-model.ipynb:335-337) -- on rows in
  * the B2F_ROWS_RANKED format (forest_rank.h): every numeric feature arrives as its rank among the forest's split values and
  * every tested (categorical feature, category) pair becomes a 0/1 value, so EVERY split is one unsigned integer compare
  * "value[f] >= t" and a node is ONE 32-bit word (t << 16 | byte offset of value[f] in the tile's value block).
  *
- * Why (round-1 ncu, profiles/r01_ncu_tile.txt): the walk is bound by shared-memory wavefronts (LSU pipe, 1 per clock per SM).
+ * Why: the tile kernel's walk is bound by shared-memory wavefronts (LSU pipe, 1 per clock per SM).
  * An 8-byte node costs two wavefronts per warp-level visit (LDS.64 is served half-warp by half-warp) plus a leaf-id load; here
  *   - a node is 4 bytes: one wavefront, and at most 32 consecutive words per level up to depth 5 -> never a bank conflict;
  *   - trees are COMPLETE in breadth-first order: child = 2i+1(+1), no child pointer, no leaf-id load -- after D levels the
  *     path bits ARE the leaf index;
  *   - per warp-level visit: LDS node, LOP3 (value address), LDS.U16 value, IMAD (value << 16 | 0xFFFF), ISETP, SEL, IMAD
  *     (child address): 3 ops on the integer ALU pipe, 2 on the FMA pipe.  (The first version tested categorical nodes by
- *     equality next to the numeric >=: 6 ALU-pipe ops per visit, and ncu showed that pipe -- one warp instruction per two
- *     cycles per scheduler -- at 77 %, i.e. the bound; profiles/r02_ncu_rank_v1.txt.)
- * and the machine is filled differently from the tile kernel (which left 60 % of its warps without a tile at 65 536 rows):
+ *     equality next to the numeric >=: 6 ALU-pipe ops per visit, which made that pipe -- one warp instruction per two
+ *     cycles per scheduler -- the bound.)
+ * and the machine is filled differently from the tile kernel (which leaves most of its warps without a tile at 65 536 rows):
  *   - one CTA per SM, 32 warps, ALL of them walk; the CTA owns a contiguous run of 32-row tiles (<= 16 per round);
  *   - phase 1  all 1024 threads stage the CTA's rows into the per-tile value block xs[tile][f >> 1][lane][f & 1] (16-bit values,
  *              TRANSPOSED: lane l's values sit in bank l, so the per-lane dynamic fetch of the walk is one conflict-free

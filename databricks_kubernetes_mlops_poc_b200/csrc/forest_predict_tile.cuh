@@ -1,5 +1,5 @@
 /*
- * forest_predict_tile.cuh -- K1b: the large-batch form of the fused scoring kernel (sm_100a).
+ * forest_predict_tile.cuh -- K1b: the large-batch form of the fused scoring kernel (sm_90a).
  *
  * Same arithmetic as k_forest_predict (forest_predict.cuh) -- it replaces
  * `classifier.predict_proba(df[all_features])[:, 1]` (reference databricks/src/02-register-model.ipynb:335-337)

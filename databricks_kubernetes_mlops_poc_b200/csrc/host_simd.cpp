@@ -14,7 +14,7 @@
  *   c_j = #{chunk maxima <= x} is the digit of the rank in the mixed radix, and selects the chunk to descend into.
  *   m <= 63: one level; m <= 1023: two (16 x up to 64: 4 KB per feature, so 14 features stay in L1); m <= 16383: three.
  *
- * AVX-512F path when the CPU has it (the B200 hosts do), else an AVX2 form of the same walk (2 x 8 lanes), else scalar.
+ * AVX-512F path when the CPU has it, else an AVX2 form of the same walk (2 x 8 lanes), else scalar.
  */
 #include <immintrin.h>
 #include <math.h>

@@ -6,7 +6,8 @@
  * Reference counterpart: `self.classifier.predict_proba(...)[:, 1].tolist()` (databricks/src/02-register-model.ipynb:335-337):
  * the model object must hand plain Python lists to the handler (they are json.dumps'ed and re-validated, app/main.py:75-86).
  * At 65 536 rows that `.tolist()` -- one PyFloat allocation per element now, one free per element when the previous response
- * is dropped -- costs more than encoding, copying and scoring the whole batch on the GPU (0.56 ms vs 0.15 ms), so the floats
+ * is dropped -- costs more than encoding, copying and scoring the whole batch (0.71 ms for the .tolist() alone against
+ * 0.70 ms for a whole recycled-float predict() call, on the host of an H100 80GB HBM3 at 400 W), so the floats
  * are recycled: the module keeps a ring of float objects it owns one reference to; an object whose reference count is back
  * to 1 (nobody but the ring holds it: the response it was part of is gone) gets its value overwritten and goes into the
  * next list.  That is what CPython's own float free list does, at a larger scale; an object something else still

@@ -76,8 +76,8 @@ static void bind_thread_near(int device) {
 
 /* CPUs this process may actually burn: the cgroup's CFS bandwidth (v2 cpu.max "quota period", v1 cpu.cfs_quota_us /
  * cpu.cfs_period_us) next to its affinity mask.  A pool of polling workers larger than the quota gets the WHOLE cgroup
- * throttled for the rest of the 100 ms period -- measured on the GPU boxes (cpu.max = 1600000 100000 on a 128-CPU host): with 48
- * workers 2 % of the 65 536-row requests took 55-75 ms instead of 0.6 (profiles/r02_e2e_stalls.json).  0 = no limit found. */
+ * throttled for the rest of the 100 ms period, and the request that was running waits for it (tools/e2e_stalls.py shows it).
+ * 0 = no limit found. */
 static double cgroup_cpu_limit() {
     double best = 0.0;
     if (FILE *f = fopen("/sys/fs/cgroup/cpu.max", "r")) {
@@ -102,8 +102,8 @@ static double cgroup_cpu_limit() {
 }
 
 /* worker threads a scorer may start by default: the GPU's NUMA node (its cores and half of their hyper-threads), capped at 48
- * and at the cgroup's CPU bandwidth minus two (the caller's thread builds the response while the workers encode; with a quota of 16:
- * 0.45 ms per 65 536-row request with 14 workers, 0.51 with 12 or 10, and 55-75 ms stalls from 17 up) */
+ * and at the cgroup's CPU bandwidth minus two (the caller's thread builds the response while the workers encode; more polling
+ * workers than the quota allows get the whole cgroup throttled, and the request in flight stalls for the rest of the period) */
 static int default_host_threads(int device) {
     cpu_set_t set;
     int local = numa_cpus_of_device(device, &set) ? CPU_COUNT(&set) : (int)std::thread::hardware_concurrency();
@@ -171,8 +171,8 @@ extern "C" void *b2f_pinned_alloc_near(int device, size_t nbytes) { return pinne
 /* One buffer for a stream that is dealt round-robin over several GPUs (b2f_predict_stream): stripe s = bytes
  * [s * stripe_bytes, (s + 1) * stripe_bytes) is the part GPU (s mod n) will copy, so its pages are first-touched from a thread
  * bound to THAT GPU's NUMA node, and only then is the whole range page-locked (cudaHostRegister keeps pages where they are).
- * A single cudaHostAlloc puts everything on the allocating thread's node and half of an 8-GPU box then copies across the
- * socket interconnect (round 1: 2.4 G rows/s on 8 GPUs from one process against 3.8 G from eight processes). */
+ * A single cudaHostAlloc puts everything on the allocating thread's node, and the GPUs of the other socket then copy across the
+ * socket interconnect. */
 #include <sys/mman.h>
 #include <map>
 static std::mutex g_striped_mu;
@@ -341,7 +341,7 @@ static void scorer_worker(b2f_scorer *s, int idx) {
     uint64_t seen = 0;
     for (;;) {
         /* spin for the next job for a while (a service under load gets the next request within a millisecond; waking 30
-         * sleeping threads through a condition variable costs ~100 us of the request that does it), then sleep */
+         * sleeping threads through a condition variable delays the request that does it), then sleep */
         uint64_t g = s->generation.load(std::memory_order_acquire);
         if (g == seen) {
             const auto until = std::chrono::steady_clock::now() + std::chrono::microseconds(s->spin_us);
@@ -447,7 +447,7 @@ extern "C" int b2f_scorer_start(b2f_scorer *s, int64_t n, const b2f_str_column *
         chunk_rows = n <= 8192 ? n : std::max<int64_t>(4096, ((n + 7) / 8 + 255) / 256 * 256);
         /* a forest that STREAMS through shared memory (500 trees x depth 8) makes the GPU the bound of a big request, and its
          * tile kernel -- one pass over the forest per launch -- wants >= 24 576 rows per launch: two chunks instead of eight
-         * (65 536 rows, GBDT 500 x d8: 0.48 ms instead of 0.67; resident forests: eight chunks are best, 0.28 vs 0.32 with four) */
+         * (resident forests keep eight: each pass over the forest is cheap, so overlap of copies and kernels wins) */
         const bool streamed = s->m->tile_ok && s->m->tp.n_pieces > s->m->tp.n_slots;
         if (streamed && row_format != B2F_ROWS_RANKED && n >= 2 * s->m->tile_min_rows)
             chunk_rows = std::max<int64_t>(s->m->tile_min_rows, ((n + 1) / 2 + 255) / 256 * 256);
@@ -459,8 +459,9 @@ extern "C" int b2f_scorer_start(b2f_scorer *s, int64_t n, const b2f_str_column *
     }
     /* chunk boundaries: equal chunks.  B200_FIRST_CHUNK_ROWS=<r> makes the first chunk of a library-chunked request r rows
      * (the caller turns results into Python objects more slowly than the pool encodes, so the request ends one list-building
-     * time after the FIRST chunk is back); measured on B200 it does not pay -- a 1 024- or 2 048-row first chunk comes back
-     * no earlier than an 8 192-row one (157 / ~100 us vs 96 us after the start of the request) -- so it is off by default */
+     * time after the FIRST chunk is back).  A small first chunk pays only when its launch and copies cost less than
+     * encoding the rows it saves, which is not the case for the default 8 192-row chunks -- so it is off by default (a choice
+     * kept from the previous GPU generation, not re-measured on the H100) */
     static const int64_t first_rows = getenv("B200_FIRST_CHUNK_ROWS") ? atoll(getenv("B200_FIRST_CHUNK_ROWS")) : 0;
     if (auto_chunks && n_chunks >= 4 && first_rows >= 256 && first_rows * 4 <= chunk_rows * 2) {
         const int64_t rest = n - first_rows, each = ((rest + (n_chunks - 2)) / (n_chunks - 1) + 255) / 256 * 256;

@@ -66,7 +66,7 @@ class TabularDrift:
     def _open(self, device: int, handles: int | None = None) -> None:
         """Upload the reference table.  ``handles`` (default ``B200_DRIFT_HANDLES`` or 4) independent device states,
         each with its own stream and scratch, let that many requests be scored concurrently: one request occupies
-        one CTA per feature (23 of the 148 SMs), and the server scores every request's drift on its own thread."""
+        one CTA per feature (23 of the 132 SMs), and the server scores every request's drift on its own thread."""
         import os
 
         self._lib = _cabi.load_library()

@@ -41,7 +41,7 @@ _F32_MAX = float(np.finfo(np.float32).max)
 
 def column_positions(df: pd.DataFrame, names, cache: dict):
     """Positions of ``names`` in ``df.columns`` (-1: absent), cached per column Index object (building an Index from a
-    list of names costs ~0.1 ms, more than a small request's whole device time)."""
+    list of names costs more than a small request's whole device time)."""
     cols = df.columns
     hit = cache.get(id(cols))
     if hit is None or hit[0] is not cols:
@@ -215,7 +215,7 @@ class RowEncoder:
         -> (StrColumn array, float64 pointer array, strides, keep-alive list), or None when a column does not have the
         expected physical type (object-dtype strings, non-numeric numerics ...: the portable path handles those).
         Column lookup goes through the block manager (one ``get_indexer`` per distinct column index, then an array fetch per
-        column) -- ``df[name]`` builds a Series per column, which alone costs ~0.3 ms for 23 columns."""
+        column) -- ``df[name]`` builds a Series per column, which for 23 columns costs more than encoding a small request."""
         if self._native_handle() is None:
             return None
         cols = df.columns
@@ -401,8 +401,8 @@ class RowEncoder:
             raise KeyError(f"{missing} not in index")  # what df[self.all_features] raises
         as_i32 = out.view(np.int32)
         if n <= self.SMALL_BATCH:
-            # small request: ONE object-array extraction of the whole frame (column selection alone costs
-            # pandas ~0.5 ms), then dictionary lookups / float() in Python
+            # small request: ONE object-array extraction of the whole frame (pandas column selection alone costs
+            # more than the rest of a small request), then dictionary lookups / float() in Python
             key = tuple(cols)
             pos = self._colpos.get(key)
             if pos is None:

@@ -1,4 +1,4 @@
-"""ForestEngine: one flattened forest resident on one B200, driven through the C ABI.
+"""ForestEngine: one flattened forest resident on one H100, driven through the C ABI.
 
 Python-side owner of a ``b2f_model*`` (``include/b2f.h``).  It replaces the object the
 reference keeps in ``self.classifier`` (``databricks/src/02-register-model.ipynb:318-322``) for the
@@ -268,11 +268,10 @@ class Scorer:
         h_enc = encoder._native_handle()
         if h_enc is None:
             raise B2FError("the native row encoder is not available")
-        # Which rows the workers write.  The host is the bound of this path (a B200 box gives the container 16 CPUs; the GPU needs
-        # ~20 us per 65 536 rows either way), so the format is chosen by HOST cost: the 64-byte float32 rows cost 2-3 ms of one
-        # core per 65 536 rows, the 32-byte ranked rows ~2 ms more (14 rank lookups per row) -- measured 0.57 ms vs 0.78 ms per
-        # 65 536-row request (profiles/r02_e2e_stalls.json).  Ranked rows are for callers that stream PRE-ENCODED rows through the
-        # C ABI, where PCIe bytes are the bound; B200_SCORER_ROWS=ranked selects them here too.
+        # Which rows the workers write.  The host is the bound of this path (a container gets a few CPUs; the GPU scores a
+        # 65 536-row chunk in far less time than they take to encode it), so the format is chosen by HOST cost: the 32-byte
+        # ranked rows need 14 rank lookups per row on top of what the 64-byte float32 rows cost.  Ranked rows are for callers that
+        # stream PRE-ENCODED rows through the C ABI, where PCIe bytes are the bound; B200_SCORER_ROWS=ranked selects them here too.
         self.fmt = self.fmt_small = ROWS_PACKED64 if encoder.packed_ok else ROWS_WORDS24
         self.rank_min_rows = 0
         info = engine.info()

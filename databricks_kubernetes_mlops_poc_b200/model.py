@@ -204,7 +204,8 @@ class B200Model:
         if len(df.columns) == 0:
             # the reference dies in df[self.all_features] on an empty request (-> HTTP 500)
             raise KeyError(f"None of {self.all_features} are in the [columns]")
-        # the drift sweep is ~2 ms of device time on its own stream: start it first, score the rows meanwhile
+        # the drift sweep takes milliseconds of device time on its own stream (2.2 ms for 1 000 rows on an H100): start it
+        # first, score the rows meanwhile
         pending = self._pool.submit(self.drift.score, df) if self.drift is not None else None
         n = len(df)
         try:

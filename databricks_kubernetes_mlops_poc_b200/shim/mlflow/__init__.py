@@ -6,7 +6,7 @@ The reference's ``app/main.py`` imports ``mlflow`` and makes exactly one call in
 
     PYTHONPATH=<repo>/databricks_kubernetes_mlops_poc_b200/shim uvicorn app.main:app --port 5000
 
-runs the reference's UNMODIFIED ``app/main.py`` on the B200 engine (SURVEY.md section 8f rank 4).  It is opt-in by path:
+runs the reference's UNMODIFIED ``app/main.py`` on the H100 engine (SURVEY.md section 8f rank 4).  It is opt-in by path:
 nothing in the package imports it, and a real mlflow installation is shadowed only for that process.
 """
 

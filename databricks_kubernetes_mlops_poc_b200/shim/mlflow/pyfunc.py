@@ -1,4 +1,4 @@
-"""``mlflow.pyfunc.load_model`` -> the B200 model (reference ``app/main.py:26-28``)."""
+"""``mlflow.pyfunc.load_model`` -> the H100 model, ``B200Model`` (reference ``app/main.py:26-28``)."""
 
 from __future__ import annotations
 

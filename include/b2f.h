@@ -1,5 +1,5 @@
 /*
- * b2f.h -- C ABI of libb200forest.so, the B200-native scoring engine behind the
+ * b2f.h -- C ABI of libb200forest.so, the H100-native scoring engine behind the
  * credit-default service's `model.predict()`.
  *
  * The reference has no native code and therefore no FFI of its own: its hot path is the

@@ -33,7 +33,7 @@ file).  The pins we build instead:
   (``tests/test_drift_cpu.py``).  alibi-detect itself is neither vendored nor installed: against it the drift path
   is "parity unpinned".  The outlier detector's oracle is sklearn's ``IsolationForest`` itself.
 * ``tests/golden/make_golden.py`` freezes inputs + library outputs into
-  ``tests/golden/*.npz`` so the GPU box (which has no ``/root/reference``) can
+  ``tests/golden/*.npz`` so a machine without a reference checkout can
   re-fit, verify the re-fit reproduces the frozen outputs, and then check the
   CUDA path against them.
 """

@@ -3,8 +3,8 @@
 ``tests/golden/curated.npz`` / ``inference.npz`` are lossless dictionary-encoded
 copies of the reference's ``databricks/data/curated.csv`` (30 000 labelled rows)
 and ``databricks/data/inference.csv`` (80 rows, different column order), written
-by ``tests/golden/make_golden.py``.  They exist because ``/root/reference`` is not
-present on the GPU box.
+by ``tests/golden/make_golden.py``.  They exist so that the tests need no checkout of
+the reference.
 """
 
 from __future__ import annotations

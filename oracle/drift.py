@@ -5,7 +5,7 @@ on a detector built as ``TabularDrift(x_ref, p_val=0.05, categories_per_feature=
 response carries ``(1 - p_val).tolist()`` (``:345-349``).
 
 The arithmetic lives in two un-vendored packages (SURVEY 8c): alibi-detect==0.12.0 (``app/requirements.txt:6``;
-NOT installed here, NOT under /root/reference) and scipy (installed; it holds the numerics).  What alibi-detect
+NOT installed, NOT in the reference checkout) and scipy (installed; it holds the numerics).  What alibi-detect
 0.12.0's ``TabularDrift.feature_score`` does, restated from the published source:
 
 * categorical feature f: the category set is the UNION of the values seen in the reference column and in the

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate the golden fixtures under tests/golden/ (run in the authoring container only).
 
-The reference (``/root/reference``) does not exist on the GPU box, and it ships no
+The reference checkout is not part of this repository, and it ships no
 golden vectors of its own (SURVEY.md section 4).  This script
 
 1. reads the reference's own data fixtures
@@ -14,7 +14,7 @@ golden vectors of its own (SURVEY.md section 4).  This script
    all 30 000 + 80 rows into ``expected_<model>.npz`` together with the sklearn version;
 3. checks the numpy and C restatements against the library before writing anything.
 
-Usage:  python tests/golden/make_golden.py [--reference /root/reference]
+Usage:  python tests/golden/make_golden.py --reference <checkout of nfmoore/databricks-kubernetes-mlops-poc>
 """
 
 from __future__ import annotations
@@ -47,7 +47,7 @@ def freeze_frame(df: pd.DataFrame, with_target: bool) -> dict:
 
 def main() -> None:
     ap = argparse.ArgumentParser()
-    ap.add_argument("--reference", default="/root/reference")
+    ap.add_argument("--reference", required=True, help="checkout of nfmoore/databricks-kubernetes-mlops-poc")
     args = ap.parse_args()
 
     cur_csv = pd.read_csv(os.path.join(args.reference, "databricks/data/curated.csv"))

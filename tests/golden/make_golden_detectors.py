@@ -10,7 +10,7 @@ frozen are the outputs of the libraries that hold the arithmetic, computed on th
 * drift detector (``:224-229,338``): per-feature statistic and float64 p-value of ``oracle.drift`` (scipy
   ``chi2_contingency`` / ``ks_2samp(method="exact")``) for three batches against the 30 000 curated rows.
 
-Usage:  python tests/golden/make_golden_detectors.py      (needs no /root/reference)
+Usage:  python tests/golden/make_golden_detectors.py      (needs no reference checkout)
 """
 
 from __future__ import annotations

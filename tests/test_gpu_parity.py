@@ -130,7 +130,7 @@ def test_batch_size_edges(curated, rf100d6):
     try:
         want_p, want_l = rp.oracle_predict(rf100d6, curated)
         rows = enc.encode_frame(curated)
-        for n in (0, 1, 2, 31, 32, 33, 147, 148 * 32 + 1, 16384, 24576, 24577, 30000):
+        for n in (0, 1, 2, 31, 32, 33, 131, 132 * 32 + 1, 147, 148 * 32 + 1, 16384, 24576, 24577, 30000):
             p, l = eng.predict_rows(rows[:n], np.float64)
             assert p.shape == (n,) and l.shape == (n,)
             if n:

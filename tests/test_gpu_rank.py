@@ -48,8 +48,8 @@ def test_rank_kernel_batch_size_edges_and_determinism(curated, rf100d6):
     try:
         want_p, want_l = rp.oracle_predict(rf100d6, curated)
         rk = enc.rank_rows(enc.encode_frame(curated))
-        # 1 .. 33: fewer tree groups than warps; 148*32+1: one tile more than CTAs; 16*32*148+1: a second round per CTA
-        for n in (0, 1, 2, 31, 32, 33, 147, 148 * 32 + 1, 4737, 16384, 30000):
+        # 1 .. 33: fewer tree groups than warps; 132*32+1: one tile more than CTAs on an H100 (132 SMs); 90 000 below: a second round per CTA
+        for n in (0, 1, 2, 31, 32, 33, 131, 132 * 32 + 1, 147, 4737, 16384, 30000):
             p, l = eng.predict_rows(rk[:n], np.float64)
             assert p.shape == (n,)
             if n:

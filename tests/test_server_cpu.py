@@ -105,42 +105,51 @@ def test_concurrent_requests_share_batches():
     assert sum(m.calls) == 120 and len(m.calls) < 40  # requests were merged into fewer engine calls
 
 
-REFERENCE_APP = "/root/reference/app"
-
-
-@pytest.mark.skipif(not __import__("os").path.exists(REFERENCE_APP + "/main.py"), reason="reference checkout not present (GPU box)")
-def test_unmodified_reference_app_runs_on_the_shim(monkeypatch):
-    """SURVEY 8f rank 4: the reference's own app/main.py, imported unmodified from /root/reference with the mlflow shim
-    ahead on the path, serves POST /predict from whatever `load_model` returns (a stub scorer here: no GPU)."""
+def test_http_responses_match_the_reference_app(monkeypatch):
+    """SURVEY 8f rank 4: the reference's own app/main.py, run unmodified on the mlflow shim with a stub plugin, answered the
+    bodies in tests/golden/reference_app.json (make_golden_reference_app.py).  This package's app, loading its model through
+    the same shim (`mlflow.pyfunc.load_model` -> `load_model`) and scoring with the same stub, gives the same status codes,
+    the same response bodies (keys in the same order) and publishes the same request schema."""
     import importlib
     import os
     import sys
+    from types import SimpleNamespace
 
     import databricks_kubernetes_mlops_poc_b200 as pkg
-    from databricks_kubernetes_mlops_poc_b200.schema import ALL_FEATURES, sample_request
+    from databricks_kubernetes_mlops_poc_b200.schema import ALL_FEATURES
+    from databricks_kubernetes_mlops_poc_b200.server import create_app
 
-    class Plugin:  # the plugin boundary: predict(DataFrame) -> dict (CustomModel.predict)
-        def predict(self, df):
-            if len(df.columns) == 0:
-                raise KeyError("no columns")  # what B200Model.predict (and the reference's CustomModel) do on []
-            n = len(df)
-            return {"predictions": [0.25] * n, "outliers": [0] * n, "feature_drift_batch": {k: 0.0 for k in ALL_FEATURES}}
+    with open(os.path.join(os.path.dirname(__file__), "golden", "reference_app.json")) as f:
+        golden = json.load(f)
 
-    monkeypatch.syspath_prepend(REFERENCE_APP)
+    class Stub(StubModel):  # the stub plugin of make_golden_reference_app.py, behind this package's scorer interface
+        def score(self, df):
+            x = df["credit_limit"].to_numpy(dtype=float)
+            return (x % 1000) / 1000.0, (x > 5000).astype(np.int32)
+
+    model = Stub()
+    model.drift = SimpleNamespace(score=lambda df: [i / 100.0 for i in range(len(ALL_FEATURES))])
     monkeypatch.syspath_prepend(os.path.join(os.path.dirname(pkg.__file__), "shim"))
-    for name in [m for m in sys.modules if m in ("mlflow", "main", "model") or m.startswith("mlflow.")]:
+    for name in [m for m in sys.modules if m == "mlflow" or m.startswith("mlflow.")]:
         monkeypatch.delitem(sys.modules, name)
-    monkeypatch.setattr(pkg, "load_model", lambda path: Plugin())
-    main = importlib.import_module("main")
+    mlflow = importlib.import_module("mlflow")
+    monkeypatch.setattr(pkg, "load_model", lambda path: model)
     try:
-        assert main.__file__.startswith(REFERENCE_APP)
-        with TestClient(main.app, raise_server_exceptions=False) as c:
-            r = c.post("/predict", json=sample_request())
-            assert r.status_code == 200 and r.json()["predictions"] == [0.25]
-            assert list(r.json()["feature_drift_batch"]) == ALL_FEATURES
-            assert c.post("/predict", json=[]).status_code == 500
+        with TestClient(create_app(loader=mlflow.pyfunc.load_model), raise_server_exceptions=False) as c:
+            for name, body in golden["bodies"].items():
+                want = golden["responses"][name]
+                r = c.post("/predict", json=body)
+                assert r.status_code == want["status"], name
+                if want["status"] == 200:
+                    got = r.json()
+                    assert got == want["json"], name
+                    assert list(got) == list(want["json"]) and list(got["feature_drift_batch"]) == list(want["json"]["feature_drift_batch"]), name
+            spec = c.get("/openapi.json").json()
+        props = spec["paths"]["/predict"]["post"]["requestBody"]["content"]["application/json"]["schema"]["items"]["properties"]
+        assert {k: {"type": v.get("type"), "default": v.get("default")} for k, v in props.items()} == golden["request_schema_properties"]
+        assert list(props) == list(golden["request_schema_properties"])
     finally:
-        for name in [m for m in sys.modules if m in ("mlflow", "main", "model") or m.startswith("mlflow.")]:
+        for name in [m for m in sys.modules if m == "mlflow" or m.startswith("mlflow.")]:
             sys.modules.pop(name, None)
 
 
