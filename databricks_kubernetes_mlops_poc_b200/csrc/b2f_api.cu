@@ -159,6 +159,7 @@ struct b2f_model {
     int rank_smem_bytes = 0;
     int rank_u = 4;
     bool rank_stream = false; /* the rank layout streams through shared memory in pieces (too large to stay resident) */
+    bool rank_pdl = true;     /* launch the rank kernel with programmatic stream serialization (B2F_NO_PDL at model creation: off) */
     int64_t launches_rank = 0;
     void *d_blob = nullptr;
     int64_t forest_bytes = 0;
@@ -509,6 +510,8 @@ static int rank_init(b2f_model *m, const uint8_t *blob) {
     rp.mul_64k = 65536u;
     rp.add_64k = 65535u;
     rp.n_pairs = (int)m->rk.pairs.size();
+    if (const char *wf = getenv("B2F_RANK_WAIT_FIRST")) rp.wait_first = atoi(wf) != 0; /* A/B: the dependency wait back at kernel entry */
+    m->rank_pdl = getenv("B2F_NO_PDL") == nullptr;
     for (int j = 0; j < 16; ++j) {
         rp.cat_shift[j] = (uint8_t)m->rk.cat_shift[j];
         rp.cat_bits[j] = (uint8_t)m->rk.cat_bits[j];
@@ -846,8 +849,23 @@ static cudaError_t launch_split(const b2f_model *m, cudaStream_t st, const void 
     return cudaGetLastError();
 }
 
-/* the rank kernel goes out with programmatic stream serialization: back-to-back launches on one stream overlap the
- * next launch's prologue (forest fill) with this launch's tail; the kernel orders its own global accesses with griddepcontrol.wait */
+#ifdef B2F_RANK_PHASES
+/* diagnostic build: every rank launch takes the next record of the buffer armed by b2f_rank_phases_arm (tools/rank_phases.py) */
+static int32_t g_rank_phase_next = 0;
+extern "C" int b2f_rank_phases_arm(b2f_model *m, void *dev_buf, int launches) {
+    if (!m || !m->rank_ok) return set_err(B2F_EINVAL, "no rank kernel on this model");
+    m->rp.phases = static_cast<unsigned long long *>(dev_buf);
+    m->rp.phase_launches = dev_buf ? launches : 0;
+    g_rank_phase_next = 0;
+    return B2F_OK;
+}
+#endif
+
+/* The rank kernel goes out with programmatic stream serialization, which relaxes the edge from one such launch to the next
+ * on the same stream only: a CTA of launch N + 1 may start as soon as a CTA of launch N retires, and the kernel reads its rows
+ * and walks before griddepcontrol.wait.  That is safe because no rank launch writes rows, and everything else that can
+ * write them (H2D copies, every other kernel of this library or of the caller) is an ordinary stream predecessor of the
+ * first relaxed launch of a chain.  The stores of launch N + 1 follow its wait, so the last launch writing a buffer wins. */
 template <int D, int U, bool ST, typename OutT>
 static cudaError_t launch_rank_du(const b2f_model *m, cudaStream_t st, const void *rows, int64_t n, void *proba, int32_t *label, int ostride) {
     const int64_t n_tiles = (n + 31) / 32;
@@ -859,10 +877,15 @@ static cudaError_t launch_rank_du(const b2f_model *m, cudaStream_t st, const voi
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    static const bool no_pdl = getenv("B2F_NO_PDL") != nullptr;
     cfg.attrs = attr;
-    cfg.numAttrs = no_pdl ? 0 : 1;
-    return cudaLaunchKernelEx(&cfg, k_forest_predict_rank<D, U, ST, OutT>, m->rp, static_cast<const uint8_t *>(rows), (long long)n,
+    cfg.numAttrs = m->rank_pdl ? 1 : 0;
+#ifdef B2F_RANK_PHASES
+    RParams rp = m->rp;
+    rp.phase_launch = g_rank_phase_next++;
+#else
+    const RParams &rp = m->rp;
+#endif
+    return cudaLaunchKernelEx(&cfg, k_forest_predict_rank<D, U, ST, OutT>, rp, static_cast<const uint8_t *>(rows), (long long)n,
                               static_cast<OutT *>(proba), label, ostride);
 }
 template <typename OutT>

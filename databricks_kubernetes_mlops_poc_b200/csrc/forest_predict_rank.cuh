@@ -30,9 +30,18 @@
  *     8 trees (2 tree groups) that travel through a two-slot ring -- thread 0 issues the TMA copy of piece k + 2 right after the
  *     barrier that ends piece k, so the copy overlaps the walk of piece k + 1 -- and warp w owns (tile w / 2, group w mod 2) of
  *     EVERY piece: its float64 sum stays in a register across the whole forest (<= 16 tiles per round).
- *   - launched with programmatic stream serialization (PDL): `griddepcontrol.launch_dependents` is issued at entry so the next
- *     launch's CTAs take over SMs as this launch's CTAs retire (its forest fill and row staging overlap this launch's tail);
- *     `griddepcontrol.wait` sits before the first global access that could depend on the previous kernel.
+ *   - launched with programmatic stream serialization (PDL): `griddepcontrol.launch_dependents` is issued at entry, so a CTA
+ *     of the next launch takes an SM as soon as a CTA of this one leaves it, and does all of its work there -- forest fill,
+ *     row staging and the whole walk -- before `griddepcontrol.wait`, which sits just before the first global store of round 0.
+ *     Ordering contract (why the reads may precede the wait):
+ *       - the attribute relaxes only the edge from one programmatic launch of this kernel to the next on the same stream;
+ *         every operation that can write a launch's rows (an H2D copy, any other kernel) is an ordinary stream predecessor
+ *         and has finished before the first relaxed launch of a chain starts;
+ *       - this kernel never writes rows or the rank layout, so nothing inside a chain changes what a later launch reads;
+ *       - the one hazard is between outputs: two launches writing the same proba / label buffer, where the last one must
+ *         win.  Every store follows the wait, and the wait runs once in every CTA (the grid never exceeds the tile count,
+ *         so every CTA has a round 0): launch N completes only after launch N - 1 has, transitively down the chain.
+ *     RParams::wait_first (B2F_RANK_WAIT_FIRST=1) puts the wait back at entry, for A/B measurement.
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -69,14 +78,42 @@ struct RParams {
     uint32_t mul_64k;        /*   ptxas keeps the two multiply-adds of a node visit as IMAD (FMA pipe) instead of strength-reducing */
     uint32_t add_64k;        /*   them to LEA / IADD3 on the integer ALU pipe, which is the pipe that bounds the walk */
     int32_t n_pairs;         /* tested (categorical feature, category) pairs = pseudo-features even(n_num) .. + n_pairs - 1 */
+    int32_t wait_first;      /* 1: griddepcontrol.wait once the forest fill is issued, before the row staging, instead of before the stores */
     uint8_t cat_shift[16];   /* bit position / width of categorical field j inside the row's categorical block */
     uint8_t cat_bits[16];
     uint8_t cat_start[16];   /* pair index of feature j's first tested category (pairs are sorted by feature, then category) */
     unsigned long long cat_mask[16]; /* bit c set: category c of feature j is tested by some node */
+#ifdef B2F_RANK_PHASES
+    unsigned long long *phases; /* [launch][CTA][B2F_RANK_PHASE_SLOTS] */
+    int32_t phase_launch;       /* this launch's index; launches at or past phase_launches record nothing */
+    int32_t phase_launches;
+#endif
 };
 
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+#ifdef B2F_RANK_PHASES
+/* Diagnostic build only (tools/rank_phases.py compiles it with -DB2F_RANK_PHASES): thread 0 of every CTA records
+ * %globaltimer at B2F_RANK_ENTRY .. B2F_RANK_EXIT and the SM it ran on.  The default build compiles all of it out. */
+#define B2F_RANK_PHASE_SLOTS 8
+enum { B2F_RANK_ENTRY = 0, B2F_RANK_FOREST_READY, B2F_RANK_ROWS_STAGED, B2F_RANK_WALK_DONE, B2F_RANK_WAIT_RELEASED, B2F_RANK_EXIT, B2F_RANK_SMID };
+__device__ __forceinline__ void rank_phase(const RParams &p, int i) {
+    if (threadIdx.x != 0 || p.phases == nullptr || p.phase_launch >= p.phase_launches) return;
+    unsigned long long *q = p.phases + ((size_t)p.phase_launch * gridDim.x + blockIdx.x) * B2F_RANK_PHASE_SLOTS;
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    q[i] = t;
+    if (i == B2F_RANK_ENTRY) {
+        uint32_t sm;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+        q[B2F_RANK_SMID] = sm;
+    }
+}
+#define RANK_PHASE(i) rank_phase(p, B2F_RANK_##i)
+#else
+#define RANK_PHASE(i) ((void)0)
+#endif
 
 __device__ __forceinline__ uint32_t lds_u16(uint32_t a) {
     uint32_t v;
@@ -124,6 +161,7 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
     const int warp = tid >> 5;
 
     pdl_launch_dependents(); /* the next launch may start filling SMs as this one's CTAs retire */
+    RANK_PHASE(ENTRY);
 
     /* shared-memory plan: [xs: max_tiles x 8 KB value blocks, 8 KB aligned][partials][forest | two-slot piece ring] */
     const uint32_t pad = (B2F_RANK_XS_BYTES - (smem_addr(smem) & (B2F_RANK_XS_BYTES - 1u))) & (B2F_RANK_XS_BYTES - 1u);
@@ -137,7 +175,6 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
         fence_mbar_init();
         fence_proxy_async();
         if constexpr (!STREAM) {
-            /* the forest is launch-invariant (never written by a kernel): safe to fetch before griddepcontrol.wait */
             mbar_arrive_expect_tx(&forest_bar[0], p.layout_bytes);
             for (uint32_t o = 0; o < p.layout_bytes; o += B2F_BULK_PIECE) {
                 const uint32_t part = min(B2F_BULK_PIECE, p.layout_bytes - o);
@@ -162,7 +199,14 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
     const uint32_t xs_addr = smem_addr(xs_all);
     bool forest_ready = false;
 
-    pdl_wait(); /* rows may have been produced by the previous kernel in the stream; outputs may still be read by it */
+    /* griddepcontrol.wait, once per CTA: the previous launch of the chain (and so every earlier one) has completed and its
+     * stores are visible before this CTA's first store; see the ordering contract at the top of this file */
+    const bool wait_first = p.wait_first != 0;
+    auto wait_previous = [&]() {
+        pdl_wait();
+        RANK_PHASE(WAIT_RELEASED);
+    };
+    if (wait_first) wait_previous();
 
     for (uint32_t round = 0; round < n_rounds; ++round) {
         const uint32_t rt0 = cta_tiles * round / n_rounds, rt1 = cta_tiles * (round + 1u) / n_rounds;
@@ -215,10 +259,12 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
             }
         }
         __syncthreads();
+        RANK_PHASE(ROWS_STAGED);
         if constexpr (!STREAM) {
             if (!forest_ready) {
                 mbar_wait(&forest_bar[0], 0);
                 forest_ready = true;
+                RANK_PHASE(FOREST_READY);
             }
         }
 
@@ -232,12 +278,15 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
             for (int piece = 0; piece < p.n_pieces; ++piece) {
                 const uint32_t k = round * (uint32_t)p.n_pieces + (uint32_t)piece;
                 mbar_wait(&forest_bar[k & 1u], (k >> 1) & 1u);
+                if (k == 0) RANK_PHASE(FOREST_READY);
                 if (mine) rank_walk_group<D, U>(forest_addr + (k & 1u) * p.piece_bytes + g_off, p.tree_stride, xs_lane, p.mul_two, p.mul_64k, p.add_64k, acc);
                 __syncthreads(); /* every warp is done with this slot: refill it while the other slot is walked */
                 if (tid == 0 && piece + 2 < p.n_pieces) issue_piece(k + 2u);
             }
             if (mine) partial[warp * 32 + lane] = acc;
             __syncthreads();
+            RANK_PHASE(WALK_DONE);
+            if (round == 0 && !wait_first) wait_previous();
             for (int r = tid; r < n_rows; r += B2F_RANK_THREADS) {
                 const int t = r >> 5, ln = r & 31;
                 double s = p.agg_mode == B2F_AGG_GBDT_LOGISTIC ? p.init_raw : 0.0;
@@ -269,6 +318,8 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
             }
         }
         __syncthreads();
+        RANK_PHASE(WALK_DONE);
+        if (round == 0 && !wait_first) wait_previous();
 
         /* ---- phase 3: one thread per row: partials in warp order -> aggregate -> store ---- */
         for (int r = tid; r < n_rows; r += B2F_RANK_THREADS) {
@@ -291,4 +342,8 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
     if constexpr (!STREAM) {
         if (!forest_ready) mbar_wait(&forest_bar[0], 0); /* never retire a CTA while a bulk copy into its shared memory is in flight */
     }
+#ifdef B2F_RANK_PHASES
+    __syncthreads(); /* EXIT = the CTA's last store, not thread 0's */
+#endif
+    RANK_PHASE(EXIT);
 }

@@ -360,7 +360,13 @@ void *b2f_device_alloc(b2f_model *m, size_t nbytes);
 void b2f_device_free(b2f_model *m, void *dptr);
 int b2f_copy_h2d(b2f_model *m, void *dst_dev, const void *src_host, size_t nbytes);
 int b2f_copy_d2h(b2f_model *m, void *dst_host, const void *src_dev, size_t nbytes);
-/* enqueue one predict launch on the model's compute stream (asynchronous) */
+/* enqueue one predict launch on the model's compute stream (asynchronous).
+ * Ordering (b2f_predict_device_ex and b2f_predict_stream_timed_ex alike): consecutive calls on one model's compute stream
+ * take effect in call order -- when several write the same proba / label buffer, the last call's values are what is left.
+ * With B2F_ROWS_RANKED rows, back-to-back launches overlap (programmatic dependent launch): a launch may read its rows
+ * while the previous ranked launch is still running.  Rows are read after every earlier operation on the stream that is
+ * not such a launch (copies, other kernels) has completed; rows must not be changed while launches that read them
+ * are in flight. */
 int b2f_predict_device(b2f_model *m, const void *rows_dev, int64_t n, void *proba1_dev,
                        int proba_is_f64, int32_t *label_dev);
 int b2f_predict_device_ex(b2f_model *m, const void *rows_dev, int64_t n, int row_format,
