@@ -23,6 +23,10 @@ PACKED_ROW_BYTES = 64
 ROWS_WORDS24 = 0
 ROWS_PACKED64 = 1
 ROWS_RANKED = 2
+OUT_F32 = 0  # output kinds (B2F_OUT_*): float proba1
+OUT_F64 = 1  # double proba1
+OUT_PAIRS = 2  # b2f_scored records
+OUT_FULL = 3  # b2f_scored_full records
 SCORED_DTYPE = np.dtype([("proba1", np.float32), ("label", np.int32)])  # b2f_scored
 SCORED_FULL_DTYPE = np.dtype(  # b2f_scored_full, 24 bytes
     [("proba1", np.float64), ("label", np.int32), ("is_outlier", np.int32), ("outlier_score", np.float32), ("reserved", np.int32)]

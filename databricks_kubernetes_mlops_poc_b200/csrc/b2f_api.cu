@@ -10,6 +10,7 @@
  */
 #include <cuda_runtime.h>
 #include <dlfcn.h>
+#include <limits.h>
 #include <nccl.h>
 #include <stdarg.h>
 #include <stddef.h>
@@ -318,11 +319,106 @@ extern "C" int b2f_ranker_rank_rows(const b2f_ranker *r, const void *rows, int64
     return B2F_OK;
 }
 
-template <int R, bool SMEM, typename OutT>
-static cudaError_t set_smem_attr(int bytes) {
-    cudaError_t e = cudaFuncSetAttribute(k_forest_predict<R, SMEM, false, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(k_forest_predict<R, SMEM, true, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+/* ------------------------------------------------------------------ kernel instantiations
+ * Launches and cudaFuncSetAttribute calls both take the instantiation from here, so each template axis is switched once. */
+template <typename OutT>
+using RankKernel = void (*)(RParams, const uint8_t *, long long, OutT *, int32_t *, int);
+
+template <int R, typename OutT>
+static auto warp_kernel_r(bool smem, bool pk) {
+    if (smem) return pk ? k_forest_predict<R, true, true, OutT> : k_forest_predict<R, true, false, OutT>;
+    return pk ? k_forest_predict<R, false, true, OutT> : k_forest_predict<R, false, false, OutT>;
+}
+template <typename OutT>
+static auto warp_kernel(int rows_per_warp, bool smem, bool pk) {
+    if (rows_per_warp == 4) return warp_kernel_r<4, OutT>(smem, pk);
+    return rows_per_warp == 2 ? warp_kernel_r<2, OutT>(smem, pk) : warp_kernel_r<1, OutT>(smem, pk);
+}
+template <typename OutT>
+static auto tile_kernel(bool pk) {
+    return pk ? k_forest_predict_tile<true, OutT> : k_forest_predict_tile<false, OutT>;
+}
+template <typename OutT>
+static auto split_kernel(bool pk) {
+    return pk ? k_forest_predict_split<2, true, OutT> : k_forest_predict_split<2, false, OutT>;
+}
+/* depths 1..8; NULL for any other depth */
+template <typename OutT, int D = 1>
+static RankKernel<OutT> rank_kernel(const b2f_model *m) {
+    if constexpr (D > 8) {
+        return nullptr;
+    } else {
+        if (m->rp.depth != D) return rank_kernel<OutT, D + 1>(m);
+        if (m->rank_stream) return k_forest_predict_rank<D, 4, true, OutT>;
+        return m->rank_u == 8 ? k_forest_predict_rank<D, 8, false, OutT> : k_forest_predict_rank<D, 4, false, OutT>;
+    }
+}
+template <typename K>
+static cudaError_t set_smem_limit(K kernel, int bytes) {
+    return kernel ? cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) : cudaErrorInvalidValue;
+}
+
+/* ------------------------------------------------------------------ environment hooks read at model creation (INTEGRATION.md) */
+enum { KN_AUTO, KN_WARP, KN_TILE, KN_SPLIT };
+struct EnvHooks {
+    int kernel = KN_AUTO;      /* B2F_KERNEL: "warp" | "tile" | "split" pins one predict kernel (tests) */
+    bool walk_global = false;  /* B2F_FORCE_WALK=global: walk the forest from global memory (test hook) */
+    bool walk_smem = false;    /* B2F_FORCE_WALK=smem: shared-memory walk, an error if the forest does not fit */
+    int64_t chunk_rows = B2F_CHUNK_ROWS; /* B2F_CHUNK_ROWS (>= 1024): rows per pipelined H2D/kernel/D2H chunk */
+    /* B2F_CHUNK_PLAN="a,b,c": per-chunk share of a batch in 1/1024ths.  65 536-row batches: 3/4 of the batch, then the rest.
+     * tools/chunk_plan_sweep.py on an H100 80GB HBM3 (700 W): the best of nine plans for both row formats -- 88 us p50 per
+     * ranked-row call against 108 us in one chunk, 145 us against 158 us with 64-byte rows */
+    std::vector<int64_t> chunk_plan{768};
+    /* B2F_SPLIT_MAX_ROWS: the latency form (one CTA per 2 rows, warp = tree group) hands over to the warp-per-row kernel at
+     * 2 048 rows: below that the warp-per-row kernel leaves most SMs idle while the latency form spreads one row's trees over a
+     * CTA's warps.  tools/split_threshold.py on an H100 80GB HBM3 (700 W), synchronous 64-byte-row calls, GBDT 500 x d8: 38 vs
+     * 64 us at 512 rows, 72 vs 80 at 2 048, 89 vs 79 at 3 072; GBDT 100 x d6: within ~5 us of each other at every size up to
+     * 4 096. */
+    int64_t split_max_rows = 2048;
+    int rows_per_warp = 2;      /* B2F_ROWS_PER_WARP: 1 | 2 | 4 */
+    int64_t tile_min_rows = -1; /* B2F_TILE_MIN_ROWS (>= 0); -1 = by the tile layout */
+    int tile_warps = 0;         /* B2F_TILE_WARPS (clamped to 1..B2F_TILE_WARPS_MAX); 0 = choose */
+    bool rank_off = false;      /* B2F_RANK=0: no rank kernel */
+    int rank_max_tiles = INT_MAX; /* B2F_RANK_MAX_TILES (>= 1): cap on the resident rank kernel's row tiles */
+    int rank_stream = -1;       /* B2F_RANK_STREAM: 1 / 0 force / forbid the streamed rank kernel; -1 = by size */
+    int rank_u = 4;             /* B2F_RANK_U: 4 | 8 trees in flight per thread */
+    bool rank_wait_first = false; /* B2F_RANK_WAIT_FIRST=1: the rank kernel's dependency wait back at kernel entry (A/B) */
+    bool no_pdl = false;        /* B2F_NO_PDL: launch the rank kernel without programmatic stream serialization */
+};
+
+static EnvHooks read_env_hooks(void) {
+    EnvHooks h;
+    if (const char *v = getenv("B2F_KERNEL"))
+        h.kernel = !strcmp(v, "warp") ? KN_WARP : !strcmp(v, "tile") ? KN_TILE : !strcmp(v, "split") ? KN_SPLIT : KN_AUTO;
+    if (const char *v = getenv("B2F_FORCE_WALK")) {
+        h.walk_global = !strcmp(v, "global");
+        h.walk_smem = !strcmp(v, "smem");
+    }
+    if (const char *v = getenv("B2F_CHUNK_ROWS"))
+        if (atoll(v) >= 1024) h.chunk_rows = atoll(v);
+    if (const char *v = getenv("B2F_CHUNK_PLAN")) {
+        h.chunk_plan.clear();
+        for (const char *q = v; *q;) {
+            h.chunk_plan.push_back(atoll(q));
+            while (*q && *q != ',') ++q;
+            if (*q == ',') ++q;
+        }
+    }
+    if (const char *v = getenv("B2F_SPLIT_MAX_ROWS")) h.split_max_rows = atoll(v);
+    if (const char *v = getenv("B2F_ROWS_PER_WARP")) {
+        const int r = atoi(v);
+        if (r == 1 || r == 2 || r == 4) h.rows_per_warp = r;
+    }
+    if (const char *v = getenv("B2F_TILE_MIN_ROWS"))
+        if (atoll(v) >= 0) h.tile_min_rows = atoll(v);
+    if (const char *v = getenv("B2F_TILE_WARPS")) h.tile_warps = std::min(B2F_TILE_WARPS_MAX, std::max(1, atoi(v)));
+    if (const char *v = getenv("B2F_RANK")) h.rank_off = !strcmp(v, "0");
+    if (const char *v = getenv("B2F_RANK_MAX_TILES")) h.rank_max_tiles = std::max(1, atoi(v));
+    if (const char *v = getenv("B2F_RANK_STREAM")) h.rank_stream = atoi(v) != 0;
+    if (const char *v = getenv("B2F_RANK_U")) h.rank_u = atoi(v) == 8 ? 8 : 4;
+    if (const char *v = getenv("B2F_RANK_WAIT_FIRST")) h.rank_wait_first = atoi(v) != 0;
+    h.no_pdl = getenv("B2F_NO_PDL") != nullptr;
+    return h;
 }
 
 
@@ -441,43 +537,21 @@ static bool build_tile_layout(const uint8_t *blob, const b2f_blob_header &h, uin
     return true;
 }
 
-template <int D, int U, bool ST, typename OutT>
-static cudaError_t rank_set_attr(int bytes) {
-    return cudaFuncSetAttribute(k_forest_predict_rank<D, U, ST, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-}
-template <int U, bool ST>
-static cudaError_t rank_set_attr_all(int depth, int bytes) {
-    cudaError_t e = cudaSuccess;
-#define RK_ATTR(DD)                                                        \
-    case DD:                                                               \
-        e = rank_set_attr<DD, U, ST, float>(bytes);                        \
-        if (e == cudaSuccess) e = rank_set_attr<DD, U, ST, double>(bytes); \
-        break;
-    switch (depth) {
-        RK_ATTR(1) RK_ATTR(2) RK_ATTR(3) RK_ATTR(4) RK_ATTR(5) RK_ATTR(6) RK_ATTR(7) RK_ATTR(8)
-        default: e = cudaErrorInvalidValue;
-    }
-#undef RK_ATTR
-    return e;
-}
-
-static int rank_init(b2f_model *m, const uint8_t *blob) {
+/* rank kernel: 4-byte integer nodes, complete trees, rows as ranks (forest_rank.h) */
+static int rank_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
     m->rank_ok = false;
     ranker_build(&m->rk, blob, m->hdr);
     if (!m->rk.ok) return B2F_OK; /* no rank layout for this forest: the other kernels serve it */
-    const char *off = getenv("B2F_RANK");
-    if (off && !strcmp(off, "0")) return B2F_OK;
+    if (env.rank_off) return B2F_OK;
     const int64_t layout_bytes = (int64_t)m->rk.layout.size();
     const int64_t base = B2F_RANK_XS_BYTES /* alignment slack */ + (int64_t)B2F_RANK_PARTIALS * 32 * 8 + 256;
     int max_tiles = (int)std::min<int64_t>(B2F_RANK_MAX_TILES, ((int64_t)m->max_smem_optin - base - layout_bytes) / B2F_RANK_XS_BYTES);
-    if (const char *mt = getenv("B2F_RANK_MAX_TILES")) max_tiles = std::min(max_tiles, std::max(1, atoi(mt)));
+    max_tiles = std::min(max_tiles, env.rank_max_tiles);
     /* resident while the whole layout fits next to a useful number of row tiles; otherwise it streams through a two-slot ring
      * in pieces of 8 trees (2 groups of 4: warp w owns (tile w / 2, group w mod 2), so <= 16 tiles per round) */
-    m->rank_stream = max_tiles < 8;
-    if (const char *fs = getenv("B2F_RANK_STREAM")) m->rank_stream = atoi(fs) != 0;
+    m->rank_stream = env.rank_stream < 0 ? max_tiles < 8 : env.rank_stream != 0;
     int64_t forest_smem = layout_bytes;
-    m->rank_u = 4;
-    if (const char *ru = getenv("B2F_RANK_U")) m->rank_u = atoi(ru) == 8 ? 8 : 4;
+    m->rank_u = env.rank_u;
     if (m->rank_stream) {
         m->rank_u = 4;
         const int64_t piece = 8 * (int64_t)m->rk.tree_stride; /* n_trees_padded is a multiple of 8 */
@@ -510,8 +584,8 @@ static int rank_init(b2f_model *m, const uint8_t *blob) {
     rp.mul_64k = 65536u;
     rp.add_64k = 65535u;
     rp.n_pairs = (int)m->rk.pairs.size();
-    if (const char *wf = getenv("B2F_RANK_WAIT_FIRST")) rp.wait_first = atoi(wf) != 0; /* A/B: the dependency wait back at kernel entry */
-    m->rank_pdl = getenv("B2F_NO_PDL") == nullptr;
+    rp.wait_first = env.rank_wait_first;
+    m->rank_pdl = !env.no_pdl;
     for (int j = 0; j < 16; ++j) {
         rp.cat_shift[j] = (uint8_t)m->rk.cat_shift[j];
         rp.cat_bits[j] = (uint8_t)m->rk.cat_bits[j];
@@ -524,32 +598,14 @@ static int rank_init(b2f_model *m, const uint8_t *blob) {
         rp.cat_mask[j] |= 1ull << c;
     }
     m->rank_smem_bytes = (int)(B2F_RANK_XS_BYTES + (int64_t)max_tiles * B2F_RANK_XS_BYTES + (int64_t)B2F_RANK_PARTIALS * 32 * 8 + forest_smem);
-    if (m->rank_stream)
-        CUDA_TRY((rank_set_attr_all<4, true>(rp.depth, m->rank_smem_bytes)));
-    else
-        CUDA_TRY(m->rank_u == 8 ? (rank_set_attr_all<8, false>(rp.depth, m->rank_smem_bytes)) : (rank_set_attr_all<4, false>(rp.depth, m->rank_smem_bytes)));
+    CUDA_TRY(set_smem_limit(rank_kernel<float>(m), m->rank_smem_bytes));
+    CUDA_TRY(set_smem_limit(rank_kernel<double>(m), m->rank_smem_bytes));
     m->rank_ok = true;
     return B2F_OK;
 }
 
-static bool kn_env_is(const char *v) {
-    const char *kn = getenv("B2F_KERNEL");
-    return kn && !strcmp(kn, v);
-}
-
-static int model_init_cuda(b2f_model *m, const uint8_t *blob, size_t nbytes) {
-    CUDA_TRY(cudaSetDevice(m->device));
-    cudaDeviceProp prop;
-    CUDA_TRY(cudaGetDeviceProperties(&prop, m->device));
-    if (prop.major != 9 || prop.minor != 0)
-        return set_err(B2F_ENODEV, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", m->device, prop.major, prop.minor);
-    m->sm_count = prop.multiProcessorCount;
-    CUDA_TRY(cudaDeviceGetAttribute(&m->max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, m->device));
-
-    CUDA_TRY(cudaMalloc(&m->d_blob, nbytes));
-    CUDA_TRY(cudaMemcpy(m->d_blob, blob, nbytes, cudaMemcpyHostToDevice));
-    m->forest_bytes = (int64_t)m->hdr.chunks_bytes;
-
+/* warp-per-row and latency kernels: the walk mode, the split hand-over and the chunking of host batches */
+static int warp_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
     KParams &kp = m->kp;
     memset(&kp, 0, sizeof(kp));
     kp.chunks = static_cast<const uint8_t *>(m->d_blob) + m->hdr.chunks_off;
@@ -577,124 +633,87 @@ static int model_init_cuda(b2f_model *m, const uint8_t *blob, size_t nbytes) {
 
     /* shared-memory residency: whole forest + static barriers must fit the opt-in limit */
     const int64_t need = (int64_t)m->hdr.chunks_bytes;
-    const char *force = getenv("B2F_FORCE_WALK"); /* "smem" | "global": test hook */
-    bool fits = need + 1024 <= (int64_t)m->max_smem_optin;
-    if (force && !strcmp(force, "global")) fits = false;
-    if (force && !strcmp(force, "smem") && !fits) return set_err(B2F_EINVAL, "B2F_FORCE_WALK=smem but forest needs %lld bytes", (long long)need);
+    const bool fits = need + 1024 <= (int64_t)m->max_smem_optin && !env.walk_global;
+    if (env.walk_smem && !fits) return set_err(B2F_EINVAL, "B2F_FORCE_WALK=smem but forest needs %lld bytes", (long long)need);
     m->walk_mode = fits ? B2F_WALK_SMEM : B2F_WALK_GLOBAL;
     m->smem_bytes = fits ? (int)need : 0;
-    if (fits) {
-        CUDA_TRY((set_smem_attr<1, true, float>(m->smem_bytes)));
-        CUDA_TRY((set_smem_attr<2, true, float>(m->smem_bytes)));
-        CUDA_TRY((set_smem_attr<4, true, float>(m->smem_bytes)));
-        CUDA_TRY((set_smem_attr<1, true, double>(m->smem_bytes)));
-        CUDA_TRY((set_smem_attr<2, true, double>(m->smem_bytes)));
-        CUDA_TRY((set_smem_attr<4, true, double>(m->smem_bytes)));
-    }
-    const char *cr = getenv("B2F_CHUNK_ROWS"); /* tuning hook: rows per pipelined H2D/kernel/D2H chunk */
-    if (cr && atoll(cr) >= 1024) m->chunk_rows = atoll(cr);
-    /* 65 536-row batches: 3/4 of the batch, then the rest.  tools/chunk_plan_sweep.py on an H100 80GB HBM3 (700 W): the best of
-     * nine plans for both row formats -- 88 us p50 per ranked-row call against 108 us in one chunk, 145 us against 158 us with
-     * 64-byte rows */
-    m->chunk_plan = {768};
-    if (const char *pl = getenv("B2F_CHUNK_PLAN")) {
-        m->chunk_plan.clear();
-        for (const char *q = pl; *q;) {
-            m->chunk_plan.push_back(atoll(q));
-            while (*q && *q != ',') ++q;
-            if (*q == ',') ++q;
-        }
-    }
-    /* latency kernel: while rows x groups warps still fit about two waves of the chip */
-    /* the latency form (one CTA per 2 rows, warp = tree group) hands over to the warp-per-row kernel at 2 048 rows: below that
-     * the warp-per-row kernel leaves most SMs idle while the latency form spreads one row's trees over a CTA's warps.
-     * tools/split_threshold.py on an H100 80GB HBM3 (700 W), synchronous 64-byte-row calls, GBDT 500 x d8: 38 vs 64 us at 512
-     * rows, 72 vs 80 at 2 048, 89 vs 79 at 3 072; GBDT 100 x d6: within ~5 us of each other at every size up to 4 096. */
-    m->split_max_rows = 2048;
-    if (const char *sp = getenv("B2F_SPLIT_MAX_ROWS")) m->split_max_rows = atoll(sp);
-    if (kn_env_is("warp") || kn_env_is("tile")) m->split_max_rows = 0; /* tests pin one kernel */
-    if (kn_env_is("split")) m->split_max_rows = INT64_MAX;
-    const char *rpw = getenv("B2F_ROWS_PER_WARP");
-    m->rows_per_warp_max = 2;
-    if (rpw) {
-        int v = atoi(rpw);
-        if (v == 1 || v == 2 || v == 4) m->rows_per_warp_max = v;
-    }
-
-    /* tile kernel: tree-major layout + shared-memory ring plan */
-    {
-        const char *kn = getenv("B2F_KERNEL"); /* "warp" | "tile" | unset = choose by batch size */
-        const char *tm = getenv("B2F_TILE_MIN_ROWS");
-        std::vector<uint8_t> layout;
-        std::vector<TPiece> pieces;
-        uint32_t slot_bytes = 0;
-        int n_slots = 0;
-        bool ok = false;
-        /* most consumer warps for which the forest still stays resident; else 16 warps and a streamed forest */
-        int cwarps = B2F_TILE_WARPS_MIN;
-        if (!(kn && !strcmp(kn, "warp"))) {
-            if (const char *tw = getenv("B2F_TILE_WARPS")) {
-                cwarps = std::min(B2F_TILE_WARPS_MAX, std::max(1, atoi(tw)));
-                const uint32_t avail = (uint32_t)m->max_smem_optin - 1024u - 4096u - (uint32_t)cwarps * B2F_TILE_XS_BYTES;
-                ok = build_tile_layout(blob, m->hdr, avail, layout, pieces, &slot_bytes, &n_slots);
-            } else {
-                for (int w = B2F_TILE_WARPS_MAX; w >= B2F_TILE_WARPS_MIN && !ok; w -= 4) {
-                    const uint32_t avail = (uint32_t)m->max_smem_optin - 1024u - 4096u - (uint32_t)w * B2F_TILE_XS_BYTES;
-                    const bool built = build_tile_layout(blob, m->hdr, avail, layout, pieces, &slot_bytes, &n_slots);
-                    const bool res = built && (int)pieces.size() <= n_slots;
-                    if (built && (res || w == B2F_TILE_WARPS_MIN)) {
-                        ok = true;
-                        cwarps = w;
-                    }
-                }
+    if (fits)
+        for (bool pk : {false, true})
+            for (int r : {1, 2, 4}) {
+                CUDA_TRY(set_smem_limit(warp_kernel<float>(r, true, pk), m->smem_bytes));
+                CUDA_TRY(set_smem_limit(warp_kernel<double>(r, true, pk), m->smem_bytes));
             }
-        }
-        if (ok) {
-            CUDA_TRY(cudaMalloc(&m->d_tile_layout, layout.size()));
-            CUDA_TRY(cudaMemcpy(m->d_tile_layout, layout.data(), layout.size(), cudaMemcpyHostToDevice));
-            CUDA_TRY(cudaMalloc((void **)&m->d_tile_pieces, pieces.size() * sizeof(TPiece)));
-            CUDA_TRY(cudaMemcpy(m->d_tile_pieces, pieces.data(), pieces.size() * sizeof(TPiece), cudaMemcpyHostToDevice));
-            TParams &tp = m->tp;
-            memset(&tp, 0, sizeof(tp));
-            tp.layout = static_cast<const uint8_t *>(m->d_tile_layout);
-            tp.pieces = m->d_tile_pieces;
-            tp.n_pieces = (int)pieces.size();
-            tp.n_slots = n_slots;
-            tp.slot_bytes = slot_bytes;
-            tp.agg_mode = kp.agg_mode;
-            tp.n_cat = kp.n_cat;
-            tp.n_num = kp.n_num;
-            tp.init_raw = kp.init_raw;
-            tp.denom = kp.denom;
-            tp.threshold = kp.threshold;
-            memcpy(tp.impute, kp.impute, sizeof(tp.impute));
-            m->tile_cwarps = cwarps;
-            m->tile_smem_bytes = 4096 + cwarps * B2F_TILE_XS_BYTES + n_slots * (int)slot_bytes;
-            m->tile_layout_bytes = (int64_t)layout.size();
-            CUDA_TRY(cudaFuncSetAttribute(k_forest_predict_tile<false, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, m->tile_smem_bytes));
-            CUDA_TRY(cudaFuncSetAttribute(k_forest_predict_tile<false, double>, cudaFuncAttributeMaxDynamicSharedMemorySize, m->tile_smem_bytes));
-            CUDA_TRY(cudaFuncSetAttribute(k_forest_predict_tile<true, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, m->tile_smem_bytes));
-            CUDA_TRY(cudaFuncSetAttribute(k_forest_predict_tile<true, double>, cudaFuncAttributeMaxDynamicSharedMemorySize, m->tile_smem_bytes));
-            m->tile_ok = true;
-            /* crossover chosen on the previous GPU generation and kept, not re-measured on the H100: a resident forest ties
-             * with the warp kernel from 65 536 rows up (and sums in sklearn's tree order); a streamed forest wins from ~24k rows */
-            m->tile_min_rows = (tp.n_pieces <= tp.n_slots) ? 65536 : 24576;
-            if (tm && atoll(tm) >= 0) m->tile_min_rows = atoll(tm);
-            if (kn && !strcmp(kn, "tile")) m->tile_min_rows = 1;
-        } else if (kn && !strcmp(kn, "tile")) {
-            return set_err(B2F_EINVAL, "B2F_KERNEL=tile but the forest's trees do not fit the tile kernel's shared-memory ring");
+    m->chunk_rows = env.chunk_rows;
+    m->chunk_plan = env.chunk_plan;
+    m->split_max_rows = env.split_max_rows;
+    if (env.kernel == KN_WARP || env.kernel == KN_TILE) m->split_max_rows = 0;
+    if (env.kernel == KN_SPLIT) m->split_max_rows = INT64_MAX;
+    m->rows_per_warp_max = env.rows_per_warp;
+    return B2F_OK;
+}
+
+/* tile kernel (large batches): tree-major layout + shared-memory ring plan */
+static int tile_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
+    std::vector<uint8_t> layout;
+    std::vector<TPiece> pieces;
+    uint32_t slot_bytes = 0;
+    int n_slots = 0;
+    bool ok = false;
+    /* most consumer warps for which the forest still stays resident, else 16 warps and a streamed forest (B2F_TILE_WARPS: that many) */
+    int cwarps = B2F_TILE_WARPS_MIN;
+    const int w_hi = env.tile_warps ? env.tile_warps : B2F_TILE_WARPS_MAX, w_lo = env.tile_warps ? env.tile_warps : B2F_TILE_WARPS_MIN;
+    for (int w = w_hi; env.kernel != KN_WARP && w >= w_lo && !ok; w -= 4) {
+        const uint32_t avail = (uint32_t)m->max_smem_optin - 1024u - 4096u - (uint32_t)w * B2F_TILE_XS_BYTES;
+        const bool built = build_tile_layout(blob, m->hdr, avail, layout, pieces, &slot_bytes, &n_slots);
+        const bool res = built && (int)pieces.size() <= n_slots;
+        if (built && (res || w == w_lo)) {
+            ok = true;
+            cwarps = w;
         }
     }
-
-    /* rank kernel: 4-byte integer nodes, complete trees, rows as ranks (forest_rank.h); only while the layout stays resident */
-    {
-        int rc = rank_init(m, blob);
-        if (rc) return rc;
+    if (!ok) {
+        if (env.kernel == KN_TILE) return set_err(B2F_EINVAL, "B2F_KERNEL=tile but the forest's trees do not fit the tile kernel's shared-memory ring");
+        return B2F_OK;
     }
+    CUDA_TRY(cudaMalloc(&m->d_tile_layout, layout.size()));
+    CUDA_TRY(cudaMemcpy(m->d_tile_layout, layout.data(), layout.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMalloc((void **)&m->d_tile_pieces, pieces.size() * sizeof(TPiece)));
+    CUDA_TRY(cudaMemcpy(m->d_tile_pieces, pieces.data(), pieces.size() * sizeof(TPiece), cudaMemcpyHostToDevice));
+    const KParams &kp = m->kp;
+    TParams &tp = m->tp;
+    memset(&tp, 0, sizeof(tp));
+    tp.layout = static_cast<const uint8_t *>(m->d_tile_layout);
+    tp.pieces = m->d_tile_pieces;
+    tp.n_pieces = (int)pieces.size();
+    tp.n_slots = n_slots;
+    tp.slot_bytes = slot_bytes;
+    tp.agg_mode = kp.agg_mode;
+    tp.n_cat = kp.n_cat;
+    tp.n_num = kp.n_num;
+    tp.init_raw = kp.init_raw;
+    tp.denom = kp.denom;
+    tp.threshold = kp.threshold;
+    memcpy(tp.impute, kp.impute, sizeof(tp.impute));
+    m->tile_cwarps = cwarps;
+    m->tile_smem_bytes = 4096 + cwarps * B2F_TILE_XS_BYTES + n_slots * (int)slot_bytes;
+    m->tile_layout_bytes = (int64_t)layout.size();
+    for (bool pk : {false, true}) {
+        CUDA_TRY(set_smem_limit(tile_kernel<float>(pk), m->tile_smem_bytes));
+        CUDA_TRY(set_smem_limit(tile_kernel<double>(pk), m->tile_smem_bytes));
+    }
+    m->tile_ok = true;
+    /* crossover chosen on the previous GPU generation and kept, not re-measured on the H100: a resident forest ties
+     * with the warp kernel from 65 536 rows up (and sums in sklearn's tree order); a streamed forest wins from ~24k rows */
+    m->tile_min_rows = (tp.n_pieces <= tp.n_slots) ? 65536 : 24576;
+    if (env.tile_min_rows >= 0) m->tile_min_rows = env.tile_min_rows;
+    if (env.kernel == KN_TILE) m->tile_min_rows = 1;
+    return B2F_OK;
+}
 
+/* streams, and the feature-moments kernel's scratch */
+static int streams_init(b2f_model *m) {
     for (int s = 0; s < B2F_STREAMS; ++s) CUDA_TRY(cudaStreamCreateWithFlags(&m->slots[s].stream, cudaStreamNonBlocking));
     CUDA_TRY(cudaStreamCreateWithFlags(&m->compute, cudaStreamNonBlocking));
-
     CUDA_TRY(cudaFuncSetAttribute(k_feature_moments, cudaFuncAttributeMaxDynamicSharedMemorySize, B2F_MOM_SMEM));
     m->mom_blocks = m->sm_count * 3; /* one full wave: 3 CTAs (3-stage 72 KB ring each) per SM */
     CUDA_TRY(cudaMalloc(&m->d_mom_partials, (size_t)m->mom_blocks * B2F_MOM_VALUES * sizeof(double)));
@@ -702,6 +721,25 @@ static int model_init_cuda(b2f_model *m, const uint8_t *blob, size_t nbytes) {
     CUDA_TRY(cudaMemset(m->d_mom_ticket, 0, sizeof(unsigned int)));
     CUDA_TRY(cudaMalloc(&m->d_mom_out, B2F_MOM_VALUES * sizeof(double)));
     return B2F_OK;
+}
+
+static int model_init_cuda(b2f_model *m, const uint8_t *blob, size_t nbytes) {
+    const EnvHooks env = read_env_hooks();
+    CUDA_TRY(cudaSetDevice(m->device));
+    cudaDeviceProp prop;
+    CUDA_TRY(cudaGetDeviceProperties(&prop, m->device));
+    if (prop.major != 9 || prop.minor != 0)
+        return set_err(B2F_ENODEV, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", m->device, prop.major, prop.minor);
+    m->sm_count = prop.multiProcessorCount;
+    CUDA_TRY(cudaDeviceGetAttribute(&m->max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, m->device));
+    CUDA_TRY(cudaMalloc(&m->d_blob, nbytes));
+    CUDA_TRY(cudaMemcpy(m->d_blob, blob, nbytes, cudaMemcpyHostToDevice));
+    m->forest_bytes = (int64_t)m->hdr.chunks_bytes;
+    int rc = warp_init(m, blob, env);
+    if (rc == B2F_OK) rc = tile_init(m, blob, env);
+    if (rc == B2F_OK) rc = rank_init(m, blob, env);
+    if (rc == B2F_OK) rc = streams_init(m);
+    return rc;
 }
 
 extern "C" b2f_model *b2f_model_create(const void *forest_blob, size_t nbytes, int device) {
@@ -821,32 +859,24 @@ extern "C" void b2f_pinned_free(void *p) {
 }
 
 /* ------------------------------------------------------------------ kernel launch */
-template <int R, bool SMEM, bool PACKED, typename OutT>
-static cudaError_t launch_one(const b2f_model *m, cudaStream_t st, const void *rows, int64_t n, void *proba, int32_t *label, int ostride) {
-    const int64_t n_batches = (n + R - 1) / R;
-    int64_t ctas = std::min<int64_t>(m->sm_count, n_batches);
-    if (ctas < 1) ctas = 1;
-    k_forest_predict<R, SMEM, PACKED, OutT><<<(unsigned)ctas, B2F_PREDICT_THREADS, SMEM ? m->smem_bytes : 0, st>>>(
-        m->kp, static_cast<const uint32_t *>(rows), (long long)n, static_cast<OutT *>(proba), label, ostride);
-    return cudaGetLastError();
+enum KernelKind { KERN_RANK, KERN_TILE, KERN_SPLIT, KERN_WARP };
+struct KernelChoice {
+    KernelKind kind;
+    int rows_per_warp = 0; /* KERN_WARP */
+    bool smem = false;     /* KERN_WARP: the forest is resident in shared memory */
+};
+
+/* which kernel scores n rows of format fmt */
+static KernelChoice pick_kernel(const b2f_model *m, int64_t n, int fmt) {
+    if (fmt == B2F_ROWS_RANKED) return {KERN_RANK}; /* ranked rows have one kernel: integer compares on the rank layout */
+    if (m->tile_ok && n >= m->tile_min_rows) return {KERN_TILE};
+    if (n <= m->split_max_rows) return {KERN_SPLIT}; /* a handful of rows: spread each row's tree groups over the warps of a CTA */
+    return {KERN_WARP, pick_rows_per_warp(m, n), m->walk_mode == B2F_WALK_SMEM};
 }
 
-template <bool PACKED, typename OutT>
-static cudaError_t launch_tile(const b2f_model *m, cudaStream_t st, const void *rows, int64_t n, void *proba, int32_t *label, int ostride) {
-    const int64_t n_tiles = (n + B2F_TILE_ROWS - 1) / B2F_TILE_ROWS;
-    const unsigned ctas = (unsigned)std::max<int64_t>(1, std::min<int64_t>(m->sm_count, n_tiles));
-    k_forest_predict_tile<PACKED, OutT><<<ctas, (unsigned)(m->tile_cwarps + 1) * 32u, m->tile_smem_bytes, st>>>(m->tp, static_cast<const uint32_t *>(rows), (long long)n,
-                                                                                           static_cast<OutT *>(proba), label, ostride);
-    return cudaGetLastError();
-}
-
-template <bool PACKED, typename OutT>
-static cudaError_t launch_split(const b2f_model *m, cudaStream_t st, const void *rows, int64_t n, void *proba, int32_t *label, int ostride) {
-    constexpr int R = 2;
-    const unsigned ctas = (unsigned)((n + R - 1) / R);
-    k_forest_predict_split<R, PACKED, OutT><<<ctas, 32u * (unsigned)m->kp.n_groups, 0, st>>>(m->kp, static_cast<const uint32_t *>(rows), (long long)n,
-                                                                                            static_cast<OutT *>(proba), label, ostride);
-    return cudaGetLastError();
+/* persistent kernels: one CTA per `rows_per_cta` rows, at most one per SM */
+static unsigned persistent_ctas(const b2f_model *m, int64_t n, int64_t rows_per_cta) {
+    return (unsigned)std::max<int64_t>(1, std::min<int64_t>(m->sm_count, (n + rows_per_cta - 1) / rows_per_cta));
 }
 
 #ifdef B2F_RANK_PHASES
@@ -866,11 +896,12 @@ extern "C" int b2f_rank_phases_arm(b2f_model *m, void *dev_buf, int launches) {
  * and walks before griddepcontrol.wait.  That is safe because no rank launch writes rows, and everything else that can
  * write them (H2D copies, every other kernel of this library or of the caller) is an ordinary stream predecessor of the
  * first relaxed launch of a chain.  The stores of launch N + 1 follow its wait, so the last launch writing a buffer wins. */
-template <int D, int U, bool ST, typename OutT>
-static cudaError_t launch_rank_du(const b2f_model *m, cudaStream_t st, const void *rows, int64_t n, void *proba, int32_t *label, int ostride) {
-    const int64_t n_tiles = (n + 31) / 32;
+template <typename OutT>
+static cudaError_t launch_rank(const b2f_model *m, cudaStream_t st, const void *rows, int64_t n, OutT *proba, int32_t *label, int ostride) {
+    const RankKernel<OutT> kernel = rank_kernel<OutT>(m);
+    if (!kernel) return cudaErrorInvalidValue;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)std::max<int64_t>(1, std::min<int64_t>(m->sm_count, n_tiles)));
+    cfg.gridDim = dim3(persistent_ctas(m, n, 32));
     cfg.blockDim = dim3(B2F_RANK_THREADS);
     cfg.dynamicSmemBytes = (size_t)m->rank_smem_bytes;
     cfg.stream = st;
@@ -885,21 +916,28 @@ static cudaError_t launch_rank_du(const b2f_model *m, cudaStream_t st, const voi
 #else
     const RParams &rp = m->rp;
 #endif
-    return cudaLaunchKernelEx(&cfg, k_forest_predict_rank<D, U, ST, OutT>, rp, static_cast<const uint8_t *>(rows), (long long)n,
-                              static_cast<OutT *>(proba), label, ostride);
+    return cudaLaunchKernelEx(&cfg, kernel, rp, static_cast<const uint8_t *>(rows), (long long)n, proba, label, ostride);
 }
+
 template <typename OutT>
-static cudaError_t launch_rank(const b2f_model *m, cudaStream_t st, const void *rows, int64_t n, void *proba, int32_t *label, int ostride) {
-#define RK_CASE(DD)                                                                                                  \
-    case DD:                                                                                                         \
-        if (m->rank_stream) return launch_rank_du<DD, 4, true, OutT>(m, st, rows, n, proba, label, ostride);          \
-        return m->rank_u == 8 ? launch_rank_du<DD, 8, false, OutT>(m, st, rows, n, proba, label, ostride)             \
-                              : launch_rank_du<DD, 4, false, OutT>(m, st, rows, n, proba, label, ostride);
-    switch (m->rp.depth) {
-        RK_CASE(1) RK_CASE(2) RK_CASE(3) RK_CASE(4) RK_CASE(5) RK_CASE(6) RK_CASE(7) RK_CASE(8)
+static cudaError_t launch_kernel(const b2f_model *m, const KernelChoice &kc, bool pk, cudaStream_t st, const void *rows, int64_t n, OutT *proba,
+                                 int32_t *label, int ostride) {
+    const uint32_t *w = static_cast<const uint32_t *>(rows);
+    switch (kc.kind) {
+    case KERN_RANK:
+        return launch_rank(m, st, rows, n, proba, label, ostride);
+    case KERN_TILE:
+        tile_kernel<OutT>(pk)<<<persistent_ctas(m, n, B2F_TILE_ROWS), (unsigned)(m->tile_cwarps + 1) * 32u, m->tile_smem_bytes, st>>>(m->tp, w, (long long)n, proba, label, ostride);
+        break;
+    case KERN_SPLIT: /* R = 2 rows per CTA */
+        split_kernel<OutT>(pk)<<<(unsigned)((n + 1) / 2), 32u * (unsigned)m->kp.n_groups, 0, st>>>(m->kp, w, (long long)n, proba, label, ostride);
+        break;
+    case KERN_WARP:
+        warp_kernel<OutT>(kc.rows_per_warp, kc.smem, pk)<<<persistent_ctas(m, n, kc.rows_per_warp), B2F_PREDICT_THREADS, kc.smem ? m->smem_bytes : 0, st>>>(
+            m->kp, w, (long long)n, proba, label, ostride);
+        break;
     }
-#undef RK_CASE
-    return cudaErrorInvalidValue;
+    return cudaGetLastError();
 }
 
 static size_t row_bytes_of(const b2f_model *m, int fmt) {
@@ -919,51 +957,57 @@ static int check_row_format(const b2f_model *m, int fmt) {
     return B2F_OK;
 }
 
-static int launch_predict(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, void *proba_dev, int f64, int32_t *label_dev,
+static int launch_predict(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, bool f64, void *proba_dev, int32_t *label_dev,
                           int ostride = 1) {
+    static const char *const names[] = {"k_forest_predict_rank", "k_forest_predict_tile", "k_forest_predict_split", "k_forest_predict"};
     if (n <= 0) return B2F_OK;
+    const KernelChoice kc = pick_kernel(m, n, fmt);
     const bool pk = fmt == B2F_ROWS_PACKED64;
-    cudaError_t e;
-    if (fmt == B2F_ROWS_RANKED) { /* ranked rows have one kernel: integer compares on the resident rank layout */
-        e = f64 ? launch_rank<double>(m, st, rows_dev, n, proba_dev, label_dev, ostride) : launch_rank<float>(m, st, rows_dev, n, proba_dev, label_dev, ostride);
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_forest_predict_rank launch failed: %s", cudaGetErrorString(e));
-        m->launches++;
-        m->launches_rank++;
-        return B2F_OK;
-    }
-    if (m->tile_ok && n >= m->tile_min_rows) {
-        e = pk ? (f64 ? launch_tile<true, double>(m, st, rows_dev, n, proba_dev, label_dev, ostride) : launch_tile<true, float>(m, st, rows_dev, n, proba_dev, label_dev, ostride))
-               : (f64 ? launch_tile<false, double>(m, st, rows_dev, n, proba_dev, label_dev, ostride) : launch_tile<false, float>(m, st, rows_dev, n, proba_dev, label_dev, ostride));
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_forest_predict_tile launch failed: %s", cudaGetErrorString(e));
-        m->launches++;
-        m->launches_tile++;
-        return B2F_OK;
-    }
-    if (n <= m->split_max_rows) { /* a handful of rows: spread each row's tree groups over the warps of a CTA */
-        e = pk ? (f64 ? launch_split<true, double>(m, st, rows_dev, n, proba_dev, label_dev, ostride) : launch_split<true, float>(m, st, rows_dev, n, proba_dev, label_dev, ostride))
-               : (f64 ? launch_split<false, double>(m, st, rows_dev, n, proba_dev, label_dev, ostride) : launch_split<false, float>(m, st, rows_dev, n, proba_dev, label_dev, ostride));
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_forest_predict_split launch failed: %s", cudaGetErrorString(e));
-        m->launches++;
-        m->launches_split++;
-        return B2F_OK;
-    }
-    const int r = pick_rows_per_warp(m, n);
-    const bool sm = m->walk_mode == B2F_WALK_SMEM;
-#define DISPATCH_T(RR, SM, PK)                                                                                      \
-    (f64 ? launch_one<RR, SM, PK, double>(m, st, rows_dev, n, proba_dev, label_dev, ostride)                         \
-         : launch_one<RR, SM, PK, float>(m, st, rows_dev, n, proba_dev, label_dev, ostride))
-#define DISPATCH(RR) (sm ? (pk ? DISPATCH_T(RR, true, true) : DISPATCH_T(RR, true, false)) : (pk ? DISPATCH_T(RR, false, true) : DISPATCH_T(RR, false, false)))
-    if (r == 4)
-        e = DISPATCH(4);
-    else if (r == 2)
-        e = DISPATCH(2);
-    else
-        e = DISPATCH(1);
-#undef DISPATCH
-#undef DISPATCH_T
-    if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_forest_predict launch failed: %s", cudaGetErrorString(e));
+    const cudaError_t e = f64 ? launch_kernel(m, kc, pk, st, rows_dev, n, static_cast<double *>(proba_dev), label_dev, ostride)
+                              : launch_kernel(m, kc, pk, st, rows_dev, n, static_cast<float *>(proba_dev), label_dev, ostride);
+    if (e != cudaSuccess) return set_err(B2F_ECUDA, "%s launch failed: %s", names[kc.kind], cudaGetErrorString(e));
     m->launches++;
+    if (kc.kind == KERN_RANK) m->launches_rank++;
+    if (kc.kind == KERN_TILE) m->launches_tile++;
+    if (kc.kind == KERN_SPLIT) m->launches_split++;
     return B2F_OK;
+}
+
+/* ------------------------------------------------------------------ output kinds (B2F_OUT_* in b2f.h)
+ * What one output row of a host-buffer call looks like, and which launches write it into a device buffer. */
+static size_t out_row_bytes(int kind) {
+    switch (kind) {
+    case B2F_OUT_F32: return sizeof(float);
+    case B2F_OUT_F64: return sizeof(double);
+    case B2F_OUT_PAIRS: return sizeof(b2f_scored);
+    case B2F_OUT_FULL: return sizeof(b2f_scored_full);
+    }
+    return 0;
+}
+
+/* have_out: the record pointer is not NULL, or there are no rows to write */
+static int out_check(const b2f_model *m, int kind, int fmt, bool have_out) {
+    if (!out_row_bytes(kind))
+        return set_err(B2F_EINVAL, "output kind %d: expected 0 (float), 1 (double), 2 (b2f_scored) or 3 (b2f_scored_full)", kind);
+    if (kind >= B2F_OUT_PAIRS && !have_out) return set_err(B2F_EINVAL, "record output requested but the output pointer is NULL");
+    if (kind == B2F_OUT_FULL && !m->outlier) return set_err(B2F_ESTATE, "no outlier forest attached (b2f_model_attach_outlier_forest)");
+    if (kind == B2F_OUT_FULL && fmt == B2F_ROWS_RANKED)
+        return set_err(B2F_EINVAL, "b2f_scored_full records take float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranks are relative to ONE forest's split values");
+    return B2F_OK;
+}
+
+/* F32 / F64: proba and label arrays (either may be NULL).  PAIRS: {float, int32} records.  FULL: the classifier, then the
+ * outlier forest, on the same device rows, into 24-byte records (label_dev is ignored for records). */
+static int out_launch(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, int kind, void *out_dev, int32_t *label_dev) {
+    static_assert(sizeof(b2f_scored_full) == 24 && offsetof(b2f_scored_full, label) == 8 && offsetof(b2f_scored_full, is_outlier) == 12 &&
+                      offsetof(b2f_scored_full, outlier_score) == 16,
+                  "b2f_scored_full layout");
+    uint8_t *rec = static_cast<uint8_t *>(out_dev);
+    if (kind == B2F_OUT_PAIRS) return launch_predict(m, st, rows_dev, n, fmt, false, rec, reinterpret_cast<int32_t *>(rec + 4), 2);
+    if (kind != B2F_OUT_FULL) return launch_predict(m, st, rows_dev, n, fmt, kind == B2F_OUT_F64, out_dev, label_dev);
+    int rc = launch_predict(m, st, rows_dev, n, fmt, true, rec, reinterpret_cast<int32_t *>(rec + 8), B2F_OSTRIDE(3, 6));
+    if (rc) return rc;
+    return launch_predict(m->outlier, st, rows_dev, n, fmt, false, rec + 16, reinterpret_cast<int32_t *>(rec + 12), B2F_OSTRIDE(6, 6));
 }
 
 /* ------------------------------------------------------------------ host-buffer pipeline */
@@ -984,40 +1028,56 @@ static int slot_reserve(b2f_model *m, Slot &sl, int64_t rows) {
     return B2F_OK;
 }
 
+/* One chunk on one slot: rows [lo, lo + cnt) of the caller's host rows -> H2D -> the output kind's launches -> D2H into the
+ * caller's host output(s) at row lo.  marks (B2F_TIMELINE, may be NULL) gets an event before the first chunk's H2D, then one
+ * after each of its H2D, launches and D2H. */
+static int submit_chunk(b2f_model *m, Slot &sl, const void *rows, int fmt, int kind, void *out, int32_t *label, int64_t lo, int64_t cnt,
+                        std::vector<cudaEvent_t> *marks) {
+    int rc = slot_reserve(m, sl, cnt);
+    if (rc) return rc;
+    auto mark = [&] {
+        if (!marks) return;
+        cudaEvent_t e;
+        cudaEventCreate(&e);
+        cudaEventRecord(e, sl.stream);
+        marks->push_back(e);
+    };
+    if (marks && marks->empty()) mark();
+    const size_t row_bytes = row_bytes_of(m, fmt), out_bytes = out_row_bytes(kind);
+    const bool records = kind == B2F_OUT_PAIRS || kind == B2F_OUT_FULL;
+    CUDA_TRY(cudaMemcpyAsync(sl.d_rows, static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, (size_t)cnt * row_bytes, cudaMemcpyHostToDevice,
+                             sl.stream));
+    mark();
+    rc = out_launch(m, sl.stream, sl.d_rows, cnt, fmt, kind, out ? sl.d_proba : nullptr, label ? sl.d_label : nullptr);
+    if (rc) return rc;
+    mark();
+    if (out)
+        CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(out) + (size_t)lo * out_bytes, sl.d_proba, (size_t)cnt * out_bytes, cudaMemcpyDeviceToHost,
+                                 sl.stream));
+    if (label && !records) CUDA_TRY(cudaMemcpyAsync(label + lo, sl.d_label, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, sl.stream));
+    mark();
+    return B2F_OK;
+}
+
 /* enqueue the whole batch; on return used_mask tells which slot streams carry work.
  * B2F_TIMELINE=1 (debug): record an event after every operation and print the schedule to stderr. */
-static int enqueue_host_batch(b2f_model *m, const void *rows, int64_t n, int fmt, void *proba, int f64, int32_t *label, uint32_t *used_mask) {
+static int enqueue_host_batch(b2f_model *m, const void *rows, int64_t n, int fmt, void *out, int kind, int32_t *label, uint32_t *used_mask) {
     *used_mask = 0;
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
+    int rc = out_check(m, kind, fmt, out || n == 0);
+    if (rc) return rc;
     if (n == 0) return B2F_OK;
     if (!rows) return set_err(B2F_EINVAL, "rows is NULL");
-    {
-        int rcf = check_row_format(m, fmt);
-        if (rcf) return rcf;
-    }
-    const size_t row_bytes = row_bytes_of(m, fmt);
+    rc = check_row_format(m, fmt);
+    if (rc) return rc;
     CUDA_TRY(cudaSetDevice(m->device));
     int64_t chunk = m->chunk_rows;
     if (n <= chunk + chunk / 2) chunk = n; /* small batch: one H2D, one launch */
-    const size_t psz = f64 == 1 ? sizeof(double) : sizeof(float);
     static const bool timeline = getenv("B2F_TIMELINE") != nullptr;
     std::vector<cudaEvent_t> tev;
-    auto mark = [&](cudaStream_t st) {
-        if (!timeline) return;
-        cudaEvent_t e;
-        cudaEventCreate(&e);
-        cudaEventRecord(e, st);
-        tev.push_back(e);
-    };
     /* chunk schedule: equal chunks by default; a plan (B2F_CHUNK_PLAN="a,b,c": fractions of the batch in
      * 1/1024ths, the last chunk takes the remainder) front-loads the copies so the un-overlapped tail --
      * the last chunk's kernel and D2H -- is short */
-    const bool pairs = f64 == 2; /* proba points at {float proba; int32 label} records, label is ignored */
-    const bool full = f64 == 3;  /* proba points at b2f_scored_full records */
-    if (full && !m->outlier) return set_err(B2F_ESTATE, "no outlier forest attached (b2f_model_attach_outlier_forest)");
-    if (full && fmt == B2F_ROWS_RANKED)
-        return set_err(B2F_EINVAL, "b2f_predict_full takes float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranks are relative to ONE forest's split values");
-    if ((pairs || full) && !proba) return set_err(B2F_EINVAL, "out is NULL");
     int c = 0;
     for (int64_t off = 0; off < n; ++c) {
         int64_t cnt = std::min(chunk, n - off);
@@ -1025,53 +1085,13 @@ static int enqueue_host_batch(b2f_model *m, const void *rows, int64_t n, int fmt
             cnt = (size_t)c < m->chunk_plan.size() ? std::max<int64_t>(1024, (n * m->chunk_plan[c] / 1024 + 1023) / 1024 * 1024) : n - off;
             cnt = std::min(cnt, n - off);
         }
-        struct Advance {
-            int64_t &o, d;
-            ~Advance() { o += d; }
-        } advance{off, cnt};
         /* slots rotate ACROSS calls too, so with several batches in flight (async ring, stream dealer) the next
          * batch's H2D does not wait for the previous batch's kernel to release the same staging buffer */
         const int slot_idx = (int)((m->next_slot + (uint64_t)c) % B2F_STREAMS);
-        Slot &sl = m->slots[slot_idx];
-        int rc = slot_reserve(m, sl, cnt);
+        rc = submit_chunk(m, m->slots[slot_idx], rows, fmt, kind, out, label, off, cnt, timeline ? &tev : nullptr);
         if (rc) return rc;
-        if (c == 0) mark(sl.stream);
-        CUDA_TRY(cudaMemcpyAsync(sl.d_rows, static_cast<const uint8_t *>(rows) + (size_t)off * row_bytes, (size_t)cnt * row_bytes,
-                                 cudaMemcpyHostToDevice, sl.stream));
-        mark(sl.stream);
-        if (full) { /* classifier, then the outlier forest, on the same device rows; 24-byte records, ONE D2H copy */
-            static_assert(sizeof(b2f_scored_full) == 24 && offsetof(b2f_scored_full, label) == 8 && offsetof(b2f_scored_full, is_outlier) == 12 &&
-                              offsetof(b2f_scored_full, outlier_score) == 16,
-                          "b2f_scored_full layout");
-            uint8_t *rec = static_cast<uint8_t *>(sl.d_proba);
-            rc = launch_predict(m, sl.stream, sl.d_rows, cnt, fmt, rec, 1, reinterpret_cast<int32_t *>(rec + 8), B2F_OSTRIDE(3, 6));
-            if (rc) return rc;
-            rc = launch_predict(m->outlier, sl.stream, sl.d_rows, cnt, fmt, rec + 16, 0, reinterpret_cast<int32_t *>(rec + 12), B2F_OSTRIDE(6, 6));
-            if (rc) return rc;
-            mark(sl.stream);
-            CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(proba) + (size_t)off * sizeof(b2f_scored_full), sl.d_proba,
-                                     (size_t)cnt * sizeof(b2f_scored_full), cudaMemcpyDeviceToHost, sl.stream));
-            mark(sl.stream);
-            *used_mask |= 1u << slot_idx;
-            continue;
-        }
-        if (pairs) { /* one interleaved device buffer, ONE D2H copy per chunk */
-            rc = launch_predict(m, sl.stream, sl.d_rows, cnt, fmt, sl.d_proba, 0, static_cast<int32_t *>(sl.d_proba) + 1, 2);
-            if (rc) return rc;
-            mark(sl.stream);
-            CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(proba) + (size_t)off * 8, sl.d_proba, (size_t)cnt * 8, cudaMemcpyDeviceToHost, sl.stream));
-            mark(sl.stream);
-            *used_mask |= 1u << slot_idx;
-            continue;
-        }
-        rc = launch_predict(m, sl.stream, sl.d_rows, cnt, fmt, proba ? sl.d_proba : nullptr, f64, label ? sl.d_label : nullptr);
-        if (rc) return rc;
-        mark(sl.stream);
-        if (proba)
-            CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(proba) + (size_t)off * psz, sl.d_proba, (size_t)cnt * psz, cudaMemcpyDeviceToHost, sl.stream));
-        if (label) CUDA_TRY(cudaMemcpyAsync(label + off, sl.d_label, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, sl.stream));
-        mark(sl.stream);
         *used_mask |= 1u << slot_idx;
+        off += cnt;
     }
     m->next_slot += (uint64_t)c;
     if (timeline) {
@@ -1094,26 +1114,25 @@ static int sync_mask(b2f_model *m, uint32_t mask) {
     return B2F_OK;
 }
 
-static int predict_host(b2f_model *m, const void *rows, int64_t n, int fmt, void *proba, int f64, int32_t *label) {
+static int predict_host(b2f_model *m, const void *rows, int64_t n, int fmt, void *out, int kind, int32_t *label) {
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
     uint32_t mask = 0;
-    int rc = enqueue_host_batch(m, rows, n, fmt, proba, f64, label, &mask);
+    int rc = enqueue_host_batch(m, rows, n, fmt, out, kind, label, &mask);
     int rc2 = sync_mask(m, mask);
     return rc ? rc : rc2;
 }
 
 extern "C" int b2f_predict(b2f_model *m, const void *rows, int64_t n, float *proba1, int32_t *label) {
-    return predict_host(m, rows, n, B2F_ROWS_WORDS24, proba1, 0, label);
+    return predict_host(m, rows, n, B2F_ROWS_WORDS24, proba1, B2F_OUT_F32, label);
 }
 extern "C" int b2f_predict_f64(b2f_model *m, const void *rows, int64_t n, double *proba1, int32_t *label) {
-    return predict_host(m, rows, n, B2F_ROWS_WORDS24, proba1, 1, label);
+    return predict_host(m, rows, n, B2F_ROWS_WORDS24, proba1, B2F_OUT_F64, label);
 }
 extern "C" int b2f_predict_ex(b2f_model *m, const void *rows, int64_t n, int row_format, void *proba1, int proba_is_f64, int32_t *label) {
-    return predict_host(m, rows, n, row_format, proba1, proba_is_f64 ? 1 : 0, label);
+    return predict_host(m, rows, n, row_format, proba1, proba_is_f64 ? B2F_OUT_F64 : B2F_OUT_F32, label);
 }
 extern "C" int b2f_predict_pairs(b2f_model *m, const void *rows, int64_t n, int row_format, b2f_scored *out) {
-    if (!out && n > 0) return set_err(B2F_EINVAL, "out is NULL");
-    return predict_host(m, rows, n, row_format, out, 2, nullptr);
+    return predict_host(m, rows, n, row_format, out, B2F_OUT_PAIRS, nullptr);
 }
 
 extern "C" int b2f_model_attach_outlier_forest(b2f_model *m, const void *forest_blob, size_t nbytes) {
@@ -1137,7 +1156,7 @@ extern "C" int b2f_model_attach_outlier_forest(b2f_model *m, const void *forest_
 }
 
 extern "C" int b2f_predict_full(b2f_model *m, const void *rows, int64_t n, int row_format, b2f_scored_full *out) {
-    return predict_host(m, rows, n, row_format, out, 3, nullptr);
+    return predict_host(m, rows, n, row_format, out, B2F_OUT_FULL, nullptr);
 }
 
 extern "C" int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned, int proba_is_f64,
@@ -1148,8 +1167,6 @@ extern "C" int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t 
 extern "C" int b2f_predict_async_ex(b2f_model *m, const void *rows_pinned, int64_t n, int row_format, void *proba1_pinned, int proba_is_f64,
                                     int32_t *label_pinned, b2f_ticket *ticket) {
     if (!m || !ticket) return set_err(B2F_EINVAL, "null argument");
-    if (proba_is_f64 < 0 || proba_is_f64 > 3) return set_err(B2F_EINVAL, "proba_is_f64 = %d: expected 0 (float), 1 (double), 2 (b2f_scored) or 3 (b2f_scored_full)", proba_is_f64);
-    if (proba_is_f64 >= 2 && n > 0 && !proba1_pinned) return set_err(B2F_EINVAL, "record output requested but the output pointer is NULL");
     const uint64_t id = m->next_ticket++;
     TicketRec &t = m->tickets[id % B2F_TICKETS];
     if (t.id != 0) { /* oldest ticket still outstanding in this ring position: retire it */
@@ -1195,14 +1212,13 @@ extern "C" int b2f_predict_multi_ex(b2f_model **models, int n_models, const void
     const size_t row_bytes = row_bytes_of(models[0], row_format);
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
     std::vector<uint32_t> masks(n_models, 0);
-    /* 0 = float, 1 = double, 2 = b2f_scored records, 3 = b2f_scored_full records */
-    const size_t psz = proba_is_f64 == 3 ? sizeof(b2f_scored_full) : (proba_is_f64 ? sizeof(double) : sizeof(float));
+    const size_t out_bytes = out_row_bytes(proba_is_f64);
     int rc = B2F_OK;
     for (int i = 0; i < n_models && rc == B2F_OK; ++i) {
         const int64_t lo = n * i / n_models, hi = n * (i + 1) / n_models;
         if (hi <= lo) continue;
         rc = enqueue_host_batch(models[i], static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, hi - lo, row_format,
-                                proba1 ? static_cast<uint8_t *>(proba1) + (size_t)lo * psz : nullptr, proba_is_f64, label ? label + lo : nullptr,
+                                proba1 ? static_cast<uint8_t *>(proba1) + (size_t)lo * out_bytes : nullptr, proba_is_f64, label ? label + lo : nullptr,
                                 &masks[i]);
     }
     for (int i = 0; i < n_models; ++i) {
@@ -1223,8 +1239,7 @@ extern "C" int b2f_predict_stream(b2f_model **models, int n_models, const void *
     if (!models || n_models <= 0 || batch <= 0 || n < 0) return set_err(B2F_EINVAL, "bad argument");
     if (inflight < 1) inflight = 1;
     if (inflight > 8) inflight = 8;
-    const size_t row_bytes = row_bytes_of(models[0], row_format);
-    const size_t psz = proba_is_f64 ? sizeof(double) : sizeof(float);
+    const size_t row_bytes = row_bytes_of(models[0], row_format), out_bytes = out_row_bytes(proba_is_f64);
     const int64_t n_batches = (n + batch - 1) / batch;
     std::vector<int> rcs(n_models, B2F_OK);
     std::vector<std::string> msgs(n_models);
@@ -1242,7 +1257,8 @@ extern "C" int b2f_predict_stream(b2f_model **models, int n_models, const void *
             }
             b2f_ticket t = 0;
             rc = b2f_predict_async_ex(m, static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, cnt, row_format,
-                                      proba1 ? static_cast<uint8_t *>(proba1) + (size_t)lo * psz : nullptr, proba_is_f64, label ? label + lo : nullptr, &t);
+                                      proba1 ? static_cast<uint8_t *>(proba1) + (size_t)lo * out_bytes : nullptr, proba_is_f64,
+                                      label ? label + lo : nullptr, &t);
             if (rc == B2F_OK) ring.push_back(t);
         }
         for (b2f_ticket t : ring) {
@@ -1298,7 +1314,7 @@ extern "C" int b2f_predict_device_ex(b2f_model *m, const void *rows_dev, int64_t
     int rcf = check_row_format(m, row_format);
     if (rcf) return rcf;
     CUDA_TRY(cudaSetDevice(m->device));
-    return launch_predict(m, m->compute, rows_dev, n, row_format, proba1_dev, proba_is_f64, label_dev);
+    return out_launch(m, m->compute, rows_dev, n, row_format, proba_is_f64 ? B2F_OUT_F64 : B2F_OUT_F32, proba1_dev, label_dev);
 }
 extern "C" int b2f_sync(b2f_model *m) {
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
@@ -1326,7 +1342,7 @@ extern "C" int b2f_predict_device_timed(b2f_model *m, const void *rows_dev, int6
     for (int i = 0; i < iters && rc == B2F_OK; ++i) {
         if (flush_l2) CUDA_TRY(cudaMemsetAsync(m->d_flush, i & 0xff, B2F_FLUSH_BYTES, m->compute));
         CUDA_TRY(cudaEventRecord(ev[2 * i], m->compute));
-        rc = launch_predict(m, m->compute, rows_dev, n, B2F_ROWS_WORDS24, proba1_dev, proba_is_f64, label_dev);
+        rc = out_launch(m, m->compute, rows_dev, n, B2F_ROWS_WORDS24, proba_is_f64 ? B2F_OUT_F64 : B2F_OUT_F32, proba1_dev, label_dev);
         CUDA_TRY(cudaEventRecord(ev[2 * i + 1], m->compute));
     }
     CUDA_TRY(cudaStreamSynchronize(m->compute));
@@ -1357,16 +1373,16 @@ extern "C" int b2f_predict_stream_timed_ex(b2f_model *m, const void *rows_dev, i
     const bool each = ms_each != nullptr;
     std::vector<cudaEvent_t> ev(each ? 2 * (size_t)steps + 2 : 2);
     for (auto &e : ev) CUDA_TRY(cudaEventCreate(&e));
-    const size_t psz = proba_is_f64 ? sizeof(double) : sizeof(float);
+    const int kind = proba_is_f64 ? B2F_OUT_F64 : B2F_OUT_F32;
+    const size_t out_bytes = out_row_bytes(kind);
     const size_t i0 = ev.size() - 2, i1 = ev.size() - 1;
     int rc = B2F_OK;
     CUDA_TRY(cudaEventRecord(ev[i0], m->compute));
     for (int i = 0; i < steps && rc == B2F_OK; ++i) {
         const size_t b = (size_t)(i % pool);
         if (each) CUDA_TRY(cudaEventRecord(ev[2 * i], m->compute));
-        rc = launch_predict(m, m->compute, static_cast<const uint8_t *>(rows_dev) + b * (size_t)n * row_bytes, n, row_format,
-                            proba1_dev ? static_cast<uint8_t *>(proba1_dev) + b * (size_t)n * psz : nullptr, proba_is_f64,
-                            label_dev ? label_dev + b * (size_t)n : nullptr);
+        rc = out_launch(m, m->compute, static_cast<const uint8_t *>(rows_dev) + b * (size_t)n * row_bytes, n, row_format, kind,
+                        proba1_dev ? static_cast<uint8_t *>(proba1_dev) + b * (size_t)n * out_bytes : nullptr, label_dev ? label_dev + b * (size_t)n : nullptr);
         if (each) CUDA_TRY(cudaEventRecord(ev[2 * i + 1], m->compute));
     }
     CUDA_TRY(cudaEventRecord(ev[i1], m->compute));

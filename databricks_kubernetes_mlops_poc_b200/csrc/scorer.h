@@ -251,8 +251,7 @@ struct b2f_scorer {
     int64_t n = 0, chunk_rows = 0;
     int64_t chunk_lo[B2F_SCORER_MAX_CHUNKS + 1] = {}; /* chunk c = rows [chunk_lo[c], chunk_lo[c + 1]) */
     int n_chunks = 0, parts_per_chunk = 1;
-    int row_format = 0, out_mode = 1;
-    size_t row_bytes = 0, out_bytes = 8;
+    int row_format = 0, out_mode = B2F_OUT_F64;
     const b2f_str_column *cats = nullptr;
     const double *const *nums = nullptr;
     const int64_t *strides = nullptr;
@@ -288,22 +287,8 @@ static void scorer_submit_chunk(b2f_scorer *s, int c) {
     {
         std::lock_guard<std::mutex> lk(s->mu);
         Slot &sl = m->slots[c % B2F_STREAMS];
-        rc = slot_reserve(m, sl, cnt);
-        cudaError_t e = cudaSuccess;
-        if (rc == B2F_OK) e = cudaMemcpyAsync(sl.d_rows, s->h_rows + (size_t)lo * s->row_bytes, (size_t)cnt * s->row_bytes, cudaMemcpyHostToDevice, sl.stream);
-        if (rc == B2F_OK && e == cudaSuccess) {
-            if (s->out_mode == 3) {
-                uint8_t *rec = static_cast<uint8_t *>(sl.d_proba);
-                rc = launch_predict(m, sl.stream, sl.d_rows, cnt, s->row_format, rec, 1, reinterpret_cast<int32_t *>(rec + 8), B2F_OSTRIDE(3, 6));
-                if (rc == B2F_OK)
-                    rc = launch_predict(m->outlier, sl.stream, sl.d_rows, cnt, s->row_format, rec + 16, 0, reinterpret_cast<int32_t *>(rec + 12), B2F_OSTRIDE(6, 6));
-            } else {
-                rc = launch_predict(m, sl.stream, sl.d_rows, cnt, s->row_format, sl.d_proba, s->out_mode, nullptr);
-            }
-        }
-        if (rc == B2F_OK && e == cudaSuccess)
-            e = cudaMemcpyAsync(s->h_out + (size_t)lo * s->out_bytes, sl.d_proba, (size_t)cnt * s->out_bytes, cudaMemcpyDeviceToHost, sl.stream);
-        if (rc == B2F_OK && e == cudaSuccess) e = cudaEventRecord(s->ev[c], sl.stream);
+        rc = submit_chunk(m, sl, s->h_rows, s->row_format, s->out_mode, s->h_out, nullptr, lo, cnt, nullptr);
+        const cudaError_t e = rc == B2F_OK ? cudaEventRecord(s->ev[c], sl.stream) : cudaSuccess;
         if (e != cudaSuccess) {
             snprintf(s->err, sizeof(s->err), "CUDA error while submitting chunk %d: %s", c, cudaGetErrorString(e));
             rc = B2F_ECUDA;
@@ -411,7 +396,7 @@ extern "C" void b2f_scorer_destroy(b2f_scorer *s) {
 
 /* Start scoring n rows given as columns (same column arguments as b2f_encoder_encode).
  *   row_format : what the rows are encoded as on their way to the GPU (B2F_ROWS_RANKED / PACKED64 / WORDS24)
- *   out_mode   : 0 = float proba, 1 = double proba, 3 = b2f_scored_full records (needs an attached outlier forest)
+ *   out_mode   : B2F_OUT_F32, B2F_OUT_F64 or B2F_OUT_FULL (b2f_scored_full records: needs an attached outlier forest)
  *   chunk_rows : rows per pipeline chunk (0 = choose: ~8 chunks for large requests)
  * Returns the number of chunks (>= 0) or a negative error.  Results appear in the scorer's pinned result buffer
  * (b2f_scorer_results) chunk by chunk; b2f_scorer_wait(chunk) blocks until that chunk is there.  The column buffers must stay
@@ -430,13 +415,13 @@ extern "C" int b2f_scorer_trace(const b2f_scorer *s, double *out, int max_chunks
 extern "C" int b2f_scorer_start(b2f_scorer *s, int64_t n, const b2f_str_column *cat_cols, const double *const *num_cols, const int64_t *num_strides,
                                 int row_format, int out_mode, int64_t chunk_rows) {
     if (!s || n < 0) return set_err(B2F_EINVAL, "bad argument");
-    if (out_mode != 0 && out_mode != 1 && out_mode != 3) return set_err(B2F_EINVAL, "out_mode must be 0, 1 or 3");
+    if (out_mode == B2F_OUT_PAIRS) return set_err(B2F_EINVAL, "out_mode must be B2F_OUT_F32, B2F_OUT_F64 or B2F_OUT_FULL");
     int rcf = check_row_format(s->m, row_format);
     if (rcf) return rcf;
     if (row_format == B2F_ROWS_RANKED && !s->e->ranker) return set_err(B2F_ESTATE, "the encoder has no ranker attached (b2f_encoder_attach_ranker)");
     if (row_format == B2F_ROWS_PACKED64 && !s->e->packed_ok) return set_err(B2F_EINVAL, "schema does not fit the packed row");
-    if (out_mode == 3 && !s->m->outlier) return set_err(B2F_ESTATE, "no outlier forest attached");
-    if (out_mode == 3 && row_format == B2F_ROWS_RANKED) return set_err(B2F_EINVAL, "full records need float32 rows");
+    rcf = out_check(s->m, out_mode, row_format, true); /* the results go to the scorer's own buffer */
+    if (rcf) return rcf;
     if (n == 0) {
         s->n = 0;
         s->n_chunks = 0;
@@ -488,8 +473,6 @@ extern "C" int b2f_scorer_start(b2f_scorer *s, int64_t n, const b2f_str_column *
     s->n_chunks = n_chunks;
     s->row_format = row_format;
     s->out_mode = out_mode;
-    s->row_bytes = row_bytes_of(s->m, row_format);
-    s->out_bytes = out_mode == 3 ? sizeof(b2f_scored_full) : (out_mode == 1 ? sizeof(double) : sizeof(float));
     s->cats = cat_cols;
     s->nums = num_cols;
     s->strides = num_strides;

@@ -13,7 +13,10 @@ import os
 import numpy as np
 
 from . import _cabi
-from ._cabi import MOMENT_VALUES, PACKED_ROW_WORDS, ROW_WORDS, ROWS_PACKED64, ROWS_RANKED, ROWS_WORDS24, B2FError, Info, PinnedBuffer, RankInfo, check, ptr
+from ._cabi import (
+    MOMENT_VALUES, OUT_F32, OUT_F64, OUT_FULL, OUT_PAIRS, PACKED_ROW_WORDS, ROW_WORDS, ROWS_PACKED64, ROWS_RANKED, ROWS_WORDS24, B2FError, Info,
+    PinnedBuffer, RankInfo, check, ptr,
+)
 from .flatten import FlatForest
 
 
@@ -159,7 +162,7 @@ class ForestEngine:
         """Asynchronous ``predict_pairs`` on pinned buffers (``out``: SCORED_DTYPE); pair with wait()."""
         t = C.c_uint64(0)
         check(
-            self._lib.b2f_predict_async_ex(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(out), 2, None, C.byref(t)),
+            self._lib.b2f_predict_async_ex(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(out), OUT_PAIRS, None, C.byref(t)),
             "b2f_predict_async_ex",
         )
         return t.value
@@ -298,7 +301,7 @@ class Scorer:
         except Exception:
             pass
 
-    def start(self, n: int, columns, out_mode: int = 1, chunk_rows: int = 0, fmt: int | None = None) -> int:
+    def start(self, n: int, columns, out_mode: int = OUT_F64, chunk_rows: int = 0, fmt: int | None = None) -> int:
         """``columns``: what ``RowEncoder.frame_columns`` returned.  -> number of chunks."""
         scol, ptrs, strides, _keep = columns
         if fmt is None:
@@ -334,7 +337,7 @@ class Scorer:
 
     def results(self) -> np.ndarray:
         """View over the pinned result buffer of the current job (valid until the next ``start``)."""
-        dt = {0: np.dtype(np.float32), 1: np.dtype(np.float64), 3: _cabi.SCORED_FULL_DTYPE}[self._mode]
+        dt = {OUT_F32: np.dtype(np.float32), OUT_F64: np.dtype(np.float64), OUT_FULL: _cabi.SCORED_FULL_DTYPE}[self._mode]
         addr = self._lib.b2f_scorer_results(self._h)
         buf = (C.c_uint8 * (self._n * dt.itemsize)).from_address(addr)
         return np.frombuffer(buf, dtype=dt, count=self._n)
@@ -408,7 +411,7 @@ class EngineGroup:
         if out is None:
             out = np.empty(n, dtype=_cabi.SCORED_FULL_DTYPE)
         check(
-            self._lib.b2f_predict_multi_ex(self._handles, len(self.engines), ptr(rows), n, self.engines[0]._fmt(rows), ptr(out), 3, None),
+            self._lib.b2f_predict_multi_ex(self._handles, len(self.engines), ptr(rows), n, self.engines[0]._fmt(rows), ptr(out), OUT_FULL, None),
             "b2f_predict_multi_ex",
         )
         return out

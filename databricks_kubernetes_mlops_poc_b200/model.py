@@ -26,6 +26,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pandas as pd
 
+from ._cabi import OUT_F64, OUT_FULL
 from ._pylists import ListBuilder
 from .encode import RowEncoder
 from .engine import EngineGroup, ForestEngine
@@ -171,7 +172,7 @@ class B200Model:
         t1 = time.perf_counter()
         # classifier only: the scorer's own choice (64-byte float32 rows: cheapest to encode; ranked rows with B200_SCORER_ROWS=ranked);
         # with the outlier forest on the same rows: float32 rows (ranks are relative to ONE forest's split values)
-        n_chunks = sc.start(n, cols, out_mode=3 if full else 1, fmt=(1 if self.encoder.packed_ok else 0) if full else None)
+        n_chunks = sc.start(n, cols, out_mode=OUT_FULL if full else OUT_F64, fmt=(1 if self.encoder.packed_ok else 0) if full else None)
         out = sc.results()
         bounds = sc.bounds
         # Python lists are built chunk by chunk while later chunks are in flight (float objects recycled: _pylists.py); what does
@@ -258,7 +259,7 @@ class _Replica:
             # the columnar request pipeline (csrc/scorer.h): column buffers -> encode threads -> H2D -> kernel(s) -> D2H
             if self.has_outlier:
                 _reject_nan(df, self.numeric_features)
-            n_chunks = sc.start(n, cols, out_mode=3 if self.has_outlier else 1,
+            n_chunks = sc.start(n, cols, out_mode=OUT_FULL if self.has_outlier else OUT_F64,
                                 fmt=(1 if self.encoder.packed_ok else 0) if self.has_outlier else None)
             for c in range(n_chunks):  # chunks ride different streams: each has its own completion event
                 sc.wait(c)

@@ -84,6 +84,13 @@ extern "C" {
 typedef struct b2f_model b2f_model;
 typedef uint64_t b2f_ticket;
 
+/* output kinds of the host-buffer entry points (the `proba_is_f64` argument of b2f_predict_async_ex, b2f_predict_multi_ex and
+ * b2f_predict_stream, the `out_mode` of b2f_scorer_start): what one output row looks like */
+#define B2F_OUT_F32 0   /* float proba1 (+ optional int32 label array) */
+#define B2F_OUT_F64 1   /* double proba1 (+ optional int32 label array) */
+#define B2F_OUT_PAIRS 2 /* b2f_scored records (label argument ignored) */
+#define B2F_OUT_FULL 3  /* b2f_scored_full records (needs an attached outlier forest; float32 row formats only) */
+
 /* one scored row, for b2f_predict_pairs: both results of a row side by side, so a chunk comes back in
  * ONE device-to-host copy instead of two */
 typedef struct b2f_scored {
@@ -259,7 +266,7 @@ int b2f_bind_caller_near(int device);
 /* NUMA node of a GPU (-1: not exposed) and the number of logical CPUs of that node this process may use */
 int b2f_device_numa_node(int device, int *n_cpus);
 void b2f_scorer_destroy(b2f_scorer *s);
-/* out_mode: 0 = float proba1, 1 = double proba1, 3 = b2f_scored_full records (attached outlier forest; float32 row formats only).
+/* out_mode: B2F_OUT_F32, B2F_OUT_F64 or B2F_OUT_FULL (B2F_OUT_PAIRS is not accepted here).
  * chunk_rows 0 = choose.  Returns the number of chunks (>= 0) or a negative error; one job at a time per scorer; the column
  * buffers must stay valid until the last chunk has been waited for. */
 int b2f_scorer_start(b2f_scorer *s, int64_t n, const b2f_str_column *cat_cols, const double *const *num_cols, const int64_t *num_strides,
@@ -304,8 +311,8 @@ int b2f_predict_full(b2f_model *m, const void *rows, int64_t n, int row_format, 
  * b2f_wait(ticket) returns.  proba_is_f64 selects double (1) or float (0) outputs. */
 int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned,
                       int proba_is_f64, int32_t *label_pinned, b2f_ticket *ticket);
-/* proba_is_f64: 0 = float, 1 = double, 2 = proba1_pinned points at b2f_scored records (label_pinned ignored),
- * 3 = proba1_pinned points at b2f_scored_full records (needs an attached outlier forest) */
+/* proba_is_f64: an output kind, B2F_OUT_F32 / B2F_OUT_F64, or B2F_OUT_PAIRS / B2F_OUT_FULL (proba1_pinned points at
+ * records, label_pinned is ignored) */
 int b2f_predict_async_ex(b2f_model *m, const void *rows_pinned, int64_t n, int row_format,
                          void *proba1_pinned, int proba_is_f64, int32_t *label_pinned,
                          b2f_ticket *ticket);
@@ -316,12 +323,13 @@ int b2f_wait(b2f_model *m, b2f_ticket ticket);
 int b2f_predict_multi(b2f_model **models, int n_models, const void *rows, int64_t n, void *proba1,
                       int proba_is_f64, int32_t *label);
 
-/* proba_is_f64 as for b2f_predict_async_ex (2 / 3: proba1 points at b2f_scored / b2f_scored_full records) */
+/* proba_is_f64: an output kind, as for b2f_predict_async_ex */
 int b2f_predict_multi_ex(b2f_model **models, int n_models, const void *rows, int64_t n, int row_format,
                          void *proba1, int proba_is_f64, int32_t *label);
 
 /* a long stream of rows in `batch`-row batches dealt round-robin: batch b -> models[b % n_models]; one host thread
- * per GPU inside the call, at most `inflight` (1..8) batches in flight per GPU; buffers should be pinned */
+ * per GPU inside the call, at most `inflight` (1..8) batches in flight per GPU; buffers should be pinned.
+ * proba_is_f64: an output kind, as for b2f_predict_async_ex */
 int b2f_predict_stream(b2f_model **models, int n_models, const void *rows, int64_t n, int64_t batch, int row_format,
                        void *proba1, int proba_is_f64, int32_t *label, int inflight);
 
@@ -361,6 +369,8 @@ void b2f_device_free(b2f_model *m, void *dptr);
 int b2f_copy_h2d(b2f_model *m, void *dst_dev, const void *src_host, size_t nbytes);
 int b2f_copy_d2h(b2f_model *m, void *dst_host, const void *src_dev, size_t nbytes);
 /* enqueue one predict launch on the model's compute stream (asynchronous).
+ * proba_is_f64 of the device-resident entry points (here and in the timed forms below) is a flag, not an output kind:
+ * non-zero = double proba1 (B2F_OUT_F64), zero = float (B2F_OUT_F32); they write no records.
  * Ordering (b2f_predict_device_ex and b2f_predict_stream_timed_ex alike): consecutive calls on one model's compute stream
  * take effect in call order -- when several write the same proba / label buffer, the last call's values are what is left.
  * With B2F_ROWS_RANKED rows, back-to-back launches overlap (programmatic dependent launch): a launch may read its rows

@@ -437,25 +437,42 @@ def test_split_kernel_small_batches(curated, adversarial, rf100d6, rf500d8, gbdt
         eng.close()
 
 
-def test_stream_dealer(curated, rf100d6):
+def test_stream_dealer(curated, iforest, rf100d6):
     """b2f_predict_stream: batches dealt round-robin over the models (one host thread per GPU inside the call)."""
-    from databricks_kubernetes_mlops_poc_b200 import flatten, training
+    from databricks_kubernetes_mlops_poc_b200 import _cabi, flatten, training
     from databricks_kubernetes_mlops_poc_b200.encode import RowEncoder
     from databricks_kubernetes_mlops_poc_b200.engine import EngineGroup, device_count
 
     flat = flatten.flatten_pipeline(rf100d6)
     enc = RowEncoder(flat)
     grp = EngineGroup(flat, devices=list(range(min(2, device_count()))))
+    n = 50_003
+    _, codes, nums = training.synth_arrays(curated, n, seed=9)
+    rows = enc.encode_arrays_packed(codes, nums)
     try:
-        n = 50_003
-        _, codes, nums = training.synth_arrays(curated, n, seed=9)
-        rows = enc.encode_arrays_packed(codes, nums)
         want_p, want_l = grp.engines[0].predict_rows(rows, np.float32)
         for batch, inflight in ((4096, 2), (65536, 1), (1000, 8)):
             p = np.full(n, -1, dtype=np.float32)
             l = np.full(n, -1, dtype=np.int32)
             grp.predict_stream(rows, batch, p, l, inflight=inflight)
             assert (p == want_p).all() and (l == want_l).all()
+    finally:
+        grp.close()
+    # records through the C ABI, dealt over two replicas (both on GPU 0 when it is the only one); 4 096 does not divide n, so
+    # every batch has to land at its own record offset.  The expected records come from one engine, batch by batch, so that
+    # each batch takes the same kernel (and float64 summation order) as in the stream.
+    grp = EngineGroup(flat, devices=[0, 1] if device_count() >= 2 else [0, 0])
+    try:
+        grp.attach_outlier_forest(flatten.flatten_isolation_forest(iforest, 9, 14, threshold=0.0))
+        one, batch = grp.engines[0], 4096
+        for kind, score in ((_cabi.OUT_PAIRS, one.predict_pairs), (_cabi.OUT_FULL, one.predict_full)):
+            want = np.concatenate([score(rows[lo:lo + batch]) for lo in range(0, n, batch)])
+            out = np.zeros(n, dtype=want.dtype)
+            _cabi.check(grp._lib.b2f_predict_stream(grp._handles, 2, _cabi.ptr(rows), n, batch, _cabi.ROWS_PACKED64, _cabi.ptr(out), kind, None, 2),
+                        "b2f_predict_stream")
+            for field in ("proba1", "label", "is_outlier", "outlier_score"):  # every field the kernels write
+                if field in want.dtype.names:
+                    assert (out[field] == want[field]).all(), (kind, field)
     finally:
         grp.close()
 
