@@ -19,6 +19,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <string>
 #include <thread>
 #include <new>
@@ -31,6 +32,7 @@
 #include "forest_predict_tile.cuh"
 #include "forest_predict_rank.cuh"
 #include "forest_rank.h"
+#include "tree_shap.cuh"
 #include "json_rows.h"
 #include "row_encoder.h"
 
@@ -122,6 +124,26 @@ struct Slot {
     int64_t cap_rows = 0;
 };
 
+/* device buffers of one stream's explain launches: phi rows and the per-range partial sums (tree_shap.cuh) */
+struct ExplainBuf {
+    double *out = nullptr;
+    int64_t out_rows = 0;
+    double *scratch = nullptr;
+    size_t scratch_bytes = 0;
+};
+
+/* an attached path table (b2f_model_attach_explainer) */
+struct Explainer {
+    b2f_paths_header hdr;
+    void *d_table = nullptr;
+    SParams sp;
+    int maxl = 9;        /* length bucket of k_tree_shap: 9, 16 or 24 */
+    int smem_bytes = 0;
+    int ctas_per_sm = 1; /* resident k_tree_shap CTAs per SM */
+    ExplainBuf slots[B2F_STREAMS];
+    ExplainBuf compute; /* b2f_explain_device */
+};
+
 struct TicketRec {
     uint64_t id = 0;
     cudaEvent_t ev[B2F_STREAMS] = {nullptr, nullptr, nullptr, nullptr};
@@ -164,6 +186,7 @@ struct b2f_model {
     int64_t launches_rank = 0;
     void *d_blob = nullptr;
     int64_t forest_bytes = 0;
+    Explainer *ex = nullptr; /* attached TreeSHAP path table (b2f_model_attach_explainer) */
     b2f_model *outlier = nullptr; /* attached isolation forest (b2f_model_attach_outlier_forest): a child handle on the
                                      same device whose kernels are launched on this handle's streams and rows */
     Slot slots[B2F_STREAMS];
@@ -771,6 +794,14 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
     cudaSetDevice(m->device);
     cudaDeviceSynchronize();
     if (m->outlier) b2f_model_destroy(m->outlier);
+    if (m->ex) {
+        for (ExplainBuf *b = m->ex->slots; b <= &m->ex->compute; ++b) {
+            if (b->out) cudaFree(b->out);
+            if (b->scratch) cudaFree(b->scratch);
+        }
+        if (m->ex->d_table) cudaFree(m->ex->d_table);
+        delete m->ex;
+    }
     if (m->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(m->comm);
     for (int s = 0; s < B2F_STREAMS; ++s) {
         Slot &sl = m->slots[s];
@@ -1010,6 +1041,95 @@ static int out_launch(b2f_model *m, cudaStream_t st, const void *rows_dev, int64
     return launch_predict(m->outlier, st, rows_dev, n, fmt, false, rec + 16, reinterpret_cast<int32_t *>(rec + 12), B2F_OSTRIDE(6, 6));
 }
 
+/* ------------------------------------------------------------------ explanations (K5: tree_shap.cuh, forest_paths.h)
+ * B2F_OUT_EXPLAIN is an output kind of the host pipeline only: b2f_explain passes it to enqueue_host_batch, so explanations
+ * ride the same chunking, slots and streams as scores.  It is not a B2F_OUT_* value: out_row_bytes does not know it, so the
+ * predict entry points refuse it. */
+#define B2F_OUT_EXPLAIN 16
+
+static int explain_fields(const b2f_model *m) { return (int)(m->hdr.n_cat + m->hdr.n_num); }
+
+static int explain_check(const b2f_model *m, int fmt, bool have_out) {
+    if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
+    if (fmt == B2F_ROWS_RANKED)
+        return set_err(B2F_EINVAL, "explanations take float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
+    if (!have_out) return set_err(B2F_EINVAL, "phi is NULL");
+    return B2F_OK;
+}
+
+/* row tiles x path ranges of one launch: one range from a full grid of row tiles up; below, enough ranges to fill every SM
+ * (at least two paths per warp).  The partials of several ranges take ranges * n * fields doubles; since ranges > 1 only when
+ * tiles < target, that is below 2 * target * 32 rows' worth: bounded by the GPU, not by n or the number of paths. */
+static int64_t explain_ranges(const b2f_model *m, int64_t n) {
+    const int64_t tiles = (n + 31) / 32, target = (int64_t)m->sm_count * m->ex->ctas_per_sm;
+    int64_t r = tiles >= target ? 1 : (target + tiles - 1) / tiles;
+    r = std::min<int64_t>(r, std::max<int64_t>(1, (int64_t)m->ex->hdr.n_paths / (2 * B2F_SHAP_WARPS)));
+    return std::max<int64_t>(1, std::min<int64_t>(r, 65535));
+}
+
+static int explain_reserve_scratch(ExplainBuf &b, cudaStream_t st, size_t bytes) {
+    if (bytes <= b.scratch_bytes) return B2F_OK;
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (b.scratch) cudaFree(b.scratch);
+    b.scratch = nullptr;
+    b.scratch_bytes = 0;
+    CUDA_TRY(cudaMalloc((void **)&b.scratch, bytes));
+    b.scratch_bytes = bytes;
+    return B2F_OK;
+}
+
+template <int MAXL>
+static auto shap_kernel(bool pk) {
+    return pk ? k_tree_shap<MAXL, true> : k_tree_shap<MAXL, false>;
+}
+static auto shap_kernel_for(int maxl, bool pk) {
+    return maxl <= 9 ? shap_kernel<9>(pk) : (maxl <= 16 ? shap_kernel<16>(pk) : shap_kernel<24>(pk));
+}
+
+/* phi_dev[n][fields] for n device rows of format fmt, on stream st, partial sums in b's scratch */
+static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, double *phi_dev, ExplainBuf &b) {
+    if (n <= 0) return B2F_OK;
+    const Explainer &ex = *m->ex;
+    const int F = explain_fields(m);
+    if (ex.hdr.n_paths == 0) { /* every tree a single leaf: nothing moves away from base_value */
+        CUDA_TRY(cudaMemsetAsync(phi_dev, 0, (size_t)n * F * sizeof(double), st));
+        return B2F_OK;
+    }
+    const int64_t ranges = explain_ranges(m, n);
+    if (ranges > 1) {
+        int rc = explain_reserve_scratch(b, st, (size_t)ranges * (size_t)n * F * sizeof(double));
+        if (rc) return rc;
+    }
+    const dim3 grid((unsigned)((n + 31) / 32), (unsigned)ranges);
+    shap_kernel_for(ex.maxl, fmt == B2F_ROWS_PACKED64)<<<grid, B2F_SHAP_THREADS, ex.smem_bytes, st>>>(
+        ex.sp, static_cast<const uint32_t *>(rows_dev), (long long)n, phi_dev, b.scratch);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_tree_shap launch failed: %s", cudaGetErrorString(e));
+    m->launches++;
+    if (ranges > 1) {
+        const int64_t values = n * F;
+        const unsigned blocks = (unsigned)std::min<int64_t>((values + 255) / 256, (int64_t)m->sm_count * 8);
+        k_tree_shap_finish<<<blocks, 256, 0, st>>>(b.scratch, (int)ranges, (long long)values, ex.hdr.denom, phi_dev);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_tree_shap_finish launch failed: %s", cudaGetErrorString(e));
+        m->launches++;
+    }
+    return B2F_OK;
+}
+
+/* the phi buffer of one slot's chunk */
+static int explain_reserve_out(b2f_model *m, ExplainBuf &b, cudaStream_t st, int64_t rows) {
+    if (rows <= b.out_rows) return B2F_OK;
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (b.out) cudaFree(b.out);
+    b.out = nullptr;
+    b.out_rows = 0;
+    const int64_t cap = std::max<int64_t>(rows, 1024);
+    CUDA_TRY(cudaMalloc((void **)&b.out, (size_t)cap * explain_fields(m) * sizeof(double)));
+    b.out_rows = cap;
+    return B2F_OK;
+}
+
 /* ------------------------------------------------------------------ host-buffer pipeline */
 static int slot_reserve(b2f_model *m, Slot &sl, int64_t rows) {
     if (rows <= sl.cap_rows) return B2F_OK;
@@ -1043,16 +1163,21 @@ static int submit_chunk(b2f_model *m, Slot &sl, const void *rows, int fmt, int k
         marks->push_back(e);
     };
     if (marks && marks->empty()) mark();
-    const size_t row_bytes = row_bytes_of(m, fmt), out_bytes = out_row_bytes(kind);
+    const bool explain = kind == B2F_OUT_EXPLAIN;
+    ExplainBuf *eb = explain ? &m->ex->slots[&sl - m->slots] : nullptr;
+    if (explain && (rc = explain_reserve_out(m, *eb, sl.stream, cnt))) return rc;
+    void *d_out = explain ? static_cast<void *>(eb->out) : sl.d_proba;
+    const size_t row_bytes = row_bytes_of(m, fmt), out_bytes = explain ? explain_fields(m) * sizeof(double) : out_row_bytes(kind);
     const bool records = kind == B2F_OUT_PAIRS || kind == B2F_OUT_FULL;
     CUDA_TRY(cudaMemcpyAsync(sl.d_rows, static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, (size_t)cnt * row_bytes, cudaMemcpyHostToDevice,
                              sl.stream));
     mark();
-    rc = out_launch(m, sl.stream, sl.d_rows, cnt, fmt, kind, out ? sl.d_proba : nullptr, label ? sl.d_label : nullptr);
+    rc = explain ? launch_explain(m, sl.stream, sl.d_rows, cnt, fmt, eb->out, *eb)
+                 : out_launch(m, sl.stream, sl.d_rows, cnt, fmt, kind, out ? sl.d_proba : nullptr, label ? sl.d_label : nullptr);
     if (rc) return rc;
     mark();
     if (out)
-        CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(out) + (size_t)lo * out_bytes, sl.d_proba, (size_t)cnt * out_bytes, cudaMemcpyDeviceToHost,
+        CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(out) + (size_t)lo * out_bytes, d_out, (size_t)cnt * out_bytes, cudaMemcpyDeviceToHost,
                                  sl.stream));
     if (label && !records) CUDA_TRY(cudaMemcpyAsync(label + lo, sl.d_label, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, sl.stream));
     mark();
@@ -1064,7 +1189,7 @@ static int submit_chunk(b2f_model *m, Slot &sl, const void *rows, int fmt, int k
 static int enqueue_host_batch(b2f_model *m, const void *rows, int64_t n, int fmt, void *out, int kind, int32_t *label, uint32_t *used_mask) {
     *used_mask = 0;
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
-    int rc = out_check(m, kind, fmt, out || n == 0);
+    int rc = kind == B2F_OUT_EXPLAIN ? explain_check(m, fmt, out || n == 0) : out_check(m, kind, fmt, out || n == 0);
     if (rc) return rc;
     if (n == 0) return B2F_OK;
     if (!rows) return set_err(B2F_EINVAL, "rows is NULL");
@@ -1157,6 +1282,190 @@ extern "C" int b2f_model_attach_outlier_forest(b2f_model *m, const void *forest_
 
 extern "C" int b2f_predict_full(b2f_model *m, const void *rows, int64_t n, int row_format, b2f_scored_full *out) {
     return predict_host(m, rows, n, row_format, out, B2F_OUT_FULL, nullptr);
+}
+
+/* ------------------------------------------------------------------ explainer: path table check, attach, explain */
+static int validate_paths(const uint8_t *t, size_t nbytes, b2f_paths_header *hdr_out) {
+    if (!t || nbytes < sizeof(b2f_paths_header)) return set_err(B2F_EINVAL, "path table too small (%zu bytes)", nbytes);
+    b2f_paths_header h;
+    memcpy(&h, t, sizeof(h));
+    if (memcmp(h.magic, B2F_PATHS_MAGIC, 8) != 0) return set_err(B2F_EINVAL, "path table: bad magic");
+    if (h.version != B2F_PATHS_VERSION) return set_err(B2F_EINVAL, "path table: version %u, expected %u", h.version, B2F_PATHS_VERSION);
+    if (h.header_bytes != B2F_PATHS_HEADER_BYTES) return set_err(B2F_EINVAL, "path table: header_bytes=%u unsupported", h.header_bytes);
+    if (h.agg_mode != B2F_AGG_RF_MEAN && h.agg_mode != B2F_AGG_GBDT_LOGISTIC)
+        return set_err(B2F_EINVAL, "path table: agg_mode %u (only RandomForest and GBDT classifiers are explained)", h.agg_mode);
+    if (h.n_cat + h.n_num > B2F_SENTINEL_WORD || h.n_cat + h.n_num == 0)
+        return set_err(B2F_EINVAL, "path table: n_cat+n_num=%u out of range [1,%u]", h.n_cat + h.n_num, B2F_SENTINEL_WORD);
+    if (h.n_trees == 0 || h.n_trees > B2F_MAX_TREES) return set_err(B2F_EINVAL, "path table: n_trees=%u out of range", h.n_trees);
+    if (h.max_len > B2F_PATHS_MAX_LEN) return set_err(B2F_EINVAL, "path table: max_len=%u exceeds %u", h.max_len, B2F_PATHS_MAX_LEN);
+    if (!(h.denom > 0.0) || !std::isfinite(h.base_value)) return set_err(B2F_EINVAL, "path table: bad denom or base_value");
+    const uint64_t elems_off = (h.paths_off + (uint64_t)h.n_paths * sizeof(b2f_path) + 15) / 16 * 16;
+    if (h.paths_off != B2F_PATHS_HEADER_BYTES || h.elems_off != elems_off || h.total_bytes != nbytes ||
+        h.elems_off + (uint64_t)h.n_elems * sizeof(b2f_path_elem) != nbytes)
+        return set_err(B2F_EINVAL, "path table: sections do not match its size (%zu bytes; truncated?)", nbytes);
+    const b2f_path *P = reinterpret_cast<const b2f_path *>(t + h.paths_off);
+    const b2f_path_elem *E = reinterpret_cast<const b2f_path_elem *>(t + h.elems_off);
+    const uint32_t F = h.n_cat + h.n_num;
+    uint64_t next = 0;
+    uint32_t longest = 0;
+    for (uint32_t p = 0; p < h.n_paths; ++p) {
+        b2f_path pr;
+        memcpy(&pr, &P[p], sizeof(pr));
+        if (pr.first != next || pr.len < 2 || pr.len > h.max_len || (uint64_t)pr.first + pr.len > h.n_elems || pr.tree >= h.n_trees ||
+            !std::isfinite(pr.leaf))
+            return set_err(B2F_EINVAL, "path table: path %u malformed (first %u, len %u)", p, pr.first, pr.len);
+        next += pr.len;
+        longest = std::max(longest, pr.len);
+        uint32_t seen = 0;
+        for (uint32_t k = 0; k < pr.len; ++k) {
+            b2f_path_elem e;
+            memcpy(&e, &E[pr.first + k], sizeof(e));
+            if (k == 0) {
+                if (e.field != B2F_PATH_BIAS_FIELD || e.kind != B2F_PE_BIAS) return set_err(B2F_EINVAL, "path table: path %u has no bias element", p);
+                continue;
+            }
+            const bool cat = e.kind == B2F_PE_CAT, num = (e.kind & ~B2F_PE_HAS_HI) == B2F_PE_NUM;
+            if (e.field >= F || (cat && e.field >= h.n_cat) || (num && e.field < h.n_cat) || !(cat || num))
+                return set_err(B2F_EINVAL, "path table: path %u element %u: field %u / kind %u invalid", p, k, e.field, e.kind);
+            if (seen & (1u << e.field)) return set_err(B2F_EINVAL, "path table: path %u tests field %u twice (elements must be merged)", p, e.field);
+            seen |= 1u << e.field;
+            if (!(e.zero_fraction > 0.0 && e.zero_fraction <= 1.0) || !(e.inv_zero_fraction >= 1.0) || !std::isfinite(e.inv_zero_fraction))
+                return set_err(B2F_EINVAL, "path table: path %u element %u: bad zero fraction", p, k);
+        }
+    }
+    if (next != h.n_elems || longest != h.max_len) return set_err(B2F_EINVAL, "path table: element count or max_len inconsistent");
+    *hdr_out = h;
+    return B2F_OK;
+}
+
+extern "C" int b2f_paths_validate(const void *paths, size_t nbytes) {
+    b2f_paths_header h;
+    return validate_paths(static_cast<const uint8_t *>(paths), nbytes, &h);
+}
+
+/* flatten.py blob_fingerprint: sum of splitmix64(w_i ^ i * golden) over the blob's 64-bit words */
+static uint64_t blob_fingerprint(const uint8_t *blob, size_t nbytes) {
+    uint64_t sum = 0;
+    for (size_t i = 0; i < nbytes / 8; ++i) {
+        uint64_t z;
+        memcpy(&z, blob + 8 * i, 8);
+        z ^= (uint64_t)i * 0x9E3779B97F4A7C15ull;
+        z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+        z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+        sum += z ^ (z >> 31);
+    }
+    return sum;
+}
+
+extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_t nbytes) {
+    if (!m) return set_err(B2F_EINVAL, "model is NULL");
+    b2f_paths_header h;
+    int rc = validate_paths(static_cast<const uint8_t *>(paths), nbytes, &h);
+    if (rc) return rc;
+    if (h.n_cat != m->hdr.n_cat || h.n_num != m->hdr.n_num || h.agg_mode != m->hdr.agg_mode || h.n_trees != m->hdr.n_trees)
+        return set_err(B2F_EINVAL, "path table: shape (%u cat, %u num, agg %u, %u trees) differs from the model's (%u, %u, %u, %u)", h.n_cat, h.n_num,
+                       h.agg_mode, h.n_trees, m->hdr.n_cat, m->hdr.n_num, m->hdr.agg_mode, m->hdr.n_trees);
+    CUDA_TRY(cudaSetDevice(m->device));
+    std::vector<uint8_t> blob(m->hdr.total_bytes);
+    CUDA_TRY(cudaMemcpy(blob.data(), m->d_blob, blob.size(), cudaMemcpyDeviceToHost));
+    if (blob_fingerprint(blob.data(), blob.size()) != h.fingerprint)
+        return set_err(B2F_EINVAL, "path table: built from another forest (fingerprint mismatch)");
+    /* replacing an explainer: nothing may still read the old table.  Waited for before anything new is allocated, so a
+     * failure here leaves the model as it was and leaks nothing. */
+    if (m->ex) CUDA_TRY(cudaDeviceSynchronize());
+    Explainer *ex = new (std::nothrow) Explainer();
+    if (!ex) return set_err(B2F_ENOMEM, "out of host memory");
+    auto fail = [&](int code) {
+        if (ex->d_table) cudaFree(ex->d_table);
+        delete ex;
+        return code;
+    };
+    ex->hdr = h;
+    if (cudaMalloc(&ex->d_table, nbytes) != cudaSuccess || cudaMemcpy(ex->d_table, paths, nbytes, cudaMemcpyHostToDevice) != cudaSuccess)
+        return fail(set_err(B2F_ENOMEM, "path table upload (%zu bytes) failed: %s", nbytes, cudaGetErrorString(cudaGetLastError())));
+    SParams &sp = ex->sp;
+    memset(&sp, 0, sizeof(sp));
+    sp.paths = reinterpret_cast<const b2f_path *>(static_cast<uint8_t *>(ex->d_table) + h.paths_off);
+    sp.elems = reinterpret_cast<const b2f_path_elem *>(static_cast<uint8_t *>(ex->d_table) + h.elems_off);
+    sp.n_paths = (int)h.n_paths;
+    sp.n_cat = (int)h.n_cat;
+    sp.n_num = (int)h.n_num;
+    sp.denom = h.denom;
+    memcpy(sp.impute, m->hdr.impute, sizeof(sp.impute));
+    ex->maxl = h.max_len <= 9 ? 9 : (h.max_len <= 16 ? 16 : 24);
+    ex->smem_bytes = shap_smem_bytes((int)(h.n_cat + h.n_num));
+    /* the EXTEND / UNWIND factors (no division in the kernel) */
+    double tab[4][B2F_SHAP_TAB_L][B2F_SHAP_TAB_L]; /* per call: concurrent attaches (other handles) share nothing on the host */
+    for (int l = 0; l < B2F_SHAP_TAB_L; ++l)
+        for (int i = 0; i < B2F_SHAP_TAB_L; ++i) {
+            tab[0][l][i] = (i + 1.0) / (l + 1.0);
+            tab[1][l][i] = (l - i) / (l + 1.0);
+            tab[2][l][i] = (l + 1.0) / (i + 1.0);
+            tab[3][l][i] = l > i ? (l + 1.0) / (l - i) : 0.0;
+        }
+    cudaError_t e = cudaMemcpyToSymbol(c_shap_tab, tab, sizeof(tab));
+    for (bool pk : {false, true})
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(shap_kernel_for(ex->maxl, pk), cudaFuncAttributeMaxDynamicSharedMemorySize, ex->smem_bytes);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ex->ctas_per_sm, shap_kernel_for(ex->maxl, false), B2F_SHAP_THREADS, ex->smem_bytes);
+    if (e != cudaSuccess) return fail(set_err(B2F_ECUDA, "explainer set-up failed: %s", cudaGetErrorString(e)));
+    ex->ctas_per_sm = std::max(1, ex->ctas_per_sm);
+    if (m->ex) { /* the device was synchronised above */
+        for (ExplainBuf *b = m->ex->slots; b <= &m->ex->compute; ++b) {
+            if (b->out) cudaFree(b->out);
+            if (b->scratch) cudaFree(b->scratch);
+        }
+        cudaFree(m->ex->d_table);
+        delete m->ex;
+    }
+    m->ex = ex;
+    return B2F_OK;
+}
+
+extern "C" int b2f_explain(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi, double *base_value, float *device_ms) {
+    if (!m) return set_err(B2F_EINVAL, "model is NULL");
+    if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
+    if (base_value) *base_value = m->ex->hdr.base_value;
+    if (device_ms) *device_ms = 0.0f;
+    CUDA_TRY(cudaSetDevice(m->device));
+    struct Events { /* destroyed on every return path */
+        cudaEvent_t e[1 + B2F_STREAMS] = {};
+        ~Events() {
+            for (cudaEvent_t x : e)
+                if (x) cudaEventDestroy(x);
+        }
+    } evs;
+    cudaEvent_t *ev = evs.e;
+    const int first = (int)(m->next_slot % B2F_STREAMS);
+    if (device_ms && n > 0) {
+        for (int i = 0; i <= B2F_STREAMS; ++i) CUDA_TRY(cudaEventCreate(&ev[i]));
+        CUDA_TRY(cudaEventRecord(ev[0], m->slots[first].stream));
+    }
+    uint32_t mask = 0;
+    int rc = enqueue_host_batch(m, rows, n, row_format, phi, B2F_OUT_EXPLAIN, nullptr, &mask);
+    if (device_ms && n > 0 && rc == B2F_OK)
+        for (int s = 0; s < B2F_STREAMS && rc == B2F_OK; ++s)
+            if ((mask & (1u << s)) && cudaEventRecord(ev[1 + s], m->slots[s].stream) != cudaSuccess)
+                rc = set_err(B2F_ECUDA, "cudaEventRecord failed: %s", cudaGetErrorString(cudaGetLastError()));
+    int rc2 = sync_mask(m, mask); /* always: the chunks already enqueued write into the caller's phi */
+    if (rc == B2F_OK) rc = rc2;
+    if (device_ms && n > 0)
+        for (int s = 0; s < B2F_STREAMS && rc == B2F_OK; ++s)
+            if (mask & (1u << s)) {
+                float ms = 0.0f;
+                CUDA_TRY(cudaEventElapsedTime(&ms, ev[0], ev[1 + s]));
+                *device_ms = std::max(*device_ms, ms);
+            }
+    return rc;
+}
+
+extern "C" int b2f_explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev) {
+    if (!m) return set_err(B2F_EINVAL, "model is NULL");
+    if (n < 0) return set_err(B2F_EINVAL, "negative row count");
+    int rc = explain_check(m, row_format, phi_dev != nullptr || n == 0);
+    if (rc == B2F_OK) rc = check_row_format(m, row_format);
+    if (rc) return rc;
+    CUDA_TRY(cudaSetDevice(m->device));
+    return launch_explain(m, m->compute, rows_dev, n, row_format, phi_dev, m->ex->compute);
 }
 
 extern "C" int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned, int proba_is_f64,

@@ -27,6 +27,12 @@ def device_count() -> int:
     return n
 
 
+def validate_paths(blob: bytes) -> None:
+    """Structural check of a TreeSHAP path table (no GPU needed); raises B2FError when malformed."""
+    buf = np.frombuffer(blob, dtype=np.uint8)
+    check(_cabi.load_library().b2f_paths_validate(ptr(buf), buf.size), "b2f_paths_validate")
+
+
 def validate_blob(blob: bytes) -> None:
     """Structural check of a forest blob (no GPU needed); raises B2FError when malformed."""
     buf = np.frombuffer(blob, dtype=np.uint8)
@@ -44,6 +50,7 @@ class ForestEngine:
         if not self._h:
             raise B2FError(f"b2f_model_create(device={device}) failed: {_cabi.last_error()}")
         self._pinned: dict[str, PinnedBuffer] = {}
+        self.explainer_attached = False
         inf = self.info()
         self.rank_words = inf["rank_row_bytes"] // 4 if inf["rank_ok"] else 0  # width of a ranked row, 0 = not available
 
@@ -169,6 +176,29 @@ class ForestEngine:
 
     def wait(self, ticket: int) -> None:
         check(self._lib.b2f_wait(self._h, ticket), "b2f_wait")
+
+    # ------------------------------------------------------------------ explanations (TreeSHAP, csrc/tree_shap.cuh)
+    def attach_explainer(self, blob: bytes) -> None:
+        """Attach a path table (``flatten.flatten_explainer``) built from this engine's forest."""
+        buf = np.frombuffer(blob, dtype=np.uint8)
+        check(self._lib.b2f_model_attach_explainer(self._h, ptr(buf), buf.size), "b2f_model_attach_explainer")
+        self.explainer_attached = True
+
+    def explain_rows(self, rows: np.ndarray, device_ms: bool = False):
+        """Encoded rows (N, 24) or packed (N, 16) -> (phi float64 (N, n_cat + n_num), base_value[, device ms]): exact
+        path-dependent TreeSHAP per request field, in probability (RandomForest) or log-odds (GBDT) space."""
+        rows = np.ascontiguousarray(rows)
+        fmt = self._fmt(rows)
+        n = rows.shape[0]
+        inf = self.info()
+        phi = np.empty((n, inf["n_cat"] + inf["n_num"]), dtype=np.float64)
+        base, ms = C.c_double(0.0), C.c_float(0.0)
+        check(self._lib.b2f_explain(self._h, ptr(rows), n, fmt, ptr(phi), C.byref(base), C.byref(ms)), "b2f_explain")
+        return (phi, base.value, ms.value) if device_ms else (phi, base.value)
+
+    def explain_device(self, rows_dev: int, n: int, phi_dev: int, fmt: int = ROWS_WORDS24) -> None:
+        """Enqueue an explanation of device-resident rows into device phi (n x fields doubles); ``sync`` waits."""
+        check(self._lib.b2f_explain_device(self._h, rows_dev, n, fmt, phi_dev), "b2f_explain_device")
 
     # ------------------------------------------------------------------ device-resident interface
     def device_alloc(self, nbytes: int) -> int:

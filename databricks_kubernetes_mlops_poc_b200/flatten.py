@@ -440,3 +440,200 @@ def parse_header(blob: bytes) -> dict:
         dict(zip(gk, struct.unpack_from(_GROUP_FMT, blob, h["groups_off"] + 32 * g)[:6])) for g in range(h["n_groups"])
     ]
     return h
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Path table for exact TreeSHAP (layout in ``csrc/forest_paths.h``)
+# ---------------------------------------------------------------------------------------------------------------------
+PATHS_MAGIC = b"B2FPATHS"
+PATHS_VERSION = 1
+PATHS_HEADER_BYTES = 256
+PATH_RECORD_BYTES = 24
+PATH_ELEM_BYTES = 48
+PATHS_MAX_LEN = 24  # bias + at most 23 fields
+PE_BIAS, PE_NUM, PE_CAT, PE_HAS_HI = 0, 1, 2, 4
+BIAS_FIELD = 0xFF
+_PATHS_HEADER_FMT = "<8s" + "I" * 10 + "dd" + "Q" * 4  # 96 bytes, padded to 256
+_PATH_RECORD = np.dtype([("first", "<u4"), ("len", "<u4"), ("tree", "<u4"), ("reserved", "<u4"), ("leaf", "<f8")])
+_PATH_ELEM = np.dtype([("field", "<u4"), ("kind", "<u4"), ("lo", "<f4"), ("hi", "<f4"), ("mask", "<u4", (4,)),
+                       ("zero_fraction", "<f8"), ("inv_zero_fraction", "<f8")])
+assert _PATH_RECORD.itemsize == PATH_RECORD_BYTES and _PATH_ELEM.itemsize == PATH_ELEM_BYTES
+
+
+def blob_fingerprint(blob: bytes) -> int:
+    """64-bit fingerprint of a forest blob: sum over its little-endian 64-bit words w_i of splitmix64(w_i ^ i * golden), mod
+    2^64 (``b2f_model_attach_explainer`` computes the same over the model's blob to tie a path table to its forest)."""
+    w = np.frombuffer(blob, dtype="<u8").astype(np.uint64)
+    z = w ^ (np.arange(w.size, dtype=np.uint64) * np.uint64(0x9E3779B97F4A7C15))
+    z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+    z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    z = z ^ (z >> np.uint64(31))
+    return int(z.sum(dtype=np.uint64))
+
+
+def _tree_paths(tree, col_word, col_code, col_is_cat, leaf_value):
+    """One sklearn ``Tree`` -> (per (leaf, ancestor) pair arrays, leaf node ids), vectorised over the tree's leaves.
+
+    Pair k belongs to leaf ``pair_leaf[k]`` (an index into the returned leaves) and says: at ``node``, the path goes to
+    ``child``.  The condition a row must meet there is expressed on the node's request field (``col_word``)."""
+    left = tree.children_left.astype(np.int64)
+    right = tree.children_right.astype(np.int64)
+    cover = tree.weighted_n_node_samples.astype(np.float64)
+    n = left.shape[0]
+    parent = np.full(n, -1, dtype=np.int64)
+    internal = np.nonzero(left != -1)[0]
+    parent[left[internal]] = internal
+    parent[right[internal]] = internal
+    leaves = np.nonzero(left == -1)[0]
+    pair_leaf, pair_node, pair_child = [], [], []
+    cur = leaves.copy()
+    idx = np.arange(leaves.size)
+    while cur.size:
+        p = parent[cur]
+        up = p >= 0
+        cur, idx, p = cur[up], idx[up], p[up]
+        pair_leaf.append(idx)
+        pair_node.append(p)
+        pair_child.append(cur)
+        cur = p
+    pl = np.concatenate(pair_leaf) if pair_leaf else np.zeros(0, np.int64)
+    pn = np.concatenate(pair_node) if pair_node else np.zeros(0, np.int64)
+    pc = np.concatenate(pair_child) if pair_child else np.zeros(0, np.int64)
+    col = tree.feature[pn].astype(np.int64)
+    thr = tree.threshold[pn].astype(np.float64)
+    go_right = pc == right[pn]
+    return dict(leaf=pl, field=col_word[col], is_cat=col_is_cat[col], code=col_code[col], thr=thr, right=go_right,
+                zf=cover[pc] / cover[pn]), leaves, leaf_value[leaves].astype(np.float64), cover
+
+
+def flatten_explainer(pipeline, flat: FlatForest | None = None) -> bytes:
+    """Fitted reference-style Pipeline -> path table for ``b2f_model_attach_explainer`` (layout in ``csrc/forest_paths.h``).
+
+    One path per leaf of every classifier tree, its nodes merged by request field as in GPUTreeShap (Mitchell et al., PeerJ
+    CS 2022): per field the product of ``cover(child) / cover(parent)`` over the path's nodes on it (cover =
+    ``tree_.weighted_n_node_samples``) and the condition a row must meet to follow the path at all of them -- a float32
+    interval ``[lo, hi)`` under the prediction kernels' compare for a numeric field, a 128-bit mask over ``code + 1`` (bit 0 =
+    unknown / missing) for a categorical one.  A categorical field is ONE player however many one-hot columns its nodes
+    test.  ``flat``: the pipeline's ``flatten_pipeline`` result when the caller already has it (its blob is fingerprinted)."""
+    if flat is None:
+        flat = flatten_pipeline(pipeline)
+    pre = pipeline.named_steps["preprocessor"]
+    clf = pipeline.named_steps["classifier"]
+    _, _, categories, _, col_word, col_code, col_is_cat, _, _ = _describe_preprocessor(pre)
+    if any(len(c) > 127 for c in categories):
+        raise NotImplementedError("explanations need categorical fields of at most 127 categories (a 128-bit code mask)")
+    n_cat, n_num = len(flat.cat_features), len(flat.num_features)
+    if flat.agg_mode == AGG_RF_MEAN:
+        trees = [e.tree_ for e in clf.estimators_]
+        denom, init = float(len(trees)), 0.0
+
+        def leaf_values(t):
+            v = t.value[:, 0, :]
+            s = v.sum(axis=1)
+            return v[:, 1] / np.where(s == 0.0, 1.0, s)
+
+    else:
+        trees = [e.tree_ for e in clf.estimators_[:, 0]]
+        denom, init = 1.0, parse_header(flat.blob)["init_raw"]
+        lr = np.float64(clf.learning_rate)
+
+        def leaf_values(t):
+            return lr * t.value[:, 0, 0].astype(np.float64)
+
+    recs, elems, expected = [], [], []
+    n_elems = 0
+    for ti, t in enumerate(trees):
+        pr, leaves, lv, cover = _tree_paths(t, col_word, col_code, col_is_cat, leaf_values(t))
+        # v(empty set) of this tree: every leaf weighted by its cover share
+        expected.append(float(np.dot(lv, cover[leaves] / cover[0])))
+        if pr["leaf"].size == 0:
+            continue  # a single-leaf tree moves only the base value
+        order = np.lexsort((pr["field"], pr["leaf"]))
+        pr = {k: v[order] for k, v in pr.items()}
+        key = pr["leaf"] * 64 + pr["field"]
+        start = np.nonzero(np.r_[True, key[1:] != key[:-1]])[0]
+        # numeric: the left branch needs x < t', the right one x >= t' (or unordered)
+        t32 = strict_upper_f32(pr["thr"])
+        lo = np.where(pr["right"] & ~pr["is_cat"], t32, np.float32(-np.inf)).astype(np.float32)
+        hi = np.where(~pr["right"] & ~pr["is_cat"], t32, np.float32(np.inf)).astype(np.float32)
+        has_hi = (~pr["right"] & ~pr["is_cat"]).astype(np.uint32)
+        # categorical: the one-hot column is 1 iff code == the column's code; left iff that value <= thr.  Bit c + 1 of the
+        # mask: code c follows the path here (c = -1: unknown, and every code no node tests)
+        left_if_match = 1.0 <= pr["thr"]
+        left_if_other = 0.0 <= pr["thr"]
+        other_ok = np.where(pr["right"], ~left_if_other, left_if_other)
+        match_ok = np.where(pr["right"], ~left_if_match, left_if_match)
+        mask = np.where(other_ok[:, None], np.uint32(0xFFFFFFFF), np.uint32(0)).repeat(4, axis=1).astype(np.uint32)
+        bit = pr["code"] + 1
+        rows = np.nonzero(pr["is_cat"])[0]
+        w, b = bit[rows] // 32, (bit[rows] % 32).astype(np.uint32)
+        one = np.left_shift(np.uint32(1), b)
+        mask[rows, w] = np.where(match_ok[rows], mask[rows, w] | one, mask[rows, w] & ~one)
+        mask[~pr["is_cat"]] = 0
+        # merge by (leaf, field)
+        m_zf = np.multiply.reduceat(pr["zf"], start)
+        m_lo = np.maximum.reduceat(lo, start)
+        m_hi = np.minimum.reduceat(hi, start)
+        m_has_hi = np.bitwise_or.reduceat(has_hi, start)
+        m_mask = np.bitwise_and.reduceat(mask, start, axis=0)
+        m_field = pr["field"][start]
+        m_cat = pr["is_cat"][start]
+        m_leaf = pr["leaf"][start]
+        counts = np.bincount(m_leaf, minlength=leaves.size)
+        have = np.nonzero(counts)[0]
+        lens = counts[have] + 1
+        # element table of this tree: per path a bias element, then its merged fields
+        e = np.zeros(int(lens.sum()), dtype=_PATH_ELEM)
+        first = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.int64)
+        pos = np.ones(e.size, dtype=bool)
+        pos[first] = False
+        bias = first
+        e["field"][bias] = BIAS_FIELD
+        e["kind"][bias] = PE_BIAS
+        e["zero_fraction"][bias] = 1.0
+        e["inv_zero_fraction"][bias] = 1.0
+        body = np.nonzero(pos)[0]  # m_* are sorted by leaf then field: they fill the non-bias slots in order
+        e["field"][body] = m_field
+        e["kind"][body] = np.where(m_cat, PE_CAT, PE_NUM | (m_has_hi * PE_HAS_HI)).astype(np.uint32)
+        e["lo"][body] = np.where(m_cat, np.float32(0), m_lo)
+        e["hi"][body] = np.where(m_cat | (m_has_hi == 0), np.float32(0), m_hi)
+        e["mask"][body] = m_mask
+        e["zero_fraction"][body] = m_zf
+        e["inv_zero_fraction"][body] = 1.0 / m_zf
+        r = np.zeros(have.size, dtype=_PATH_RECORD)
+        r["first"] = first + n_elems
+        r["len"] = lens
+        r["tree"] = ti
+        r["leaf"] = lv[have]
+        recs.append(r)
+        elems.append(e)
+        n_elems += e.size
+    recs = np.concatenate(recs) if recs else np.zeros(0, dtype=_PATH_RECORD)
+    elems = np.concatenate(elems) if elems else np.zeros(0, dtype=_PATH_ELEM)
+    max_len = int(recs["len"].max()) if recs.size else 0
+    if max_len > PATHS_MAX_LEN:
+        raise NotImplementedError(f"merged path of {max_len} elements exceeds {PATHS_MAX_LEN}")
+    ex = np.asarray(expected, dtype=np.float64)
+    base = float(ex.sum() / denom) if flat.agg_mode == AGG_RF_MEAN else float(init + ex.sum())
+    paths_off = PATHS_HEADER_BYTES
+    elems_off = (paths_off + recs.nbytes + 15) // 16 * 16
+    total = elems_off + elems.nbytes
+    header = struct.pack(_PATHS_HEADER_FMT, PATHS_MAGIC, PATHS_VERSION, PATHS_HEADER_BYTES, n_cat, n_num, flat.agg_mode,
+                         len(trees), recs.size, max_len, elems.size, 0, base, denom, blob_fingerprint(flat.blob), paths_off,
+                         elems_off, total)
+    out = bytearray(total)
+    out[: len(header)] = header
+    out[paths_off : paths_off + recs.nbytes] = recs.tobytes()
+    out[elems_off:] = elems.tobytes()
+    return bytes(out)
+
+
+def parse_explainer(paths: bytes) -> dict:
+    """Decode a path table (host-side mirror of ``forest_paths.h``): header fields plus ``paths`` / ``elems`` record arrays."""
+    f = struct.unpack_from(_PATHS_HEADER_FMT, paths, 0)
+    keys = ["magic", "version", "header_bytes", "n_cat", "n_num", "agg_mode", "n_trees", "n_paths", "max_len", "n_elems",
+            "reserved0", "base_value", "denom", "fingerprint", "paths_off", "elems_off", "total_bytes"]
+    h = dict(zip(keys, f))
+    h["paths"] = np.frombuffer(paths, dtype=_PATH_RECORD, count=h["n_paths"], offset=h["paths_off"])
+    h["elems"] = np.frombuffer(paths, dtype=_PATH_ELEM, count=h["n_elems"], offset=h["elems_off"])
+    return h

@@ -30,17 +30,19 @@ from ._cabi import OUT_F64, OUT_FULL
 from ._pylists import ListBuilder
 from .encode import RowEncoder
 from .engine import EngineGroup, ForestEngine
-from .flatten import FlatForest, flatten_isolation_forest, flatten_pipeline
+from .flatten import AGG_RF_MEAN, FlatForest, flatten_explainer, flatten_isolation_forest, flatten_pipeline
 
 BLOB_FILE = "forest.b2f.npz"
 OUTLIER_BLOB_FILE = "outlier.b2f"
 DRIFT_FILE = "drift_reference.npz"
+EXPLAIN_FILE = "explain.b2f"  # TreeSHAP path table (flatten_explainer); optional
 OUTLIER_PICKLE = os.path.join("artifacts", "outlier.pkl")  # joblib.dump(outlier, ".../outlier.pkl"), 02-register-model.ipynb:264,326-328
 SKLEARN_PICKLE = os.path.join("artifacts", "classifier", "model", "model.pkl")  # MLflow layout, 02-register-model.ipynb:317-321
 
 
 class B200Model:
-    def __init__(self, flat: FlatForest, devices=None, drift=None, proba_dtype=np.float64, outlier_blob: bytes | None = None, host_threads: int = 0):
+    def __init__(self, flat: FlatForest, devices=None, drift=None, proba_dtype=np.float64, outlier_blob: bytes | None = None, host_threads: int = 0,
+                 explain_blob: bytes | None = None):
         self.flat = flat
         self.all_features = flat.all_features
         self.categorical_features = list(flat.cat_features)
@@ -60,6 +62,10 @@ class B200Model:
         self.outlier_blob = outlier_blob
         if outlier_blob is not None:
             (self.group if self.group is not None else self.engine).attach_outlier_forest(outlier_blob)
+        # the explainer (TreeSHAP path table) lives on the first GPU only: explain() runs there
+        self.explain_blob = explain_blob
+        if explain_blob is not None:
+            self.engine.attach_explainer(explain_blob)
         # one scoring replica per GPU for the server's round-robin batcher (each has its own handle,
         # pinned staging and worker thread; the forest is replicated, rows are independent)
         engines = self.group.engines if self.group is not None else [self.engine]
@@ -73,12 +79,15 @@ class B200Model:
 
     # ------------------------------------------------------------------ construction
     @classmethod
-    def from_pipeline(cls, pipeline, reference_frame: pd.DataFrame | None = None, outlier=None, **kw) -> "B200Model":
+    def from_pipeline(cls, pipeline, reference_frame: pd.DataFrame | None = None, outlier=None, explain: bool = False, **kw) -> "B200Model":
         """Fitted sklearn Pipeline (the reference's model.pkl) -> model on the GPU.
 
         ``outlier``: the reference's fitted outlier detector (an alibi-detect ``IForest`` or a bare sklearn
-        ``IsolationForest`` plus ``outlier_threshold=``), flattened into a second forest over the same rows."""
+        ``IsolationForest`` plus ``outlier_threshold=``), flattened into a second forest over the same rows.
+        ``explain``: also build the TreeSHAP path table, so that ``explain()`` works."""
         flat = flatten_pipeline(pipeline)
+        if explain:
+            kw["explain_blob"] = flatten_explainer(pipeline, flat)
         drift = None
         if reference_frame is not None:
             from .drift import TabularDrift
@@ -208,16 +217,8 @@ class B200Model:
         # the drift sweep takes milliseconds of device time on its own stream (2.2 ms for 1 000 rows on an H100): start it
         # first, score the rows meanwhile
         pending = self._pool.submit(self.drift.score, df) if self.drift is not None else None
-        n = len(df)
         try:
-            fast = self._pipeline(df)
-            if fast is not None:
-                preds, flags = fast
-                flags = flags if flags is not None else [0] * n
-            else:
-                proba, _, fl = self._score(df, want_outliers=True)
-                preds = proba.tolist()
-                flags = fl.tolist() if fl is not None else [0] * n
+            preds, flags = self._predictions(df)
         finally:
             drift_scores = pending.result() if pending is not None else [0.0] * len(self.all_features)
         return {
@@ -225,6 +226,55 @@ class B200Model:
             "outliers": flags,
             "feature_drift_batch": dict(zip(self.all_features, drift_scores)),
         }
+
+
+    def _predictions(self, df: pd.DataFrame):
+        """-> (predictions list, outlier-flag list): what ``predict`` returns for these rows, without the drift scores."""
+        n = len(df)
+        fast = self._pipeline(df)
+        if fast is not None:
+            preds, flags = fast
+            return preds, flags if flags is not None else [0] * n
+        proba, _, fl = self._score(df, want_outliers=True)
+        return proba.tolist(), fl.tolist() if fl is not None else [0] * n
+
+    # ------------------------------------------------------------------ explanations
+    @property
+    def explainer_attached(self) -> bool:
+        return self.explain_blob is not None
+
+    @property
+    def explain_output(self) -> str:
+        """The space contributions are in: the probability (RandomForest) or the raw margin (GBDT)."""
+        return "probability" if self.flat.agg_mode == AGG_RF_MEAN else "log_odds"
+
+    def explain(self, model_input) -> dict:
+        """Exact path-dependent TreeSHAP contributions of every request field to every row's score.
+
+        -> ``{"feature_names": all_features, "output": "probability" | "log_odds", "base_value": float,
+        "contributions": float64 (n, n_fields), "predictions": the classifier's P(class 1) for these rows}``, with
+        ``base_value + contributions[i].sum()`` equal to row i's probability (RandomForest) or raw margin (GBDT; the
+        probability is its logistic).  A categorical field is one player, so its contribution is not the sum of per one-hot
+        column values other tools report.  Raises RuntimeError when the model has no explainer.
+
+        Everything runs on the FIRST GPU's handle only (the explainer lives there): the contributions, and the predictions,
+        which come from that GPU's scoring replica (``replicas[0].score``, the same call the HTTP batcher's first worker makes)
+        with the classifier alone.  So a row with a NaN numeric is explained even when an outlier forest is attached (the
+        outlier detector, not the classifier, refuses NaN in ``predict``).  On one GPU the predictions are the numbers
+        ``predict`` returns; a multi-GPU ``predict`` slices the batch over all GPUs and may differ from them in the last bits.
+        Calls on one handle must not overlap: a caller that also scores on ``replicas[0]`` from other threads serialises the
+        two (the HTTP server takes the first batcher worker's lock)."""
+        if self.explain_blob is None:
+            raise RuntimeError("this model has no explainer: build it with from_pipeline(..., explain=True) or load a model directory "
+                               f"that holds {EXPLAIN_FILE} (save_model_dir(..., explain_blob=flatten_explainer(pipeline)))")
+        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
+        if len(df.columns) == 0:
+            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        rows = self.encoder.encode_frame(df)
+        phi, base = self.engine.explain_rows(rows)
+        proba, _ = self.replicas[0].score(df, want_outliers=False)
+        return {"feature_names": list(self.all_features), "output": self.explain_output, "base_value": float(base),
+                "contributions": phi, "predictions": proba.tolist()}
 
 
 def _reject_nan(df: pd.DataFrame, numeric_features) -> None:
@@ -250,21 +300,23 @@ class _Replica:
                 self._scorer_failed = True
         return self._scorer
 
-    def score(self, df: pd.DataFrame):
-        """-> (proba1 float64 (n,), is_outlier int32 (n,) or None)."""
+    def score(self, df: pd.DataFrame, want_outliers: bool = True):
+        """-> (proba1 float64 (n,), is_outlier int32 (n,) or None).  ``want_outliers=False``: the classifier alone (no
+        outlier forest, so NaN numerics are accepted), on the same row format and kernels as the full pass."""
         n = len(df)
+        full = self.has_outlier and want_outliers
         sc = self._scorer_for() if n else None
         cols = self.encoder.frame_columns(df) if sc is not None else None
         if cols is not None:
             # the columnar request pipeline (csrc/scorer.h): column buffers -> encode threads -> H2D -> kernel(s) -> D2H
-            if self.has_outlier:
+            if full:
                 _reject_nan(df, self.numeric_features)
-            n_chunks = sc.start(n, cols, out_mode=OUT_FULL if self.has_outlier else OUT_F64,
+            n_chunks = sc.start(n, cols, out_mode=OUT_FULL if full else OUT_F64,
                                 fmt=(1 if self.encoder.packed_ok else 0) if self.has_outlier else None)
             for c in range(n_chunks):  # chunks ride different streams: each has its own completion event
                 sc.wait(c)
             out = sc.results()
-            if self.has_outlier:
+            if full:
                 return np.array(out["proba1"], dtype=np.float64), np.array(out["is_outlier"])
             return np.array(out, dtype=np.float64), None
         packed = self.encoder.packed_ok and n > self.encoder.SMALL_BATCH
@@ -273,7 +325,7 @@ class _Replica:
             self.encoder.encode_frame_packed(df, out=rows)
         else:
             self.encoder.encode_frame(df, out=rows)
-        if self.has_outlier:
+        if full:
             _reject_nan(df, self.numeric_features)
             rec = self.engine.predict_full(rows, out=self.engine.staging_full(n))
             return np.array(rec["proba1"], dtype=np.float64), np.array(rec["is_outlier"])
@@ -285,10 +337,15 @@ class _Replica:
 
 
 # ---------------------------------------------------------------------- loading
-def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | None = None, outlier_blob: bytes | None = None) -> None:
-    """Write the GPU-side artefact next to (or instead of) the MLflow pickles."""
+def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | None = None, outlier_blob: bytes | None = None,
+                   explain_blob: bytes | None = None) -> None:
+    """Write the GPU-side artefact next to (or instead of) the MLflow pickles.  ``explain_blob``: the TreeSHAP path table
+    (``flatten_explainer``), written as ``explain.b2f`` so that ``load_model`` attaches it."""
     os.makedirs(path, exist_ok=True)
     flat.save(os.path.join(path, BLOB_FILE))
+    if explain_blob is not None:
+        with open(os.path.join(path, EXPLAIN_FILE), "wb") as f:
+            f.write(explain_blob)
     if outlier_blob is not None:
         with open(os.path.join(path, OUTLIER_BLOB_FILE), "wb") as f:
             f.write(outlier_blob)
@@ -352,4 +409,8 @@ def load_model(path: str, devices=None, **kw) -> B200Model:
 
         drift = TabularDrift.load(drift_path, device=devices[0])
     outlier_blob = _load_outlier_blob(path, flat) if os.environ.get("B200_OUTLIERS", "gpu") != "off" else None
+    explain_path = os.path.join(path, EXPLAIN_FILE)
+    if "explain_blob" not in kw and os.path.exists(explain_path) and os.environ.get("B200_EXPLAIN", "gpu") != "off":
+        with open(explain_path, "rb") as f:
+            kw["explain_blob"] = f.read()
     return B200Model(flat, devices=devices, drift=drift, outlier_blob=outlier_blob, **kw)

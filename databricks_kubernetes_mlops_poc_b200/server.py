@@ -77,6 +77,9 @@ class MicroBatcher:
         self.batches = 0
         self.rows = 0
         self._stop = False
+        # replica i's engine handle is driven by worker i only, under locks[i]: another caller of that handle (the /explain
+        # handler on the first GPU) takes the same lock, so calls on one handle never overlap (include/b2f.h)
+        self.locks = [threading.Lock() for _ in self.models]
         self._threads = [threading.Thread(target=self._run, args=(i,), daemon=True, name=f"b200-batcher-{i}")
                          for i in range(len(self.models))]
         for t in self._threads:
@@ -135,23 +138,27 @@ class MicroBatcher:
             items = self._collect()
             if items is None:
                 return
-            try:
-                parts = self._score_items(model, items)
-                for it, part in zip(items, parts):
+            with self.locks[idx]:
+                self._serve(model, items)
+
+    def _serve(self, model, items) -> None:
+        try:
+            parts = self._score_items(model, items)
+            for it, part in zip(items, parts):
+                it.loop.call_soon_threadsafe(_resolve, it.future, part, None)
+        except BaseException as e:  # surfaces as HTTP 500, like any model exception in the reference
+            if len(items) == 1:
+                items[0].loop.call_soon_threadsafe(_resolve, items[0].future, None, e)
+                return
+            # the reference scores requests independently (app/main.py:72): a request the model rejects (a value
+            # that overflows float32, NaN with the outlier forest attached ...) must fail ALONE -- re-score the
+            # batch one request at a time and route each outcome to its own caller
+            for it in items:
+                try:
+                    part = self._score_items(model, [it])[0]
                     it.loop.call_soon_threadsafe(_resolve, it.future, part, None)
-            except BaseException as e:  # surfaces as HTTP 500, like any model exception in the reference
-                if len(items) == 1:
-                    items[0].loop.call_soon_threadsafe(_resolve, items[0].future, None, e)
-                    continue
-                # the reference scores requests independently (app/main.py:72): a request the model rejects (a value
-                # that overflows float32, NaN with the outlier forest attached ...) must fail ALONE -- re-score the
-                # batch one request at a time and route each outcome to its own caller
-                for it in items:
-                    try:
-                        part = self._score_items(model, [it])[0]
-                        it.loop.call_soon_threadsafe(_resolve, it.future, part, None)
-                    except BaseException as e1:
-                        it.loop.call_soon_threadsafe(_resolve, it.future, None, e1)
+                except BaseException as e1:
+                    it.loop.call_soon_threadsafe(_resolve, it.future, None, e1)
 
 
 def _resolve(fut, value, err):
@@ -231,6 +238,28 @@ def create_app(model=None, loader=None) -> FastAPI:
             closer()
 
     app = FastAPI(title=_service_name(), docs_url="/", lifespan=lifespan)
+
+    @app.post("/explain", openapi_extra={"requestBody": _REQUEST_SCHEMA})
+    async def explain(request: Request):
+        """Explain each applicant's score: exact TreeSHAP contribution of every request field (probability space for a random
+        forest, log-odds for a GBDT), the base value they start from, and the predictions themselves.  501 when the model was
+        loaded without an explainer."""
+        input_df = parser.frame(await request.body())
+        if len(input_df) == 0:
+            raise KeyError(f"None of {ALL_FEATURES} are in the [columns]")
+        m = ml_models["credit_default"]
+        if not getattr(m, "explainer_attached", False):
+            return Response(content=json.dumps({"detail": "this model has no explainer"}), status_code=501, media_type="application/json")
+        batcher = ml_models["_batcher"]
+
+        def run():
+            with batcher.locks[0]:  # the explainer sits on the first GPU, whose handle batcher worker 0 drives
+                return m.explain(input_df)
+
+        out = await asyncio.get_running_loop().run_in_executor(None, run)
+        body = {"feature_names": list(out["feature_names"]), "output": out["output"], "base_value": float(out["base_value"]),
+                "predictions": list(out["predictions"]), "contributions": np.asarray(out["contributions"], dtype=np.float64).tolist()}
+        return Response(content=json.dumps(body, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
 
     @app.post("/predict", response_model=ModelOutput, openapi_extra={"requestBody": _REQUEST_SCHEMA})
     async def predict(request: Request):

@@ -307,6 +307,26 @@ int b2f_predict_pairs(b2f_model *m, const void *rows, int64_t n, int row_format,
 int b2f_model_attach_outlier_forest(b2f_model *m, const void *forest_blob, size_t nbytes);
 int b2f_predict_full(b2f_model *m, const void *rows, int64_t n, int row_format, b2f_scored_full *out);
 
+/* ---- per-row explanations: exact path-dependent TreeSHAP contributions per request field (no reference counterpart: the
+ *      reference returns scores only).  Players are the model's n_cat + n_num request fields in row-word order (a categorical
+ *      field is ONE player, however many one-hot columns its nodes test); the game is Lundberg et al.'s path-dependent
+ *      conditional expectation (arXiv:1802.03888, Algorithms 1-2) with cover = tree_.weighted_n_node_samples.  Output space:
+ *      probability for a RandomForest, log-odds (raw margin) for a GBDT; base_value + sum_f phi[f] is that prediction.  Rows are
+ *      explained as they are scored (NaN -> median, float32 compares, unknown category = code -1).
+ * The explainer is a path table (csrc/forest_paths.h, written by flatten.py flatten_explainer) tied to one forest blob by a
+ * fingerprint; a model without one behaves exactly as before.  Sums run in a fixed order without atomics: the same batch
+ * gives bit-identical results on every run (another batch size may group partial sums differently, in the last bits). */
+int b2f_paths_validate(const void *paths, size_t nbytes); /* structural check of a path table; needs no GPU */
+/* B2F_EINVAL if the table was built from another forest (fingerprint) or its shape differs from the model's; replaces an
+ * explainer attached before */
+int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_t nbytes);
+/* rows: B2F_ROWS_WORDS24 or B2F_ROWS_PACKED64 in host memory (B2F_ROWS_RANKED: B2F_EINVAL); phi: n x (n_cat + n_num) doubles,
+ * row-major; base_value, device_ms (copies + kernels, CUDA events; 0 for n = 0) may be NULL.  Pipelined over the model's
+ * streams like b2f_predict_ex.  B2F_ESTATE without an explainer. */
+int b2f_explain(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi, double *base_value, float *device_ms);
+/* device-resident form: enqueued on the compute stream (asynchronous, like b2f_predict_device_ex; b2f_sync waits) */
+int b2f_explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev);
+
 /* asynchronous form for the request-batching ring: buffers must be pinned and stay valid until
  * b2f_wait(ticket) returns.  proba_is_f64 selects double (1) or float (0) outputs. */
 int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned,
