@@ -33,6 +33,7 @@
 #include "forest_predict_rank.cuh"
 #include "forest_rank.h"
 #include "tree_shap.cuh"
+#include "tree_shap_interactions.cuh"
 #include "json_rows.h"
 #include "row_encoder.h"
 
@@ -124,10 +125,11 @@ struct Slot {
     int64_t cap_rows = 0;
 };
 
-/* device buffers of one stream's explain launches: phi rows and the per-range partial sums (tree_shap.cuh) */
+/* device buffers of one stream's explain launches: phi (or interaction) rows and the per-range partial sums (tree_shap.cuh,
+ * tree_shap_interactions.cuh); both kinds share them, grown to the larger request */
 struct ExplainBuf {
     double *out = nullptr;
-    int64_t out_rows = 0;
+    size_t out_bytes = 0;
     double *scratch = nullptr;
     size_t scratch_bytes = 0;
 };
@@ -140,6 +142,9 @@ struct Explainer {
     int maxl = 9;        /* length bucket of k_tree_shap: 9, 16 or 24 */
     int smem_bytes = 0;
     int ctas_per_sm = 1; /* resident k_tree_shap CTAs per SM */
+    IParams ip;          /* k_tree_shap_interactions: sp plus each warp's fields (inter_assign) */
+    int inter_smem_bytes = 0;
+    int inter_ctas_per_sm = 1;
     ExplainBuf slots[B2F_STREAMS];
     ExplainBuf compute; /* b2f_explain_device */
 };
@@ -1044,24 +1049,36 @@ static int out_launch(b2f_model *m, cudaStream_t st, const void *rows_dev, int64
 /* ------------------------------------------------------------------ explanations (K5: tree_shap.cuh, forest_paths.h)
  * B2F_OUT_EXPLAIN is an output kind of the host pipeline only: b2f_explain passes it to enqueue_host_batch, so explanations
  * ride the same chunking, slots and streams as scores.  It is not a B2F_OUT_* value: out_row_bytes does not know it, so the
- * predict entry points refuse it. */
+ * predict entry points refuse it.  B2F_OUT_INTERACTIONS is its sibling for b2f_explain_interactions (tree_shap_interactions.cuh):
+ * F x F doubles per row. */
 #define B2F_OUT_EXPLAIN 16
+#define B2F_OUT_INTERACTIONS 17
+/* rows per chunk of an interactions batch (4 232 B of output per row for 23 fields), with no chunk plan: every chunk of
+ * 16 384 rows is 512 row tiles, more than the SMs hold at once, so it runs as one range and needs no scratch */
+#define B2F_INTER_CHUNK_ROWS 16384
 
 static int explain_fields(const b2f_model *m) { return (int)(m->hdr.n_cat + m->hdr.n_num); }
+static bool explain_kind(int kind) { return kind == B2F_OUT_EXPLAIN || kind == B2F_OUT_INTERACTIONS; }
+static size_t explain_row_bytes(const b2f_model *m, int kind) {
+    const size_t F = (size_t)explain_fields(m);
+    return (kind == B2F_OUT_INTERACTIONS ? F * F : F) * sizeof(double);
+}
 
-static int explain_check(const b2f_model *m, int fmt, bool have_out) {
+static int explain_check(const b2f_model *m, int fmt, int kind, bool have_out) {
     if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
     if (fmt == B2F_ROWS_RANKED)
         return set_err(B2F_EINVAL, "explanations take float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
-    if (!have_out) return set_err(B2F_EINVAL, "phi is NULL");
+    if (!have_out) return set_err(B2F_EINVAL, kind == B2F_OUT_INTERACTIONS ? "phi2 is NULL" : "phi is NULL");
     return B2F_OK;
 }
 
 /* row tiles x path ranges of one launch: one range from a full grid of row tiles up; below, enough ranges to fill every SM
- * (at least two paths per warp).  The partials of several ranges take ranges * n * fields doubles; since ranges > 1 only when
- * tiles < target, that is below 2 * target * 32 rows' worth: bounded by the GPU, not by n or the number of paths. */
-static int64_t explain_ranges(const b2f_model *m, int64_t n) {
-    const int64_t tiles = (n + 31) / 32, target = (int64_t)m->sm_count * m->ex->ctas_per_sm;
+ * (at least sixteen paths per range: two per warp for k_tree_shap).  The partials of several ranges take ranges * n * values
+ * doubles (values: fields, or F(F+1)/2 triangle slots for interactions); since ranges > 1 only when tiles < target, that is
+ * below 2 * target * 32 rows' worth: bounded by the GPU, not by n or the number of paths. */
+static int64_t explain_ranges(const b2f_model *m, int64_t n, int kind) {
+    const int ctas = kind == B2F_OUT_INTERACTIONS ? m->ex->inter_ctas_per_sm : m->ex->ctas_per_sm;
+    const int64_t tiles = (n + 31) / 32, target = (int64_t)m->sm_count * ctas;
     int64_t r = tiles >= target ? 1 : (target + tiles - 1) / tiles;
     r = std::min<int64_t>(r, std::max<int64_t>(1, (int64_t)m->ex->hdr.n_paths / (2 * B2F_SHAP_WARPS)));
     return std::max<int64_t>(1, std::min<int64_t>(r, 65535));
@@ -1095,7 +1112,7 @@ static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, i
         CUDA_TRY(cudaMemsetAsync(phi_dev, 0, (size_t)n * F * sizeof(double), st));
         return B2F_OK;
     }
-    const int64_t ranges = explain_ranges(m, n);
+    const int64_t ranges = explain_ranges(m, n, B2F_OUT_EXPLAIN);
     if (ranges > 1) {
         int rc = explain_reserve_scratch(b, st, (size_t)ranges * (size_t)n * F * sizeof(double));
         if (rc) return rc;
@@ -1117,16 +1134,55 @@ static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, i
     return B2F_OK;
 }
 
-/* the phi buffer of one slot's chunk */
-static int explain_reserve_out(b2f_model *m, ExplainBuf &b, cudaStream_t st, int64_t rows) {
-    if (rows <= b.out_rows) return B2F_OK;
+template <int MAXL>
+static auto inter_kernel(bool pk) {
+    return pk ? k_tree_shap_interactions<MAXL, true> : k_tree_shap_interactions<MAXL, false>;
+}
+static auto inter_kernel_for(int maxl, bool pk) {
+    return maxl <= 9 ? inter_kernel<9>(pk) : (maxl <= 16 ? inter_kernel<16>(pk) : inter_kernel<24>(pk));
+}
+
+/* phi2_dev[n][fields][fields] for n device rows of format fmt, on stream st, partial triangles in b's scratch */
+static int launch_interactions(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, double *phi2_dev, ExplainBuf &b) {
+    if (n <= 0) return B2F_OK;
+    const Explainer &ex = *m->ex;
+    const int F = explain_fields(m), T = inter_slots(F);
+    if (ex.hdr.n_paths == 0) {
+        CUDA_TRY(cudaMemsetAsync(phi2_dev, 0, (size_t)n * F * F * sizeof(double), st));
+        return B2F_OK;
+    }
+    const int64_t ranges = explain_ranges(m, n, B2F_OUT_INTERACTIONS);
+    if (ranges > 1) {
+        int rc = explain_reserve_scratch(b, st, (size_t)ranges * (size_t)n * T * sizeof(double));
+        if (rc) return rc;
+    }
+    const dim3 grid((unsigned)((n + 31) / 32), (unsigned)ranges);
+    inter_kernel_for(ex.maxl, fmt == B2F_ROWS_PACKED64)<<<grid, B2F_SHAP_THREADS, ex.inter_smem_bytes, st>>>(
+        ex.ip, static_cast<const uint32_t *>(rows_dev), (long long)n, phi2_dev, b.scratch);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_tree_shap_interactions launch failed: %s", cudaGetErrorString(e));
+    m->launches++;
+    if (ranges > 1) {
+        const unsigned blocks = (unsigned)std::min<int64_t>(n, (int64_t)m->sm_count * 8);
+        k_tree_shap_interactions_finish<<<blocks, 256, (size_t)T * sizeof(double), st>>>(b.scratch, (int)ranges, (long long)n, F, ex.hdr.denom,
+                                                                                         phi2_dev);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_tree_shap_interactions_finish launch failed: %s", cudaGetErrorString(e));
+        m->launches++;
+    }
+    return B2F_OK;
+}
+
+/* the output buffer of one slot's chunk: rows of row_bytes (at least 1024 rows' worth) */
+static int explain_reserve_out(ExplainBuf &b, cudaStream_t st, int64_t rows, size_t row_bytes) {
+    if ((size_t)rows * row_bytes <= b.out_bytes) return B2F_OK;
     CUDA_TRY(cudaStreamSynchronize(st));
     if (b.out) cudaFree(b.out);
     b.out = nullptr;
-    b.out_rows = 0;
-    const int64_t cap = std::max<int64_t>(rows, 1024);
-    CUDA_TRY(cudaMalloc((void **)&b.out, (size_t)cap * explain_fields(m) * sizeof(double)));
-    b.out_rows = cap;
+    b.out_bytes = 0;
+    const size_t cap = (size_t)std::max<int64_t>(rows, 1024) * row_bytes;
+    CUDA_TRY(cudaMalloc((void **)&b.out, cap));
+    b.out_bytes = cap;
     return B2F_OK;
 }
 
@@ -1163,17 +1219,18 @@ static int submit_chunk(b2f_model *m, Slot &sl, const void *rows, int fmt, int k
         marks->push_back(e);
     };
     if (marks && marks->empty()) mark();
-    const bool explain = kind == B2F_OUT_EXPLAIN;
+    const bool explain = explain_kind(kind);
     ExplainBuf *eb = explain ? &m->ex->slots[&sl - m->slots] : nullptr;
-    if (explain && (rc = explain_reserve_out(m, *eb, sl.stream, cnt))) return rc;
+    const size_t row_bytes = row_bytes_of(m, fmt), out_bytes = explain ? explain_row_bytes(m, kind) : out_row_bytes(kind);
+    if (explain && (rc = explain_reserve_out(*eb, sl.stream, cnt, out_bytes))) return rc;
     void *d_out = explain ? static_cast<void *>(eb->out) : sl.d_proba;
-    const size_t row_bytes = row_bytes_of(m, fmt), out_bytes = explain ? explain_fields(m) * sizeof(double) : out_row_bytes(kind);
     const bool records = kind == B2F_OUT_PAIRS || kind == B2F_OUT_FULL;
     CUDA_TRY(cudaMemcpyAsync(sl.d_rows, static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, (size_t)cnt * row_bytes, cudaMemcpyHostToDevice,
                              sl.stream));
     mark();
-    rc = explain ? launch_explain(m, sl.stream, sl.d_rows, cnt, fmt, eb->out, *eb)
-                 : out_launch(m, sl.stream, sl.d_rows, cnt, fmt, kind, out ? sl.d_proba : nullptr, label ? sl.d_label : nullptr);
+    rc = kind == B2F_OUT_EXPLAIN        ? launch_explain(m, sl.stream, sl.d_rows, cnt, fmt, eb->out, *eb)
+         : kind == B2F_OUT_INTERACTIONS ? launch_interactions(m, sl.stream, sl.d_rows, cnt, fmt, eb->out, *eb)
+                                        : out_launch(m, sl.stream, sl.d_rows, cnt, fmt, kind, out ? sl.d_proba : nullptr, label ? sl.d_label : nullptr);
     if (rc) return rc;
     mark();
     if (out)
@@ -1189,14 +1246,15 @@ static int submit_chunk(b2f_model *m, Slot &sl, const void *rows, int fmt, int k
 static int enqueue_host_batch(b2f_model *m, const void *rows, int64_t n, int fmt, void *out, int kind, int32_t *label, uint32_t *used_mask) {
     *used_mask = 0;
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
-    int rc = kind == B2F_OUT_EXPLAIN ? explain_check(m, fmt, out || n == 0) : out_check(m, kind, fmt, out || n == 0);
+    int rc = explain_kind(kind) ? explain_check(m, fmt, kind, out || n == 0) : out_check(m, kind, fmt, out || n == 0);
     if (rc) return rc;
     if (n == 0) return B2F_OK;
     if (!rows) return set_err(B2F_EINVAL, "rows is NULL");
     rc = check_row_format(m, fmt);
     if (rc) return rc;
     CUDA_TRY(cudaSetDevice(m->device));
-    int64_t chunk = m->chunk_rows;
+    const bool inter = kind == B2F_OUT_INTERACTIONS;
+    int64_t chunk = inter ? B2F_INTER_CHUNK_ROWS : m->chunk_rows;
     if (n <= chunk + chunk / 2) chunk = n; /* small batch: one H2D, one launch */
     static const bool timeline = getenv("B2F_TIMELINE") != nullptr;
     std::vector<cudaEvent_t> tev;
@@ -1206,7 +1264,7 @@ static int enqueue_host_batch(b2f_model *m, const void *rows, int64_t n, int fmt
     int c = 0;
     for (int64_t off = 0; off < n; ++c) {
         int64_t cnt = std::min(chunk, n - off);
-        if (!m->chunk_plan.empty() && chunk != n && n >= 2 * m->chunk_rows) {
+        if (!inter && !m->chunk_plan.empty() && chunk != n && n >= 2 * m->chunk_rows) {
             cnt = (size_t)c < m->chunk_plan.size() ? std::max<int64_t>(1024, (n * m->chunk_plan[c] / 1024 + 1023) / 1024 * 1024) : n - off;
             cnt = std::min(cnt, n - off);
         }
@@ -1357,6 +1415,38 @@ static uint64_t blob_fingerprint(const uint8_t *blob, size_t nbytes) {
     return sum;
 }
 
+/* the fields each warp of k_tree_shap_interactions owns, balancing the counted pair work: per path of d elements that holds
+ * field f, its owner unwinds f (d steps) and takes the unwound sum of every element of a higher field (d - 1 steps each).
+ * Longest work first, each field to the warp with the least work so far (ties: the lower field, the lower warp). */
+static void inter_assign(const uint8_t *t, const b2f_paths_header &h, uint32_t own[B2F_SHAP_WARPS]) {
+    const int F = (int)(h.n_cat + h.n_num);
+    const b2f_path *P = reinterpret_cast<const b2f_path *>(t + h.paths_off);
+    const b2f_path_elem *E = reinterpret_cast<const b2f_path_elem *>(t + h.elems_off);
+    std::vector<double> work(F, 0.0);
+    for (uint32_t p = 0; p < h.n_paths; ++p) {
+        b2f_path pr;
+        memcpy(&pr, &P[p], sizeof(pr));
+        uint32_t fields[B2F_PATHS_MAX_LEN];
+        for (uint32_t k = 1; k < pr.len; ++k) memcpy(&fields[k], &E[pr.first + k].field, sizeof(uint32_t));
+        const double d = pr.len - 1.0;
+        for (uint32_t k = 1; k < pr.len; ++k) {
+            int higher = 0;
+            for (uint32_t j = 1; j < pr.len; ++j) higher += fields[j] > fields[k];
+            work[fields[k]] += d + higher * (d - 1.0);
+        }
+    }
+    std::vector<int> order(F);
+    for (int f = 0; f < F; ++f) order[f] = f;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return work[a] > work[b]; });
+    double load[B2F_SHAP_WARPS] = {};
+    for (int w = 0; w < B2F_SHAP_WARPS; ++w) own[w] = 0;
+    for (int f : order) {
+        const int w = (int)(std::min_element(load, load + B2F_SHAP_WARPS) - load);
+        own[w] |= 1u << f;
+        load[w] += work[f];
+    }
+}
+
 extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_t nbytes) {
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
     b2f_paths_header h;
@@ -1407,8 +1497,18 @@ extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_
     for (bool pk : {false, true})
         if (e == cudaSuccess) e = cudaFuncSetAttribute(shap_kernel_for(ex->maxl, pk), cudaFuncAttributeMaxDynamicSharedMemorySize, ex->smem_bytes);
     if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ex->ctas_per_sm, shap_kernel_for(ex->maxl, false), B2F_SHAP_THREADS, ex->smem_bytes);
+    ex->ip.s = sp;
+    inter_assign(static_cast<const uint8_t *>(paths), h, ex->ip.own);
+    ex->inter_smem_bytes = inter_smem_bytes((int)(h.n_cat + h.n_num));
+    for (bool pk : {false, true})
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(inter_kernel_for(ex->maxl, pk), cudaFuncAttributeMaxDynamicSharedMemorySize, ex->inter_smem_bytes);
+    if (e == cudaSuccess)
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ex->inter_ctas_per_sm, inter_kernel_for(ex->maxl, false), B2F_SHAP_THREADS,
+                                                          ex->inter_smem_bytes);
     if (e != cudaSuccess) return fail(set_err(B2F_ECUDA, "explainer set-up failed: %s", cudaGetErrorString(e)));
     ex->ctas_per_sm = std::max(1, ex->ctas_per_sm);
+    ex->inter_ctas_per_sm = std::max(1, ex->inter_ctas_per_sm);
     if (m->ex) { /* the device was synchronised above */
         for (ExplainBuf *b = m->ex->slots; b <= &m->ex->compute; ++b) {
             if (b->out) cudaFree(b->out);
@@ -1421,7 +1521,8 @@ extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_
     return B2F_OK;
 }
 
-extern "C" int b2f_explain(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi, double *base_value, float *device_ms) {
+/* b2f_explain / b2f_explain_interactions: kind B2F_OUT_EXPLAIN or B2F_OUT_INTERACTIONS */
+static int explain_host(b2f_model *m, const void *rows, int64_t n, int row_format, double *out, int kind, double *base_value, float *device_ms) {
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
     if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
     if (base_value) *base_value = m->ex->hdr.base_value;
@@ -1441,12 +1542,12 @@ extern "C" int b2f_explain(b2f_model *m, const void *rows, int64_t n, int row_fo
         CUDA_TRY(cudaEventRecord(ev[0], m->slots[first].stream));
     }
     uint32_t mask = 0;
-    int rc = enqueue_host_batch(m, rows, n, row_format, phi, B2F_OUT_EXPLAIN, nullptr, &mask);
+    int rc = enqueue_host_batch(m, rows, n, row_format, out, kind, nullptr, &mask);
     if (device_ms && n > 0 && rc == B2F_OK)
         for (int s = 0; s < B2F_STREAMS && rc == B2F_OK; ++s)
             if ((mask & (1u << s)) && cudaEventRecord(ev[1 + s], m->slots[s].stream) != cudaSuccess)
                 rc = set_err(B2F_ECUDA, "cudaEventRecord failed: %s", cudaGetErrorString(cudaGetLastError()));
-    int rc2 = sync_mask(m, mask); /* always: the chunks already enqueued write into the caller's phi */
+    int rc2 = sync_mask(m, mask); /* always: the chunks already enqueued write into the caller's output */
     if (rc == B2F_OK) rc = rc2;
     if (device_ms && n > 0)
         for (int s = 0; s < B2F_STREAMS && rc == B2F_OK; ++s)
@@ -1458,14 +1559,30 @@ extern "C" int b2f_explain(b2f_model *m, const void *rows, int64_t n, int row_fo
     return rc;
 }
 
-extern "C" int b2f_explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev) {
+extern "C" int b2f_explain(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi, double *base_value, float *device_ms) {
+    return explain_host(m, rows, n, row_format, phi, B2F_OUT_EXPLAIN, base_value, device_ms);
+}
+extern "C" int b2f_explain_interactions(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi2, double *base_value,
+                                        float *device_ms) {
+    return explain_host(m, rows, n, row_format, phi2, B2F_OUT_INTERACTIONS, base_value, device_ms);
+}
+
+/* b2f_explain_device / b2f_explain_interactions_device */
+static int explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *out_dev, int kind) {
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
-    int rc = explain_check(m, row_format, phi_dev != nullptr || n == 0);
+    int rc = explain_check(m, row_format, kind, out_dev != nullptr || n == 0);
     if (rc == B2F_OK) rc = check_row_format(m, row_format);
     if (rc) return rc;
     CUDA_TRY(cudaSetDevice(m->device));
-    return launch_explain(m, m->compute, rows_dev, n, row_format, phi_dev, m->ex->compute);
+    return kind == B2F_OUT_INTERACTIONS ? launch_interactions(m, m->compute, rows_dev, n, row_format, out_dev, m->ex->compute)
+                                        : launch_explain(m, m->compute, rows_dev, n, row_format, out_dev, m->ex->compute);
+}
+extern "C" int b2f_explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev) {
+    return explain_device(m, rows_dev, n, row_format, phi_dev, B2F_OUT_EXPLAIN);
+}
+extern "C" int b2f_explain_interactions_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi2_dev) {
+    return explain_device(m, rows_dev, n, row_format, phi2_dev, B2F_OUT_INTERACTIONS);
 }
 
 extern "C" int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned, int proba_is_f64,

@@ -200,6 +200,25 @@ class ForestEngine:
         """Enqueue an explanation of device-resident rows into device phi (n x fields doubles); ``sync`` waits."""
         check(self._lib.b2f_explain_device(self._h, rows_dev, n, fmt, phi_dev), "b2f_explain_device")
 
+    def explain_interactions_rows(self, rows: np.ndarray, device_ms: bool = False):
+        """Encoded rows (N, 24) or packed (N, 16) -> (phi2 float64 (N, F, F), base_value[, device ms]) with F = n_cat + n_num:
+        exact path-dependent SHAP interaction values per pair of request fields.  Each matrix is symmetric, its rows sum to
+        ``explain_rows``' phi and its total to the prediction - base_value."""
+        rows = np.ascontiguousarray(rows)
+        fmt = self._fmt(rows)
+        n = rows.shape[0]
+        inf = self.info()
+        F = inf["n_cat"] + inf["n_num"]
+        phi2 = np.empty((n, F, F), dtype=np.float64)
+        base, ms = C.c_double(0.0), C.c_float(0.0)
+        check(self._lib.b2f_explain_interactions(self._h, ptr(rows), n, fmt, ptr(phi2), C.byref(base), C.byref(ms)),
+              "b2f_explain_interactions")
+        return (phi2, base.value, ms.value) if device_ms else (phi2, base.value)
+
+    def explain_interactions_device(self, rows_dev: int, n: int, phi2_dev: int, fmt: int = ROWS_WORDS24) -> None:
+        """Enqueue interaction values of device-resident rows into device phi2 (n x fields x fields doubles); ``sync`` waits."""
+        check(self._lib.b2f_explain_interactions_device(self._h, rows_dev, n, fmt, phi2_dev), "b2f_explain_interactions_device")
+
     # ------------------------------------------------------------------ device-resident interface
     def device_alloc(self, nbytes: int) -> int:
         p = self._lib.b2f_device_alloc(self._h, nbytes)

@@ -239,11 +239,9 @@ def create_app(model=None, loader=None) -> FastAPI:
 
     app = FastAPI(title=_service_name(), docs_url="/", lifespan=lifespan)
 
-    @app.post("/explain", openapi_extra={"requestBody": _REQUEST_SCHEMA})
-    async def explain(request: Request):
-        """Explain each applicant's score: exact TreeSHAP contribution of every request field (probability space for a random
-        forest, log-odds for a GBDT), the base value they start from, and the predictions themselves.  501 when the model was
-        loaded without an explainer."""
+    async def explained(request: Request, method: str, key: str) -> Response:
+        """The body and error rules of /explain and /explain/interactions: parse like /predict, 501 without an explainer, run
+        ``model.<method>`` under the first batcher worker's lock and answer its ``key`` array as nested lists."""
         input_df = parser.frame(await request.body())
         if len(input_df) == 0:
             raise KeyError(f"None of {ALL_FEATURES} are in the [columns]")
@@ -254,12 +252,26 @@ def create_app(model=None, loader=None) -> FastAPI:
 
         def run():
             with batcher.locks[0]:  # the explainer sits on the first GPU, whose handle batcher worker 0 drives
-                return m.explain(input_df)
+                return getattr(m, method)(input_df)
 
         out = await asyncio.get_running_loop().run_in_executor(None, run)
         body = {"feature_names": list(out["feature_names"]), "output": out["output"], "base_value": float(out["base_value"]),
-                "predictions": list(out["predictions"]), "contributions": np.asarray(out["contributions"], dtype=np.float64).tolist()}
+                "predictions": list(out["predictions"]), key: np.asarray(out[key], dtype=np.float64).tolist()}
         return Response(content=json.dumps(body, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
+
+    @app.post("/explain", openapi_extra={"requestBody": _REQUEST_SCHEMA})
+    async def explain(request: Request):
+        """Explain each applicant's score: exact TreeSHAP contribution of every request field (probability space for a random
+        forest, log-odds for a GBDT), the base value they start from, and the predictions themselves.  501 when the model was
+        loaded without an explainer."""
+        return await explained(request, "explain", "contributions")
+
+    @app.post("/explain/interactions", openapi_extra={"requestBody": _REQUEST_SCHEMA})
+    async def explain_interactions(request: Request):
+        """Explain each applicant's score by pairs of request fields: exact TreeSHAP interaction values, one symmetric
+        fields x fields matrix per applicant whose rows sum to /explain's contributions (same output space, base value and
+        predictions).  501 when the model was loaded without an explainer."""
+        return await explained(request, "explain_interactions", "interactions")
 
     @app.post("/predict", response_model=ModelOutput, openapi_extra={"requestBody": _REQUEST_SCHEMA})
     async def predict(request: Request):

@@ -326,6 +326,16 @@ int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_t nbytes);
 int b2f_explain(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi, double *base_value, float *device_ms);
 /* device-resident form: enqueued on the compute stream (asynchronous, like b2f_predict_device_ex; b2f_sync waits) */
 int b2f_explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev);
+/* SHAP interaction values (Lundberg et al., arXiv:1802.03888 §4; shap's shap_interaction_values) of the same players, game
+ * and output space: phi2 is n x F x F doubles, row-major (F = n_cat + n_num), entry [i][a][b] the Shapley interaction index
+ * of fields a != b for row i, and [i][a][a] = phi_a - sum_{b != a} phi2[i][a][b].  Every matrix is exactly symmetric (each
+ * pair is computed once); each of its rows sums to that field's b2f_explain value and the whole matrix to the prediction -
+ * base_value.  Fields that never share a path get exactly 0.  Arguments and errors as b2f_explain (B2F_ESTATE without an
+ * explainer; B2F_EINVAL for ranked rows, a NULL phi2 with n > 0, n < 0).  Output buffers are allocated on the first call
+ * (chunks of at most 16 384 rows per stream); a model that never asks for interactions allocates nothing for them. */
+int b2f_explain_interactions(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi2, double *base_value, float *device_ms);
+/* device-resident form: enqueued on the compute stream (asynchronous, like b2f_explain_device; b2f_sync waits) */
+int b2f_explain_interactions_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi2_dev);
 
 /* asynchronous form for the request-batching ring: buffers must be pinned and stay valid until
  * b2f_wait(ticket) returns.  proba_is_f64 selects double (1) or float (0) outputs. */
