@@ -134,17 +134,19 @@ struct ExplainBuf {
     size_t scratch_bytes = 0;
 };
 
+/* the launch shape of one explanation kernel (k_tree_shap or k_tree_shap_interactions) */
+struct ExplainKernel {
+    int smem_bytes = 0;
+    int ctas_per_sm = 1; /* resident CTAs per SM */
+};
+
 /* an attached path table (b2f_model_attach_explainer) */
 struct Explainer {
     b2f_paths_header hdr;
     void *d_table = nullptr;
-    SParams sp;
-    int maxl = 9;        /* length bucket of k_tree_shap: 9, 16 or 24 */
-    int smem_bytes = 0;
-    int ctas_per_sm = 1; /* resident k_tree_shap CTAs per SM */
-    IParams ip;          /* k_tree_shap_interactions: sp plus each warp's fields (inter_assign) */
-    int inter_smem_bytes = 0;
-    int inter_ctas_per_sm = 1;
+    IParams ip;   /* k_tree_shap takes ip.s; k_tree_shap_interactions also each warp's fields (inter_assign) */
+    int maxl = 9; /* length bucket of both kernels: 9, 16 or 24 */
+    ExplainKernel kernels[2]; /* [kind - B2F_OUT_EXPLAIN] */
     ExplainBuf slots[B2F_STREAMS];
     ExplainBuf compute; /* b2f_explain_device */
 };
@@ -794,19 +796,22 @@ extern "C" b2f_model *b2f_model_create(const void *forest_blob, size_t nbytes, i
     return m;
 }
 
+/* frees an explainer and its device buffers; nothing on the device may still use them */
+static void explainer_free(Explainer *ex) {
+    for (ExplainBuf *b = ex->slots; b <= &ex->compute; ++b) {
+        if (b->out) cudaFree(b->out);
+        if (b->scratch) cudaFree(b->scratch);
+    }
+    if (ex->d_table) cudaFree(ex->d_table);
+    delete ex;
+}
+
 extern "C" void b2f_model_destroy(b2f_model *m) {
     if (!m) return;
     cudaSetDevice(m->device);
     cudaDeviceSynchronize();
     if (m->outlier) b2f_model_destroy(m->outlier);
-    if (m->ex) {
-        for (ExplainBuf *b = m->ex->slots; b <= &m->ex->compute; ++b) {
-            if (b->out) cudaFree(b->out);
-            if (b->scratch) cudaFree(b->scratch);
-        }
-        if (m->ex->d_table) cudaFree(m->ex->d_table);
-        delete m->ex;
-    }
+    if (m->ex) explainer_free(m->ex);
     if (m->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(m->comm);
     for (int s = 0; s < B2F_STREAMS; ++s) {
         Slot &sl = m->slots[s];
@@ -1056,6 +1061,8 @@ static int out_launch(b2f_model *m, cudaStream_t st, const void *rows_dev, int64
 /* rows per chunk of an interactions batch (4 232 B of output per row for 23 fields), with no chunk plan: every chunk of
  * 16 384 rows is 512 row tiles, more than the SMs hold at once, so it runs as one range and needs no scratch */
 #define B2F_INTER_CHUNK_ROWS 16384
+/* the fixed rows per chunk of a host batch of this kind, or 0: the model's chunk size and chunk plan */
+static int64_t fixed_chunk_rows(int kind) { return kind == B2F_OUT_INTERACTIONS ? B2F_INTER_CHUNK_ROWS : 0; }
 
 static int explain_fields(const b2f_model *m) { return (int)(m->hdr.n_cat + m->hdr.n_num); }
 static bool explain_kind(int kind) { return kind == B2F_OUT_EXPLAIN || kind == B2F_OUT_INTERACTIONS; }
@@ -1077,8 +1084,7 @@ static int explain_check(const b2f_model *m, int fmt, int kind, bool have_out) {
  * doubles (values: fields, or F(F+1)/2 triangle slots for interactions); since ranges > 1 only when tiles < target, that is
  * below 2 * target * 32 rows' worth: bounded by the GPU, not by n or the number of paths. */
 static int64_t explain_ranges(const b2f_model *m, int64_t n, int kind) {
-    const int ctas = kind == B2F_OUT_INTERACTIONS ? m->ex->inter_ctas_per_sm : m->ex->ctas_per_sm;
-    const int64_t tiles = (n + 31) / 32, target = (int64_t)m->sm_count * ctas;
+    const int64_t tiles = (n + 31) / 32, target = (int64_t)m->sm_count * m->ex->kernels[kind - B2F_OUT_EXPLAIN].ctas_per_sm;
     int64_t r = tiles >= target ? 1 : (target + tiles - 1) / tiles;
     r = std::min<int64_t>(r, std::max<int64_t>(1, (int64_t)m->ex->hdr.n_paths / (2 * B2F_SHAP_WARPS)));
     return std::max<int64_t>(1, std::min<int64_t>(r, 65535));
@@ -1096,78 +1102,55 @@ static int explain_reserve_scratch(ExplainBuf &b, cudaStream_t st, size_t bytes)
 }
 
 template <int MAXL>
-static auto shap_kernel(bool pk) {
-    return pk ? k_tree_shap<MAXL, true> : k_tree_shap<MAXL, false>;
+static const void *explain_kernel_l(int kind, bool pk) {
+    if (kind == B2F_OUT_INTERACTIONS)
+        return pk ? (const void *)k_tree_shap_interactions<MAXL, true> : (const void *)k_tree_shap_interactions<MAXL, false>;
+    return pk ? (const void *)k_tree_shap<MAXL, true> : (const void *)k_tree_shap<MAXL, false>;
 }
-static auto shap_kernel_for(int maxl, bool pk) {
-    return maxl <= 9 ? shap_kernel<9>(pk) : (maxl <= 16 ? shap_kernel<16>(pk) : shap_kernel<24>(pk));
+/* the kind's kernel for the path-length bucket maxl and the row format.  Both take (params, rows, n, out, partials): IParams
+ * for interactions, its SParams otherwise. */
+static const void *explain_kernel(int kind, int maxl, bool pk) {
+    return maxl <= 9 ? explain_kernel_l<9>(kind, pk) : (maxl <= 16 ? explain_kernel_l<16>(kind, pk) : explain_kernel_l<24>(kind, pk));
 }
 
-/* phi_dev[n][fields] for n device rows of format fmt, on stream st, partial sums in b's scratch */
-static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, double *phi_dev, ExplainBuf &b) {
+/* out_dev[n] rows of explain_row_bytes (phi, or the F x F interaction matrix) for n device rows of format fmt, on stream st,
+ * partial sums (phi, or the triangle) in b's scratch */
+static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, int kind, double *out_dev, ExplainBuf &b) {
     if (n <= 0) return B2F_OK;
-    const Explainer &ex = *m->ex;
-    const int F = explain_fields(m);
+    Explainer &ex = *m->ex;
+    const bool inter = kind == B2F_OUT_INTERACTIONS;
+    const char *name = inter ? "k_tree_shap_interactions" : "k_tree_shap";
+    const int F = explain_fields(m), values = inter ? inter_slots(F) : F; /* partial sums per row */
     if (ex.hdr.n_paths == 0) { /* every tree a single leaf: nothing moves away from base_value */
-        CUDA_TRY(cudaMemsetAsync(phi_dev, 0, (size_t)n * F * sizeof(double), st));
+        CUDA_TRY(cudaMemsetAsync(out_dev, 0, (size_t)n * explain_row_bytes(m, kind), st));
         return B2F_OK;
     }
-    const int64_t ranges = explain_ranges(m, n, B2F_OUT_EXPLAIN);
+    const int64_t ranges = explain_ranges(m, n, kind);
     if (ranges > 1) {
-        int rc = explain_reserve_scratch(b, st, (size_t)ranges * (size_t)n * F * sizeof(double));
+        int rc = explain_reserve_scratch(b, st, (size_t)ranges * (size_t)n * values * sizeof(double));
         if (rc) return rc;
     }
-    const dim3 grid((unsigned)((n + 31) / 32), (unsigned)ranges);
-    shap_kernel_for(ex.maxl, fmt == B2F_ROWS_PACKED64)<<<grid, B2F_SHAP_THREADS, ex.smem_bytes, st>>>(
-        ex.sp, static_cast<const uint32_t *>(rows_dev), (long long)n, phi_dev, b.scratch);
+    const uint32_t *rows = static_cast<const uint32_t *>(rows_dev);
+    long long n_rows = n;
+    void *args[] = {inter ? static_cast<void *>(&ex.ip) : static_cast<void *>(&ex.ip.s), &rows, &n_rows, &out_dev, &b.scratch};
+    /* a failed launch is also the thread's last error, taken (and cleared) below as after <<< >>> */
+    cudaLaunchKernel(explain_kernel(kind, ex.maxl, fmt == B2F_ROWS_PACKED64), dim3((unsigned)((n + 31) / 32), (unsigned)ranges),
+                     dim3(B2F_SHAP_THREADS), args, (size_t)ex.kernels[kind - B2F_OUT_EXPLAIN].smem_bytes, st);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_tree_shap launch failed: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return set_err(B2F_ECUDA, "%s launch failed: %s", name, cudaGetErrorString(e));
     m->launches++;
     if (ranges > 1) {
-        const int64_t values = n * F;
-        const unsigned blocks = (unsigned)std::min<int64_t>((values + 255) / 256, (int64_t)m->sm_count * 8);
-        k_tree_shap_finish<<<blocks, 256, 0, st>>>(b.scratch, (int)ranges, (long long)values, ex.hdr.denom, phi_dev);
+        if (inter) { /* one CTA per row, its triangle in shared memory */
+            const unsigned blocks = (unsigned)std::min<int64_t>(n, (int64_t)m->sm_count * 8);
+            k_tree_shap_interactions_finish<<<blocks, 256, (size_t)values * sizeof(double), st>>>(b.scratch, (int)ranges, n_rows, F, ex.hdr.denom,
+                                                                                                  out_dev);
+        } else {
+            const int64_t n_values = n * F;
+            const unsigned blocks = (unsigned)std::min<int64_t>((n_values + 255) / 256, (int64_t)m->sm_count * 8);
+            k_tree_shap_finish<<<blocks, 256, 0, st>>>(b.scratch, (int)ranges, (long long)n_values, ex.hdr.denom, out_dev);
+        }
         e = cudaGetLastError();
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_tree_shap_finish launch failed: %s", cudaGetErrorString(e));
-        m->launches++;
-    }
-    return B2F_OK;
-}
-
-template <int MAXL>
-static auto inter_kernel(bool pk) {
-    return pk ? k_tree_shap_interactions<MAXL, true> : k_tree_shap_interactions<MAXL, false>;
-}
-static auto inter_kernel_for(int maxl, bool pk) {
-    return maxl <= 9 ? inter_kernel<9>(pk) : (maxl <= 16 ? inter_kernel<16>(pk) : inter_kernel<24>(pk));
-}
-
-/* phi2_dev[n][fields][fields] for n device rows of format fmt, on stream st, partial triangles in b's scratch */
-static int launch_interactions(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, double *phi2_dev, ExplainBuf &b) {
-    if (n <= 0) return B2F_OK;
-    const Explainer &ex = *m->ex;
-    const int F = explain_fields(m), T = inter_slots(F);
-    if (ex.hdr.n_paths == 0) {
-        CUDA_TRY(cudaMemsetAsync(phi2_dev, 0, (size_t)n * F * F * sizeof(double), st));
-        return B2F_OK;
-    }
-    const int64_t ranges = explain_ranges(m, n, B2F_OUT_INTERACTIONS);
-    if (ranges > 1) {
-        int rc = explain_reserve_scratch(b, st, (size_t)ranges * (size_t)n * T * sizeof(double));
-        if (rc) return rc;
-    }
-    const dim3 grid((unsigned)((n + 31) / 32), (unsigned)ranges);
-    inter_kernel_for(ex.maxl, fmt == B2F_ROWS_PACKED64)<<<grid, B2F_SHAP_THREADS, ex.inter_smem_bytes, st>>>(
-        ex.ip, static_cast<const uint32_t *>(rows_dev), (long long)n, phi2_dev, b.scratch);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_tree_shap_interactions launch failed: %s", cudaGetErrorString(e));
-    m->launches++;
-    if (ranges > 1) {
-        const unsigned blocks = (unsigned)std::min<int64_t>(n, (int64_t)m->sm_count * 8);
-        k_tree_shap_interactions_finish<<<blocks, 256, (size_t)T * sizeof(double), st>>>(b.scratch, (int)ranges, (long long)n, F, ex.hdr.denom,
-                                                                                         phi2_dev);
-        e = cudaGetLastError();
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_tree_shap_interactions_finish launch failed: %s", cudaGetErrorString(e));
+        if (e != cudaSuccess) return set_err(B2F_ECUDA, "%s_finish launch failed: %s", name, cudaGetErrorString(e));
         m->launches++;
     }
     return B2F_OK;
@@ -1228,9 +1211,8 @@ static int submit_chunk(b2f_model *m, Slot &sl, const void *rows, int fmt, int k
     CUDA_TRY(cudaMemcpyAsync(sl.d_rows, static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, (size_t)cnt * row_bytes, cudaMemcpyHostToDevice,
                              sl.stream));
     mark();
-    rc = kind == B2F_OUT_EXPLAIN        ? launch_explain(m, sl.stream, sl.d_rows, cnt, fmt, eb->out, *eb)
-         : kind == B2F_OUT_INTERACTIONS ? launch_interactions(m, sl.stream, sl.d_rows, cnt, fmt, eb->out, *eb)
-                                        : out_launch(m, sl.stream, sl.d_rows, cnt, fmt, kind, out ? sl.d_proba : nullptr, label ? sl.d_label : nullptr);
+    rc = explain ? launch_explain(m, sl.stream, sl.d_rows, cnt, fmt, kind, eb->out, *eb)
+                 : out_launch(m, sl.stream, sl.d_rows, cnt, fmt, kind, out ? sl.d_proba : nullptr, label ? sl.d_label : nullptr);
     if (rc) return rc;
     mark();
     if (out)
@@ -1253,18 +1235,19 @@ static int enqueue_host_batch(b2f_model *m, const void *rows, int64_t n, int fmt
     rc = check_row_format(m, fmt);
     if (rc) return rc;
     CUDA_TRY(cudaSetDevice(m->device));
-    const bool inter = kind == B2F_OUT_INTERACTIONS;
-    int64_t chunk = inter ? B2F_INTER_CHUNK_ROWS : m->chunk_rows;
+    const int64_t fixed_chunk = fixed_chunk_rows(kind);
+    int64_t chunk = fixed_chunk ? fixed_chunk : m->chunk_rows;
     if (n <= chunk + chunk / 2) chunk = n; /* small batch: one H2D, one launch */
     static const bool timeline = getenv("B2F_TIMELINE") != nullptr;
     std::vector<cudaEvent_t> tev;
     /* chunk schedule: equal chunks by default; a plan (B2F_CHUNK_PLAN="a,b,c": fractions of the batch in
      * 1/1024ths, the last chunk takes the remainder) front-loads the copies so the un-overlapped tail --
      * the last chunk's kernel and D2H -- is short */
+    const bool planned = !fixed_chunk && !m->chunk_plan.empty() && chunk != n && n >= 2 * m->chunk_rows;
     int c = 0;
     for (int64_t off = 0; off < n; ++c) {
         int64_t cnt = std::min(chunk, n - off);
-        if (!inter && !m->chunk_plan.empty() && chunk != n && n >= 2 * m->chunk_rows) {
+        if (planned) {
             cnt = (size_t)c < m->chunk_plan.size() ? std::max<int64_t>(1024, (n * m->chunk_plan[c] / 1024 + 1023) / 1024 * 1024) : n - off;
             cnt = std::min(cnt, n - off);
         }
@@ -1466,14 +1449,13 @@ extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_
     Explainer *ex = new (std::nothrow) Explainer();
     if (!ex) return set_err(B2F_ENOMEM, "out of host memory");
     auto fail = [&](int code) {
-        if (ex->d_table) cudaFree(ex->d_table);
-        delete ex;
+        explainer_free(ex);
         return code;
     };
     ex->hdr = h;
     if (cudaMalloc(&ex->d_table, nbytes) != cudaSuccess || cudaMemcpy(ex->d_table, paths, nbytes, cudaMemcpyHostToDevice) != cudaSuccess)
         return fail(set_err(B2F_ENOMEM, "path table upload (%zu bytes) failed: %s", nbytes, cudaGetErrorString(cudaGetLastError())));
-    SParams &sp = ex->sp;
+    SParams &sp = ex->ip.s;
     memset(&sp, 0, sizeof(sp));
     sp.paths = reinterpret_cast<const b2f_path *>(static_cast<uint8_t *>(ex->d_table) + h.paths_off);
     sp.elems = reinterpret_cast<const b2f_path_elem *>(static_cast<uint8_t *>(ex->d_table) + h.elems_off);
@@ -1483,7 +1465,7 @@ extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_
     sp.denom = h.denom;
     memcpy(sp.impute, m->hdr.impute, sizeof(sp.impute));
     ex->maxl = h.max_len <= 9 ? 9 : (h.max_len <= 16 ? 16 : 24);
-    ex->smem_bytes = shap_smem_bytes((int)(h.n_cat + h.n_num));
+    inter_assign(static_cast<const uint8_t *>(paths), h, ex->ip.own);
     /* the EXTEND / UNWIND factors (no division in the kernel) */
     double tab[4][B2F_SHAP_TAB_L][B2F_SHAP_TAB_L]; /* per call: concurrent attaches (other handles) share nothing on the host */
     for (int l = 0; l < B2F_SHAP_TAB_L; ++l)
@@ -1494,29 +1476,16 @@ extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_
             tab[3][l][i] = l > i ? (l + 1.0) / (l - i) : 0.0;
         }
     cudaError_t e = cudaMemcpyToSymbol(c_shap_tab, tab, sizeof(tab));
-    for (bool pk : {false, true})
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(shap_kernel_for(ex->maxl, pk), cudaFuncAttributeMaxDynamicSharedMemorySize, ex->smem_bytes);
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ex->ctas_per_sm, shap_kernel_for(ex->maxl, false), B2F_SHAP_THREADS, ex->smem_bytes);
-    ex->ip.s = sp;
-    inter_assign(static_cast<const uint8_t *>(paths), h, ex->ip.own);
-    ex->inter_smem_bytes = inter_smem_bytes((int)(h.n_cat + h.n_num));
-    for (bool pk : {false, true})
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(inter_kernel_for(ex->maxl, pk), cudaFuncAttributeMaxDynamicSharedMemorySize, ex->inter_smem_bytes);
-    if (e == cudaSuccess)
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ex->inter_ctas_per_sm, inter_kernel_for(ex->maxl, false), B2F_SHAP_THREADS,
-                                                          ex->inter_smem_bytes);
-    if (e != cudaSuccess) return fail(set_err(B2F_ECUDA, "explainer set-up failed: %s", cudaGetErrorString(e)));
-    ex->ctas_per_sm = std::max(1, ex->ctas_per_sm);
-    ex->inter_ctas_per_sm = std::max(1, ex->inter_ctas_per_sm);
-    if (m->ex) { /* the device was synchronised above */
-        for (ExplainBuf *b = m->ex->slots; b <= &m->ex->compute; ++b) {
-            if (b->out) cudaFree(b->out);
-            if (b->scratch) cudaFree(b->scratch);
-        }
-        cudaFree(m->ex->d_table);
-        delete m->ex;
+    for (int kind : {B2F_OUT_EXPLAIN, B2F_OUT_INTERACTIONS}) {
+        ExplainKernel &k = ex->kernels[kind - B2F_OUT_EXPLAIN];
+        k.smem_bytes = kind == B2F_OUT_INTERACTIONS ? inter_smem_bytes(sp.n_cat + sp.n_num) : shap_smem_bytes(sp.n_cat + sp.n_num);
+        for (bool pk : {false, true})
+            if (e == cudaSuccess) e = cudaFuncSetAttribute(explain_kernel(kind, ex->maxl, pk), cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem_bytes);
+        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k.ctas_per_sm, explain_kernel(kind, ex->maxl, false), B2F_SHAP_THREADS, k.smem_bytes);
+        k.ctas_per_sm = std::max(1, k.ctas_per_sm);
     }
+    if (e != cudaSuccess) return fail(set_err(B2F_ECUDA, "explainer set-up failed: %s", cudaGetErrorString(e)));
+    if (m->ex) explainer_free(m->ex); /* the device was synchronised above */
     m->ex = ex;
     return B2F_OK;
 }
@@ -1575,8 +1544,7 @@ static int explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row
     if (rc == B2F_OK) rc = check_row_format(m, row_format);
     if (rc) return rc;
     CUDA_TRY(cudaSetDevice(m->device));
-    return kind == B2F_OUT_INTERACTIONS ? launch_interactions(m, m->compute, rows_dev, n, row_format, out_dev, m->ex->compute)
-                                        : launch_explain(m, m->compute, rows_dev, n, row_format, out_dev, m->ex->compute);
+    return launch_explain(m, m->compute, rows_dev, n, row_format, kind, out_dev, m->ex->compute);
 }
 extern "C" int b2f_explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev) {
     return explain_device(m, rows_dev, n, row_format, phi_dev, B2F_OUT_EXPLAIN);

@@ -64,6 +64,25 @@ __device__ __forceinline__ uint32_t shap_row_word(const SParams &p, const uint32
     return v;
 }
 
+/* xs[f * 32 + c] = imputed word f of the tile's row row0 + c (0 past n), for f < F; all threads of the CTA */
+template <bool PACKED>
+__device__ __forceinline__ void shap_stage_tile(const SParams &p, const uint32_t *__restrict__ rows, long long n, long long row0, int F, uint32_t *xs) {
+    for (int i = threadIdx.x; i < 32 * F; i += B2F_SHAP_THREADS) {
+        const long long row = row0 + (i & 31);
+        xs[i] = row < n ? shap_row_word<PACKED>(p, rows, row, i >> 5) : 0u;
+    }
+}
+
+/* a[j] for a run-time j < N, reading a at compile-time indices only (so a stays in registers) */
+template <int N>
+__device__ __forceinline__ double shap_pick(const double (&a)[N], int j) {
+    double v = a[0];
+#pragma unroll
+    for (int k = 1; k < N; ++k)
+        if (k == j) v = a[k];
+    return v;
+}
+
 /* does this lane's row follow the path at element e?  -> also the element's field and zero-fraction pair */
 __device__ __forceinline__ bool shap_follows(const b2f_path_elem *e, const uint32_t *xs, int lane, uint32_t &field, double &z, double &iz) {
     const uint4 q0 = __ldg(reinterpret_cast<const uint4 *>(e));
@@ -85,16 +104,11 @@ __device__ __forceinline__ bool shap_follows(const b2f_path_elem *e, const uint3
     return above && below;
 }
 
-/* one path for this warp's 32 rows: EXTEND, then the closed-form UNWIND sum per element, added into my[field][lane] */
+/* EXTEND over the len elements E[0..len) of one path (E[0] the bias) for this lane's row: pw[0..len) the path's polynomial,
+ * pw[len..MAXL) = 0, and ones bit k set when the row follows element k (bit 0 always).  Returns pw[len - 1]. */
 template <int MAXL>
-__device__ __forceinline__ void shap_path(const SParams &p, int q, const uint32_t *xs, double *my, int lane) {
-    /* a 24-byte record is 8-byte aligned only: {first, len} and the leaf are two 8-byte loads */
-    const uint2 rec = __ldg(reinterpret_cast<const uint2 *>(p.paths + q));
-    const double leaf = __ldg(&p.paths[q].leaf);
-    const int len = (int)rec.y;
-    const b2f_path_elem *E = p.elems + rec.x;
-    double pw[MAXL];
-    uint32_t ones = 1u; /* bit k: this lane's row follows the path at element k (the bias always) */
+__device__ __forceinline__ double shap_extend(const b2f_path_elem *E, int len, const uint32_t *xs, int lane, double (&pw)[MAXL], uint32_t &ones) {
+    ones = 1u;
     pw[0] = 1.0;
 #pragma unroll
     for (int l = 1; l < MAXL; ++l) {
@@ -112,30 +126,58 @@ __device__ __forceinline__ void shap_path(const SParams &p, int q, const uint32_
             }
         }
     }
-    const int d = len - 1;
-    double last = pw[0];
+    return shap_pick(pw, len - 1);
+}
+
+/* The closed-form UNWIND of one element out of the polynomial pw[0..d] (d < N, last = pw[d]): the sum of the unwound
+ * polynomial's d entries.  o: the row follows the element, z / iz: its zero fraction and reciprocal.  STORE: w[0..N-1)
+ * also receives the unwound entries (0 from d on), the polynomial of the path without the element. */
+template <bool STORE, int N>
+__device__ __forceinline__ double shap_unwound_sum(const double (&pw)[N], int d, double last, bool o, double z, double iz, double *w = nullptr) {
+    double tot = 0.0;
+    if (o) {
+        double nxt = last;
 #pragma unroll
-    for (int j = 1; j < MAXL; ++j)
-        if (j == d) last = pw[j];
+        for (int i = N - 2; i >= 0; --i) {
+            if constexpr (STORE) w[i] = 0.0;
+            if (i < d) {
+                const double tmp = nxt * c_shap_tab[2][d][i];
+                if constexpr (STORE) w[i] = tmp;
+                tot += tmp;
+                nxt = pw[i] - tmp * z * c_shap_tab[1][d][i];
+            }
+        }
+    } else {
+#pragma unroll
+        for (int i = N - 2; i >= 0; --i) {
+            if constexpr (STORE) w[i] = 0.0;
+            if (i < d) {
+                const double tmp = pw[i] * iz * c_shap_tab[3][d][i];
+                if constexpr (STORE) w[i] = tmp;
+                tot += tmp;
+            }
+        }
+    }
+    return tot;
+}
+
+/* one path for this warp's 32 rows: EXTEND, then the closed-form UNWIND sum per element, added into my[field][lane] */
+template <int MAXL>
+__device__ __forceinline__ void shap_path(const SParams &p, int q, const uint32_t *xs, double *my, int lane) {
+    /* a 24-byte record is 8-byte aligned only: {first, len} and the leaf are two 8-byte loads */
+    const uint2 rec = __ldg(reinterpret_cast<const uint2 *>(p.paths + q));
+    const double leaf = __ldg(&p.paths[q].leaf);
+    const int len = (int)rec.y;
+    const b2f_path_elem *E = p.elems + rec.x;
+    double pw[MAXL];
+    uint32_t ones;
+    const double last = shap_extend(E, len, xs, lane, pw, ones);
+    const int d = len - 1;
     for (int k = 1; k < len; ++k) {
         const double2 zz = __ldg(reinterpret_cast<const double2 *>(E + k) + 2);
         const uint32_t field = __ldg(&E[k].field);
         const bool o = (ones >> k) & 1u;
-        double tot = 0.0;
-        if (o) {
-            double nxt = last;
-#pragma unroll
-            for (int i = MAXL - 2; i >= 0; --i)
-                if (i < d) {
-                    const double tmp = nxt * c_shap_tab[2][d][i];
-                    tot += tmp;
-                    nxt = pw[i] - tmp * zz.x * c_shap_tab[1][d][i];
-                }
-        } else {
-#pragma unroll
-            for (int i = MAXL - 2; i >= 0; --i)
-                if (i < d) tot += pw[i] * zz.y * c_shap_tab[3][d][i];
-        }
+        const double tot = shap_unwound_sum<false>(pw, d, last, o, zz.x, zz.y);
         my[field * 32 + lane] += tot * ((o ? 1.0 : 0.0) - zz.x) * leaf;
     }
 }
@@ -152,10 +194,7 @@ __global__ void __launch_bounds__(B2F_SHAP_THREADS, 2)
     double *acc = reinterpret_cast<double *>(shap_smem + 24 * 32 * 4); /* [warps][F][32] */
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long row0 = (long long)blockIdx.x * 32;
-    for (int i = threadIdx.x; i < 32 * F; i += B2F_SHAP_THREADS) {
-        const long long row = row0 + (i & 31);
-        xs[i] = row < n ? shap_row_word<PACKED>(p, rows, row, i >> 5) : 0u;
-    }
+    shap_stage_tile<PACKED>(p, rows, n, row0, F, xs);
     double *my = acc + (size_t)warp * F * 32;
     for (int f = 0; f < F; ++f) my[f * 32 + lane] = 0.0;
     __syncthreads();

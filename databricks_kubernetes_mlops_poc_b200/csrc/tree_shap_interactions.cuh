@@ -58,86 +58,27 @@ __device__ __forceinline__ void inter_path(const IParams &ip, uint32_t own, int 
     if (!(held & own)) return;
     const double leaf = __ldg(&p.paths[q].leaf);
     double pw[MAXL];
-    uint32_t ones = 1u;
-    pw[0] = 1.0;
-#pragma unroll
-    for (int l = 1; l < MAXL; ++l) {
-        pw[l] = 0.0;
-        if (l < len) {
-            uint32_t field;
-            double z, iz;
-            const bool o = shap_follows(E + l, xs, lane, field, z, iz);
-            ones |= (uint32_t)o << l;
-#pragma unroll
-            for (int i = l - 1; i >= 0; --i) {
-                const double pi = pw[i];
-                if (o) pw[i + 1] = fma(pi, c_shap_tab[0][l][i], pw[i + 1]);
-                pw[i] = z * pi * c_shap_tab[1][l][i];
-            }
-        }
-    }
+    uint32_t ones;
+    const double last = shap_extend(E, len, xs, lane, pw, ones);
     const int d = len - 1;
-    double last = pw[0];
-#pragma unroll
-    for (int j = 1; j < MAXL; ++j)
-        if (j == d) last = pw[j];
     for (int ka = 1; ka < len; ++ka) {
         const uint32_t fa = __ldg(&E[ka].field);
         if (!((own >> fa) & 1u)) continue;
         const double2 za = __ldg(reinterpret_cast<const double2 *>(E + ka) + 2);
         const bool oa = (ones >> ka) & 1u;
-        /* w = pw with a unwound (d entries), tot = their sum */
-        double w[MAXL - 1];
-        double tot = 0.0;
-        if (oa) {
-            double nxt = last;
-#pragma unroll
-            for (int i = MAXL - 2; i >= 0; --i) {
-                w[i] = 0.0;
-                if (i < d) {
-                    w[i] = nxt * c_shap_tab[2][d][i];
-                    tot += w[i];
-                    nxt = pw[i] - w[i] * za.x * c_shap_tab[1][d][i];
-                }
-            }
-        } else {
-#pragma unroll
-            for (int i = MAXL - 2; i >= 0; --i) {
-                w[i] = 0.0;
-                if (i < d) {
-                    w[i] = pw[i] * za.y * c_shap_tab[3][d][i];
-                    tot += w[i];
-                }
-            }
-        }
+        double w[MAXL - 1]; /* pw with a unwound (d entries) */
+        const double tot = shap_unwound_sum<true>(pw, d, last, oa, za.x, za.y, w);
         const double ga = ((oa ? 1.0 : 0.0) - za.x) * leaf;
         acc[inter_slot(F, (int)fa, (int)fa) * 32 + lane] += tot * ga;
         const double ha = 0.5 * ga;
         const int e = d - 1; /* w holds e + 1 entries */
-        double wlast = w[0];
-#pragma unroll
-        for (int j = 1; j < MAXL - 1; ++j)
-            if (j == e) wlast = w[j];
+        const double wlast = shap_pick(w, e);
         for (int kb = 1; kb < len; ++kb) {
             const uint32_t fb = __ldg(&E[kb].field);
             if (fb <= fa) continue; /* the pair belongs to the owner of the lower field; fa itself is met once */
             const double2 zb = __ldg(reinterpret_cast<const double2 *>(E + kb) + 2);
             const bool ob = (ones >> kb) & 1u;
-            double t = 0.0;
-            if (ob) {
-                double nxt = wlast;
-#pragma unroll
-                for (int i = MAXL - 3; i >= 0; --i)
-                    if (i < e) {
-                        const double tmp = nxt * c_shap_tab[2][e][i];
-                        t += tmp;
-                        nxt = w[i] - tmp * zb.x * c_shap_tab[1][e][i];
-                    }
-            } else {
-#pragma unroll
-                for (int i = MAXL - 3; i >= 0; --i)
-                    if (i < e) t += w[i] * zb.y * c_shap_tab[3][e][i];
-            }
+            const double t = shap_unwound_sum<false>(w, e, wlast, ob, zb.x, zb.y);
             acc[inter_slot(F, (int)fa, (int)fb) * 32 + lane] += t * ha * ((ob ? 1.0 : 0.0) - zb.x);
         }
     }
@@ -163,10 +104,7 @@ __global__ void __launch_bounds__(B2F_SHAP_THREADS, InterBlocks<MAXL>::value)
     double *acc = reinterpret_cast<double *>(inter_smem + 24 * 32 * 4); /* [T][32] */
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long row0 = (long long)blockIdx.x * 32;
-    for (int i = threadIdx.x; i < 32 * F; i += B2F_SHAP_THREADS) {
-        const long long row = row0 + (i & 31);
-        xs[i] = row < n ? shap_row_word<PACKED>(p, rows, row, i >> 5) : 0u;
-    }
+    shap_stage_tile<PACKED>(p, rows, n, row0, F, xs);
     for (int i = threadIdx.x; i < 32 * T; i += B2F_SHAP_THREADS) acc[i] = 0.0;
     __syncthreads();
 

@@ -187,14 +187,7 @@ class ForestEngine:
     def explain_rows(self, rows: np.ndarray, device_ms: bool = False):
         """Encoded rows (N, 24) or packed (N, 16) -> (phi float64 (N, n_cat + n_num), base_value[, device ms]): exact
         path-dependent TreeSHAP per request field, in probability (RandomForest) or log-odds (GBDT) space."""
-        rows = np.ascontiguousarray(rows)
-        fmt = self._fmt(rows)
-        n = rows.shape[0]
-        inf = self.info()
-        phi = np.empty((n, inf["n_cat"] + inf["n_num"]), dtype=np.float64)
-        base, ms = C.c_double(0.0), C.c_float(0.0)
-        check(self._lib.b2f_explain(self._h, ptr(rows), n, fmt, ptr(phi), C.byref(base), C.byref(ms)), "b2f_explain")
-        return (phi, base.value, ms.value) if device_ms else (phi, base.value)
+        return self._explained("b2f_explain", 1, rows, device_ms)
 
     def explain_device(self, rows_dev: int, n: int, phi_dev: int, fmt: int = ROWS_WORDS24) -> None:
         """Enqueue an explanation of device-resident rows into device phi (n x fields doubles); ``sync`` waits."""
@@ -204,20 +197,23 @@ class ForestEngine:
         """Encoded rows (N, 24) or packed (N, 16) -> (phi2 float64 (N, F, F), base_value[, device ms]) with F = n_cat + n_num:
         exact path-dependent SHAP interaction values per pair of request fields.  Each matrix is symmetric, its rows sum to
         ``explain_rows``' phi and its total to the prediction - base_value."""
-        rows = np.ascontiguousarray(rows)
-        fmt = self._fmt(rows)
-        n = rows.shape[0]
-        inf = self.info()
-        F = inf["n_cat"] + inf["n_num"]
-        phi2 = np.empty((n, F, F), dtype=np.float64)
-        base, ms = C.c_double(0.0), C.c_float(0.0)
-        check(self._lib.b2f_explain_interactions(self._h, ptr(rows), n, fmt, ptr(phi2), C.byref(base), C.byref(ms)),
-              "b2f_explain_interactions")
-        return (phi2, base.value, ms.value) if device_ms else (phi2, base.value)
+        return self._explained("b2f_explain_interactions", 2, rows, device_ms)
 
     def explain_interactions_device(self, rows_dev: int, n: int, phi2_dev: int, fmt: int = ROWS_WORDS24) -> None:
         """Enqueue interaction values of device-resident rows into device phi2 (n x fields x fields doubles); ``sync`` waits."""
         check(self._lib.b2f_explain_interactions_device(self._h, rows_dev, n, fmt, phi2_dev), "b2f_explain_interactions_device")
+
+    def _explained(self, fn: str, field_axes: int, rows: np.ndarray, device_ms: bool):
+        """C function ``fn`` (b2f_explain / b2f_explain_interactions) on host rows into float64 of shape (N,) + (F,) * field_axes
+        with F = n_cat + n_num -> (values, base_value[, device ms])."""
+        rows = np.ascontiguousarray(rows)
+        fmt = self._fmt(rows)
+        n = rows.shape[0]
+        inf = self.info()
+        out = np.empty((n,) + (inf["n_cat"] + inf["n_num"],) * field_axes, dtype=np.float64)
+        base, ms = C.c_double(0.0), C.c_float(0.0)
+        check(getattr(self._lib, fn)(self._h, ptr(rows), n, fmt, ptr(out), C.byref(base), C.byref(ms)), fn)
+        return (out, base.value, ms.value) if device_ms else (out, base.value)
 
     # ------------------------------------------------------------------ device-resident interface
     def device_alloc(self, nbytes: int) -> int:

@@ -264,11 +264,7 @@ class B200Model:
         ``predict`` returns; a multi-GPU ``predict`` slices the batch over all GPUs and may differ from them in the last bits.
         Calls on one handle must not overlap: a caller that also scores on ``replicas[0]`` from other threads serialises the
         two (the HTTP server takes the first batcher worker's lock)."""
-        df, rows = self._explain_rows(model_input)
-        phi, base = self.engine.explain_rows(rows)
-        proba, _ = self.replicas[0].score(df, want_outliers=False)
-        return {"feature_names": list(self.all_features), "output": self.explain_output, "base_value": float(base),
-                "contributions": phi, "predictions": proba.tolist()}
+        return self._explained(model_input, "explain_rows", "contributions")
 
     def explain_interactions(self, model_input) -> dict:
         """Exact path-dependent SHAP interaction values of every pair of request fields for every row's score.
@@ -279,20 +275,20 @@ class B200Model:
         row of the matrix sums to ``explain``'s contribution of that field and the whole matrix to the prediction -
         base_value.  Any model with an explainer has them; the same rules as ``explain`` apply (first GPU's handle only,
         predictions from ``replicas[0].score`` with the classifier alone, RuntimeError without an explainer)."""
-        df, rows = self._explain_rows(model_input)
-        phi2, base = self.engine.explain_interactions_rows(rows)
-        proba, _ = self.replicas[0].score(df, want_outliers=False)
-        return {"feature_names": list(self.all_features), "output": self.explain_output, "base_value": float(base),
-                "interactions": phi2, "predictions": proba.tolist()}
+        return self._explained(model_input, "explain_interactions_rows", "interactions")
 
-    def _explain_rows(self, model_input):
+    def _explained(self, model_input, method: str, key: str) -> dict:
+        """``engine.<method>`` on the encoded rows, answered as ``key`` beside the keys both explanations share."""
         if self.explain_blob is None:
             raise RuntimeError("this model has no explainer: build it with from_pipeline(..., explain=True) or load a model directory "
                                f"that holds {EXPLAIN_FILE} (save_model_dir(..., explain_blob=flatten_explainer(pipeline)))")
         df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
         if len(df.columns) == 0:
             raise KeyError(f"None of {self.all_features} are in the [columns]")
-        return df, self.encoder.encode_frame(df)
+        values, base = getattr(self.engine, method)(self.encoder.encode_frame(df))
+        proba, _ = self.replicas[0].score(df, want_outliers=False)
+        return {"feature_names": list(self.all_features), "output": self.explain_output, "base_value": float(base),
+                key: values, "predictions": proba.tolist()}
 
 
 def _reject_nan(df: pd.DataFrame, numeric_features) -> None:
