@@ -575,13 +575,19 @@ static int rank_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
     if (env.rank_off) return B2F_OK;
     const int64_t layout_bytes = (int64_t)m->rk.layout.size();
     const int64_t base = B2F_RANK_XS_BYTES /* alignment slack */ + (int64_t)B2F_RANK_PARTIALS * 32 * 8 + 256;
-    int max_tiles = (int)std::min<int64_t>(B2F_RANK_MAX_TILES, ((int64_t)m->max_smem_optin - base - layout_bytes) / B2F_RANK_XS_BYTES);
-    max_tiles = std::min(max_tiles, env.rank_max_tiles);
-    /* resident while the whole layout fits next to a useful number of row tiles; otherwise it streams through a two-slot ring
-     * in pieces of 8 trees (2 groups of 4: warp w owns (tile w / 2, group w mod 2), so <= 16 tiles per round) */
-    m->rank_stream = env.rank_stream < 0 ? max_tiles < 8 : env.rank_stream != 0;
-    int64_t forest_smem = layout_bytes;
     m->rank_u = env.rank_u;
+    /* resident: the CTA copies and walks the first ceil(n_trees / U) groups only (stub trees complete the last one) */
+    const int n_groups = (m->rk.n_trees + m->rank_u - 1) / m->rank_u;
+    const int64_t walked_bytes = (int64_t)n_groups * m->rank_u * m->rk.tree_stride;
+    int max_tiles = (int)std::min<int64_t>(B2F_RANK_MAX_TILES, ((int64_t)m->max_smem_optin - base - walked_bytes) / B2F_RANK_XS_BYTES);
+    max_tiles = std::min(max_tiles, env.rank_max_tiles);
+    /* resident while the walked trees fit next to a useful number of row tiles and their top levels fit the parameter block's
+     * table; otherwise the layout streams through a two-slot ring in pieces of 8 trees (2 groups of 4: warp w owns
+     * (tile w / 2, group w mod 2), so <= 16 tiles per round) */
+    const bool top_fits = m->rk.n_trees <= B2F_RANK_TOP_TREES;
+    if (env.rank_stream == 0 && !top_fits) return B2F_OK; /* resident forced but impossible: no rank kernel */
+    m->rank_stream = env.rank_stream < 0 ? (max_tiles < 8 || !top_fits) : env.rank_stream != 0;
+    int64_t forest_smem = walked_bytes;
     if (m->rank_stream) {
         m->rank_u = 4;
         const int64_t piece = 8 * (int64_t)m->rk.tree_stride; /* n_trees_padded is a multiple of 8 */
@@ -594,9 +600,17 @@ static int rank_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
     RParams &rp = m->rp;
     memset(&rp, 0, sizeof(rp));
     rp.layout = static_cast<const uint8_t *>(m->d_rank_layout);
-    rp.layout_bytes = (uint32_t)layout_bytes;
+    rp.layout_bytes = (uint32_t)(m->rank_stream ? layout_bytes : walked_bytes);
     rp.tree_stride = m->rk.tree_stride;
     rp.n_trees_padded = m->rk.n_trees_padded;
+    rp.n_groups = n_groups;
+    if (!m->rank_stream) {
+        for (int t = 0; t < m->rk.n_trees; ++t) {
+            const uint32_t *nodes = reinterpret_cast<const uint32_t *>(m->rk.layout.data() + (size_t)t * m->rk.tree_stride);
+            rp.top_root[t] = nodes[0];
+            if (m->rk.depth >= 2) rp.top_kids[t] = make_uint2(nodes[1], nodes[2]); /* stumps have no level 1 */
+        }
+    }
     rp.depth = m->rk.depth;
     rp.agg_mode = (int)m->hdr.agg_mode;
     rp.n_cat = m->rk.n_cat;

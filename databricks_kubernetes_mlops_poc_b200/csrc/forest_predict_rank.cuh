@@ -55,12 +55,14 @@
 #define B2F_RANK_MAX_TILES 16                       /* 32-row tiles per CTA per round */
 #define B2F_RANK_XS_BYTES 8192                      /* per tile: 64 words x 32 lanes x 4 B (128 16-bit values per lane), 8 KB aligned */
 #define B2F_RANK_PARTIALS (B2F_RANK_WARPS + B2F_RANK_MAX_TILES)
+#define B2F_RANK_TOP_TREES 288                      /* resident forests: trees whose level-0/1 node words ride in RParams::top_* */
 
 struct RParams {
     const uint8_t *layout;   /* device: n_trees_padded complete trees, tree_stride bytes each */
-    uint32_t layout_bytes;   /* multiple of 16 */
+    uint32_t layout_bytes;   /* resident: the first n_groups * U trees (what the CTA copies); STREAM: all of them. Multiple of 16 */
     uint32_t tree_stride;    /* 2^D * 12 */
     int32_t n_trees_padded;  /* multiple of 8 */
+    int32_t n_groups;        /* resident: tree groups walked per tile, ceil(n_trees / U); later groups hold stub trees only */
     int32_t depth;
     int32_t agg_mode;
     int32_t n_cat;
@@ -88,7 +90,13 @@ struct RParams {
     int32_t phase_launch;       /* this launch's index; launches at or past phase_launches record nothing */
     int32_t phase_launches;
 #endif
+    /* resident: tree t's root word and its two level-1 words {first child, second child}, read by the walk from the
+     * constant bank (one warp-uniform load each) instead of shared memory; zero for stub trees.  Unused when STREAM. */
+    uint32_t top_root[B2F_RANK_TOP_TREES];
+    uint2 top_kids[B2F_RANK_TOP_TREES];
 };
+/* the whole parameter block (RParams + 5 pointer-sized arguments) stays under the classic 4 KB kernel-parameter limit */
+static_assert(sizeof(RParams) + 5 * 8 <= 4096, "rank kernel parameters exceed 4 KB");
 
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -123,14 +131,19 @@ __device__ __forceinline__ uint32_t lds_u16(uint32_t a) {
 
 /* walk U consecutive trees (first tree at shared address t0) for this lane's row; payloads are added in tree order.
  * A chain keeps the ABSOLUTE shared address a = B + 4i of its node (B = the tree's base): the child 2i+1 (+1) sits at
- * 2a - B + 4 (+4), i.e. one SEL between the two per-tree constants (4 - B, 8 - B) and one multiply-add (FMA pipe). */
-template <int D, int U>
-__device__ __forceinline__ void rank_walk_group(uint32_t t0, uint32_t tree_stride, uint32_t xs_lane, uint32_t m2, uint32_t m64k, uint32_t a64k,
-                                                double &acc) {
+ * 2a - B + 4 (+4), i.e. one SEL between the two per-tree constants (4 - B, 8 - B) and one multiply-add (FMA pipe).
+ * TOP (resident layout): the node words of levels 0 and 1 are the same for every lane of the warp, so they come from the
+ * parameter block (p.top_root / p.top_kids of tree `tree0 + u`, warp-uniform constant loads) and cost no shared-memory
+ * wavefront; level 1 picks its word on the level-0 outcome (ptxas: an LDC predicated on it).  Levels 2 .. D-1 read shared
+ * memory. */
+template <int D, int U, bool TOP>
+__device__ __forceinline__ void rank_walk_group(const RParams &p, int tree0, uint32_t t0, uint32_t xs_lane, double &acc) {
+    const uint32_t m2 = p.mul_two, m64k = p.mul_64k, a64k = p.add_64k;
     uint32_t at[U], k4[U], k8[U];
+    bool second0[U]; /* TOP: the level-0 outcome of each chain */
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-        at[u] = t0 + u * tree_stride;
+        at[u] = t0 + u * p.tree_stride;
         k4[u] = 4u - at[u];
         k8[u] = 8u - at[u];
     }
@@ -138,10 +151,20 @@ __device__ __forceinline__ void rank_walk_group(uint32_t t0, uint32_t tree_strid
     for (int d = 0; d < D; ++d) {
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            const uint32_t nw = lds32(at[u]);
+            uint32_t nw;
+            if (TOP && d == 0) {
+                nw = p.top_root[tree0 + u];
+            } else if (TOP && d == 1) {
+                const uint2 kids = p.top_kids[tree0 + u];
+                nw = second0[u] ? kids.y : kids.x;
+            } else {
+                nw = lds32(at[u]);
+            }
             const uint32_t v = lds_u16(xs_lane | (nw & 0x1F82u)); /* value[f] of this lane's row */
             const uint32_t x = v * m64k + a64k;                   /* (v << 16 | 0xFFFF) >= node  <=>  v >= t   (IMAD) */
-            at[u] = at[u] * m2 + (x >= nw ? k8[u] : k4[u]);       /* IMAD */
+            const bool second = x >= nw;
+            if (d == 0) second0[u] = second;
+            at[u] = at[u] * m2 + (second ? k8[u] : k4[u]);        /* IMAD */
         }
     }
     /* a = B + 4 (2^D - 1 + leaf): payload at B + 4 * 2^D + 8 * leaf = 2a - B - 4 * 2^D + 8 = (a + a + k4) + (4 - 4 * 2^D) */
@@ -194,7 +217,7 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
     const uint32_t tq = n_tiles / gridDim.x, tr = n_tiles % gridDim.x;
     const uint32_t tile0 = blockIdx.x * tq + min(blockIdx.x, tr), cta_tiles = tq + (blockIdx.x < tr ? 1u : 0u);
     const uint32_t n_rounds = (cta_tiles + (uint32_t)p.max_tiles - 1u) / (uint32_t)p.max_tiles;
-    const int groups = p.n_trees_padded / U; /* tree groups per tile */
+    const int groups = p.n_trees_padded / U; /* tree groups per tile in the work split (resident: the first n_groups are walked) */
     const uint32_t forest_addr = smem_addr(forest);
     const uint32_t xs_addr = smem_addr(xs_all);
     bool forest_ready = false;
@@ -279,7 +302,7 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
                 const uint32_t k = round * (uint32_t)p.n_pieces + (uint32_t)piece;
                 mbar_wait(&forest_bar[k & 1u], (k >> 1) & 1u);
                 if (k == 0) RANK_PHASE(FOREST_READY);
-                if (mine) rank_walk_group<D, U>(forest_addr + (k & 1u) * p.piece_bytes + g_off, p.tree_stride, xs_lane, p.mul_two, p.mul_64k, p.add_64k, acc);
+                if (mine) rank_walk_group<D, U, false>(p, 0, forest_addr + (k & 1u) * p.piece_bytes + g_off, xs_lane, acc);
                 __syncthreads(); /* every warp is done with this slot: refill it while the other slot is walked */
                 if (tid == 0 && piece + 2 < p.n_pieces) issue_piece(k + 2u);
             }
@@ -301,7 +324,9 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
             continue;
         }
 
-        /* ---- phase 2: walk.  units = T x groups, warp w takes [w * units / 32, (w + 1) * units / 32) ---- */
+        /* ---- phase 2: walk.  units = T x groups, warp w takes [w * units / 32, (w + 1) * units / 32); the units of a tile's
+         *      stub-only groups (g >= n_groups, zero payloads) are skipped, not walked, so the float64 partials keep the
+         *      grouping of the padded forest while no warp spends a wavefront on a stub ---- */
         {
             const int units = T * groups;
             int u = warp * units / B2F_RANK_WARPS; /* units <= 16 tiles x 128 groups: 32-bit */
@@ -311,8 +336,8 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
                 const int g_end = min(groups, u_end - t * groups);
                 const uint32_t xs_lane = xs_addr + (uint32_t)t * B2F_RANK_XS_BYTES + (uint32_t)lane * 4u;
                 double acc = 0.0;
-                for (int g = u - t * groups; g < g_end; ++g)
-                    rank_walk_group<D, U>(forest_addr + (uint32_t)(g * U) * p.tree_stride, p.tree_stride, xs_lane, p.mul_two, p.mul_64k, p.add_64k, acc);
+                for (int g = u - t * groups; g < min(g_end, p.n_groups); ++g)
+                    rank_walk_group<D, U, true>(p, g * U, forest_addr + (uint32_t)(g * U) * p.tree_stride, xs_lane, acc);
                 partial[(warp + t) * 32 + lane] = acc; /* slot (warp + tile) is unique to this (warp, tile) segment */
                 u = t * groups + g_end;
             }
