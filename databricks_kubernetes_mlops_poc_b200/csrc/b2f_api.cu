@@ -34,6 +34,7 @@
 #include "forest_rank.h"
 #include "tree_shap.cuh"
 #include "tree_shap_interactions.cuh"
+#include "tree_shap_interventional.cuh"
 #include "json_rows.h"
 #include "row_encoder.h"
 
@@ -134,10 +135,19 @@ struct ExplainBuf {
     size_t scratch_bytes = 0;
 };
 
-/* the launch shape of one explanation kernel (k_tree_shap or k_tree_shap_interactions) */
+/* the launch shape of one explanation kernel (k_tree_shap, k_tree_shap_interactions or k_tree_shap_interventional) */
 struct ExplainKernel {
     int smem_bytes = 0;
     int ctas_per_sm = 1; /* resident CTAs per SM */
+};
+
+/* an attached background set (b2f_model_attach_background; tree_shap_interventional.cuh) */
+struct Background {
+    void *d_table = nullptr; /* offsets[n_paths + 1] int64, then the {mask, count} entries */
+    size_t bytes = 0;
+    int64_t rows = 0;        /* 0: none attached */
+    double base_value = 0.0; /* mean over the background rows of the prediction, in the output space */
+    VParams vp{};            /* vp.s: the explainer's SParams with denom * rows */
 };
 
 /* an attached path table (b2f_model_attach_explainer) */
@@ -145,8 +155,9 @@ struct Explainer {
     b2f_paths_header hdr;
     void *d_table = nullptr;
     IParams ip;   /* k_tree_shap takes ip.s; k_tree_shap_interactions also each warp's fields (inter_assign) */
-    int maxl = 9; /* length bucket of both kernels: 9, 16 or 24 */
-    ExplainKernel kernels[2]; /* [kind - B2F_OUT_EXPLAIN] */
+    int maxl = 9; /* length bucket of the kernels: 9, 16 or 24 */
+    ExplainKernel kernels[3]; /* [kind - B2F_OUT_EXPLAIN] */
+    Background bg;            /* k_tree_shap_interventional's table (b2f_model_attach_background) */
     ExplainBuf slots[B2F_STREAMS];
     ExplainBuf compute; /* b2f_explain_device */
 };
@@ -817,6 +828,7 @@ static void explainer_free(Explainer *ex) {
         if (b->scratch) cudaFree(b->scratch);
     }
     if (ex->d_table) cudaFree(ex->d_table);
+    if (ex->bg.d_table) cudaFree(ex->bg.d_table);
     delete ex;
 }
 
@@ -1069,9 +1081,11 @@ static int out_launch(b2f_model *m, cudaStream_t st, const void *rows_dev, int64
  * B2F_OUT_EXPLAIN is an output kind of the host pipeline only: b2f_explain passes it to enqueue_host_batch, so explanations
  * ride the same chunking, slots and streams as scores.  It is not a B2F_OUT_* value: out_row_bytes does not know it, so the
  * predict entry points refuse it.  B2F_OUT_INTERACTIONS is its sibling for b2f_explain_interactions (tree_shap_interactions.cuh):
- * F x F doubles per row. */
+ * F x F doubles per row.  B2F_OUT_INTERVENTIONAL is the third, for b2f_explain_interventional (tree_shap_interventional.cuh):
+ * F doubles per row, against the attached background. */
 #define B2F_OUT_EXPLAIN 16
 #define B2F_OUT_INTERACTIONS 17
+#define B2F_OUT_INTERVENTIONAL 18
 /* rows per chunk of an interactions batch (4 232 B of output per row for 23 fields), with no chunk plan: every chunk of
  * 16 384 rows is 512 row tiles, more than the SMs hold at once, so it runs as one range and needs no scratch */
 #define B2F_INTER_CHUNK_ROWS 16384
@@ -1079,7 +1093,7 @@ static int out_launch(b2f_model *m, cudaStream_t st, const void *rows_dev, int64
 static int64_t fixed_chunk_rows(int kind) { return kind == B2F_OUT_INTERACTIONS ? B2F_INTER_CHUNK_ROWS : 0; }
 
 static int explain_fields(const b2f_model *m) { return (int)(m->hdr.n_cat + m->hdr.n_num); }
-static bool explain_kind(int kind) { return kind == B2F_OUT_EXPLAIN || kind == B2F_OUT_INTERACTIONS; }
+static bool explain_kind(int kind) { return kind >= B2F_OUT_EXPLAIN && kind <= B2F_OUT_INTERVENTIONAL; }
 static size_t explain_row_bytes(const b2f_model *m, int kind) {
     const size_t F = (size_t)explain_fields(m);
     return (kind == B2F_OUT_INTERACTIONS ? F * F : F) * sizeof(double);
@@ -1087,6 +1101,7 @@ static size_t explain_row_bytes(const b2f_model *m, int kind) {
 
 static int explain_check(const b2f_model *m, int fmt, int kind, bool have_out) {
     if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
+    if (kind == B2F_OUT_INTERVENTIONAL && !m->ex->bg.rows) return set_err(B2F_ESTATE, "no background attached (b2f_model_attach_background)");
     if (fmt == B2F_ROWS_RANKED)
         return set_err(B2F_EINVAL, "explanations take float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
     if (!have_out) return set_err(B2F_EINVAL, kind == B2F_OUT_INTERACTIONS ? "phi2 is NULL" : "phi is NULL");
@@ -1119,10 +1134,12 @@ template <int MAXL>
 static const void *explain_kernel_l(int kind, bool pk) {
     if (kind == B2F_OUT_INTERACTIONS)
         return pk ? (const void *)k_tree_shap_interactions<MAXL, true> : (const void *)k_tree_shap_interactions<MAXL, false>;
+    if (kind == B2F_OUT_INTERVENTIONAL)
+        return pk ? (const void *)k_tree_shap_interventional<MAXL, true> : (const void *)k_tree_shap_interventional<MAXL, false>;
     return pk ? (const void *)k_tree_shap<MAXL, true> : (const void *)k_tree_shap<MAXL, false>;
 }
-/* the kind's kernel for the path-length bucket maxl and the row format.  Both take (params, rows, n, out, partials): IParams
- * for interactions, its SParams otherwise. */
+/* the kind's kernel for the path-length bucket maxl and the row format.  All take (params, rows, n, out, partials): IParams
+ * for interactions, the background's VParams for interventional values, the SParams otherwise. */
 static const void *explain_kernel(int kind, int maxl, bool pk) {
     return maxl <= 9 ? explain_kernel_l<9>(kind, pk) : (maxl <= 16 ? explain_kernel_l<16>(kind, pk) : explain_kernel_l<24>(kind, pk));
 }
@@ -1132,8 +1149,10 @@ static const void *explain_kernel(int kind, int maxl, bool pk) {
 static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, int kind, double *out_dev, ExplainBuf &b) {
     if (n <= 0) return B2F_OK;
     Explainer &ex = *m->ex;
-    const bool inter = kind == B2F_OUT_INTERACTIONS;
-    const char *name = inter ? "k_tree_shap_interactions" : "k_tree_shap";
+    const bool inter = kind == B2F_OUT_INTERACTIONS, interv = kind == B2F_OUT_INTERVENTIONAL;
+    const char *name = inter ? "k_tree_shap_interactions" : (interv ? "k_tree_shap_interventional" : "k_tree_shap");
+    void *params = inter ? static_cast<void *>(&ex.ip) : (interv ? static_cast<void *>(&ex.bg.vp) : static_cast<void *>(&ex.ip.s));
+    const double denom = interv ? ex.bg.vp.s.denom : ex.hdr.denom; /* phi = sum / denom (interventional: / (denom * rows)) */
     const int F = explain_fields(m), values = inter ? inter_slots(F) : F; /* partial sums per row */
     if (ex.hdr.n_paths == 0) { /* every tree a single leaf: nothing moves away from base_value */
         CUDA_TRY(cudaMemsetAsync(out_dev, 0, (size_t)n * explain_row_bytes(m, kind), st));
@@ -1146,7 +1165,7 @@ static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, i
     }
     const uint32_t *rows = static_cast<const uint32_t *>(rows_dev);
     long long n_rows = n;
-    void *args[] = {inter ? static_cast<void *>(&ex.ip) : static_cast<void *>(&ex.ip.s), &rows, &n_rows, &out_dev, &b.scratch};
+    void *args[] = {params, &rows, &n_rows, &out_dev, &b.scratch};
     /* a failed launch is also the thread's last error, taken (and cleared) below as after <<< >>> */
     cudaLaunchKernel(explain_kernel(kind, ex.maxl, fmt == B2F_ROWS_PACKED64), dim3((unsigned)((n + 31) / 32), (unsigned)ranges),
                      dim3(B2F_SHAP_THREADS), args, (size_t)ex.kernels[kind - B2F_OUT_EXPLAIN].smem_bytes, st);
@@ -1156,12 +1175,12 @@ static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, i
     if (ranges > 1) {
         if (inter) { /* one CTA per row, its triangle in shared memory */
             const unsigned blocks = (unsigned)std::min<int64_t>(n, (int64_t)m->sm_count * 8);
-            k_tree_shap_interactions_finish<<<blocks, 256, (size_t)values * sizeof(double), st>>>(b.scratch, (int)ranges, n_rows, F, ex.hdr.denom,
+            k_tree_shap_interactions_finish<<<blocks, 256, (size_t)values * sizeof(double), st>>>(b.scratch, (int)ranges, n_rows, F, denom,
                                                                                                   out_dev);
         } else {
             const int64_t n_values = n * F;
             const unsigned blocks = (unsigned)std::min<int64_t>((n_values + 255) / 256, (int64_t)m->sm_count * 8);
-            k_tree_shap_finish<<<blocks, 256, 0, st>>>(b.scratch, (int)ranges, (long long)n_values, ex.hdr.denom, out_dev);
+            k_tree_shap_finish<<<blocks, 256, 0, st>>>(b.scratch, (int)ranges, (long long)n_values, denom, out_dev);
         }
         e = cudaGetLastError();
         if (e != cudaSuccess) return set_err(B2F_ECUDA, "%s_finish launch failed: %s", name, cudaGetErrorString(e));
@@ -1490,9 +1509,10 @@ extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_
             tab[3][l][i] = l > i ? (l + 1.0) / (l - i) : 0.0;
         }
     cudaError_t e = cudaMemcpyToSymbol(c_shap_tab, tab, sizeof(tab));
-    for (int kind : {B2F_OUT_EXPLAIN, B2F_OUT_INTERACTIONS}) {
+    for (int kind : {B2F_OUT_EXPLAIN, B2F_OUT_INTERACTIONS, B2F_OUT_INTERVENTIONAL}) {
         ExplainKernel &k = ex->kernels[kind - B2F_OUT_EXPLAIN];
-        k.smem_bytes = kind == B2F_OUT_INTERACTIONS ? inter_smem_bytes(sp.n_cat + sp.n_num) : shap_smem_bytes(sp.n_cat + sp.n_num);
+        const int F = sp.n_cat + sp.n_num;
+        k.smem_bytes = kind == B2F_OUT_INTERACTIONS ? inter_smem_bytes(F) : (kind == B2F_OUT_INTERVENTIONAL ? interv_smem_bytes(F) : shap_smem_bytes(F));
         for (bool pk : {false, true})
             if (e == cudaSuccess) e = cudaFuncSetAttribute(explain_kernel(kind, ex->maxl, pk), cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem_bytes);
         if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k.ctas_per_sm, explain_kernel(kind, ex->maxl, false), B2F_SHAP_THREADS, k.smem_bytes);
@@ -1504,11 +1524,12 @@ extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_
     return B2F_OK;
 }
 
-/* b2f_explain / b2f_explain_interactions: kind B2F_OUT_EXPLAIN or B2F_OUT_INTERACTIONS */
+/* b2f_explain / b2f_explain_interactions / b2f_explain_interventional: kind B2F_OUT_EXPLAIN, B2F_OUT_INTERACTIONS or
+ * B2F_OUT_INTERVENTIONAL */
 static int explain_host(b2f_model *m, const void *rows, int64_t n, int row_format, double *out, int kind, double *base_value, float *device_ms) {
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
     if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
-    if (base_value) *base_value = m->ex->hdr.base_value;
+    if (base_value) *base_value = kind == B2F_OUT_INTERVENTIONAL ? m->ex->bg.base_value : m->ex->hdr.base_value;
     if (device_ms) *device_ms = 0.0f;
     CUDA_TRY(cudaSetDevice(m->device));
     struct Events { /* destroyed on every return path */
@@ -1550,7 +1571,7 @@ extern "C" int b2f_explain_interactions(b2f_model *m, const void *rows, int64_t 
     return explain_host(m, rows, n, row_format, phi2, B2F_OUT_INTERACTIONS, base_value, device_ms);
 }
 
-/* b2f_explain_device / b2f_explain_interactions_device */
+/* b2f_explain_device / b2f_explain_interactions_device / b2f_explain_interventional_device */
 static int explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *out_dev, int kind) {
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
@@ -1565,6 +1586,92 @@ extern "C" int b2f_explain_device(b2f_model *m, const void *rows_dev, int64_t n,
 }
 extern "C" int b2f_explain_interactions_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi2_dev) {
     return explain_device(m, rows_dev, n, row_format, phi2_dev, B2F_OUT_INTERACTIONS);
+}
+
+/* The background table of n host rows (tree_shap_interventional.cuh): the rows' imputed words in tiles, a counting pass,
+ * the offsets (scanned on the host), one allocation sized from them, a fill pass.  base_value = the path table's
+ * path-dependent base value plus each path's move to the background mean (k_background_table), added in path order. */
+extern "C" int b2f_model_attach_background(b2f_model *m, const void *rows, int64_t n, int row_format, size_t *table_bytes) {
+    if (!m) return set_err(B2F_EINVAL, "model is NULL");
+    if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
+    if (n <= 0) return set_err(B2F_EINVAL, "background needs at least one row (n = %lld)", (long long)n);
+    if (!rows) return set_err(B2F_EINVAL, "rows is NULL");
+    if (row_format == B2F_ROWS_RANKED)
+        return set_err(B2F_EINVAL, "a background takes float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
+    int rc = check_row_format(m, row_format);
+    if (rc) return rc;
+    CUDA_TRY(cudaSetDevice(m->device));
+    Explainer &ex = *m->ex;
+    const int64_t P = ex.hdr.n_paths, tiles = (n + 31) / 32;
+    const int F = explain_fields(m);
+    const bool pk = row_format == B2F_ROWS_PACKED64;
+    Background bg;
+    bg.rows = n;
+    bg.vp.s = ex.ip.s;
+    bg.vp.s.denom = ex.hdr.denom * (double)n;
+    void *d_rows = nullptr, *d_words = nullptr, *d_counts = nullptr, *d_moved = nullptr;
+    auto done = [&](int code) { /* frees the scratch, and the new table unless it was attached */
+        for (void *b : {d_rows, d_words, d_counts, d_moved})
+            if (b) cudaFree(b);
+        if (code != B2F_OK && bg.d_table) cudaFree(bg.d_table);
+        return code;
+    };
+    auto cuda_fail = [&](const char *what) {
+        return done(set_err(B2F_ECUDA, "background %s failed: %s", what, cudaGetErrorString(cudaGetLastError())));
+    };
+    const size_t rows_bytes = (size_t)n * row_bytes_of(m, row_format), words_bytes = (size_t)tiles * F * 32 * sizeof(uint32_t);
+    if (cudaMalloc(&d_rows, rows_bytes) != cudaSuccess || cudaMalloc(&d_words, words_bytes) != cudaSuccess ||
+        cudaMalloc(&d_counts, (size_t)std::max<int64_t>(P, 1) * sizeof(long long)) != cudaSuccess ||
+        cudaMalloc(&d_moved, (size_t)std::max<int64_t>(P, 1) * sizeof(double)) != cudaSuccess)
+        return done(set_err(B2F_ENOMEM, "background scratch (%zu bytes of rows, %zu of words) allocation failed: %s", rows_bytes, words_bytes,
+                            cudaGetErrorString(cudaGetLastError())));
+    if (cudaMemcpy(d_rows, rows, rows_bytes, cudaMemcpyHostToDevice) != cudaSuccess) return cuda_fail("upload");
+    const uint32_t *rw = static_cast<const uint32_t *>(d_rows);
+    uint32_t *words = static_cast<uint32_t *>(d_words);
+    long long *counts = static_cast<long long *>(d_counts);
+    double *moved = static_cast<double *>(d_moved);
+    if (pk)
+        k_background_words<true><<<(unsigned)tiles, B2F_SHAP_THREADS>>>(bg.vp.s, rw, (long long)n, words);
+    else
+        k_background_words<false><<<(unsigned)tiles, B2F_SHAP_THREADS>>>(bg.vp.s, rw, (long long)n, words);
+    const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>(P, (int64_t)m->sm_count * 32));
+    if (P) k_background_table<false><<<grid, B2F_SHAP_THREADS>>>(bg.vp, words, (long long)n, counts, nullptr, nullptr);
+    if (cudaGetLastError() != cudaSuccess) return cuda_fail("counting pass");
+    std::vector<long long> off((size_t)P + 1, 0);
+    if (P && cudaMemcpy(off.data() + 1, counts, (size_t)P * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess)
+        return cuda_fail("counting pass");
+    for (int64_t p = 0; p < P; ++p) off[p + 1] += off[p];
+    const size_t off_bytes = off.size() * sizeof(long long);
+    bg.bytes = off_bytes + (size_t)off[P] * sizeof(uint2);
+    if (cudaMalloc(&bg.d_table, bg.bytes) != cudaSuccess) {
+        bg.d_table = nullptr;
+        return done(set_err(B2F_ENOMEM, "background table (%zu bytes) allocation failed: %s", bg.bytes, cudaGetErrorString(cudaGetLastError())));
+    }
+    bg.vp.offsets = static_cast<const long long *>(bg.d_table);
+    bg.vp.entries = reinterpret_cast<const uint2 *>(static_cast<uint8_t *>(bg.d_table) + off_bytes);
+    if (cudaMemcpy(bg.d_table, off.data(), off_bytes, cudaMemcpyHostToDevice) != cudaSuccess) return cuda_fail("offsets upload");
+    if (P)
+        k_background_table<true><<<grid, B2F_SHAP_THREADS>>>(bg.vp, words, (long long)n, nullptr, const_cast<uint2 *>(bg.vp.entries), moved);
+    if (cudaGetLastError() != cudaSuccess) return cuda_fail("fill pass");
+    std::vector<double> mv((size_t)P);
+    if (P && cudaMemcpy(mv.data(), moved, (size_t)P * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) return cuda_fail("fill pass");
+    double sum = 0.0;
+    for (double v : mv) sum += v;
+    bg.base_value = ex.hdr.base_value + sum / ex.hdr.denom;
+    /* replacing a background: nothing may still read the old table */
+    if (cudaDeviceSynchronize() != cudaSuccess) return cuda_fail("synchronise");
+    if (ex.bg.d_table) cudaFree(ex.bg.d_table);
+    ex.bg = bg;
+    if (table_bytes) *table_bytes = bg.bytes;
+    return done(B2F_OK);
+}
+
+extern "C" int b2f_explain_interventional(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi, double *base_value,
+                                          float *device_ms) {
+    return explain_host(m, rows, n, row_format, phi, B2F_OUT_INTERVENTIONAL, base_value, device_ms);
+}
+extern "C" int b2f_explain_interventional_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev) {
+    return explain_device(m, rows_dev, n, row_format, phi_dev, B2F_OUT_INTERVENTIONAL);
 }
 
 extern "C" int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned, int proba_is_f64,

@@ -51,6 +51,7 @@ class ForestEngine:
             raise B2FError(f"b2f_model_create(device={device}) failed: {_cabi.last_error()}")
         self._pinned: dict[str, PinnedBuffer] = {}
         self.explainer_attached = False
+        self.background_rows = 0
         inf = self.info()
         self.rank_words = inf["rank_row_bytes"] // 4 if inf["rank_ok"] else 0  # width of a ranked row, 0 = not available
 
@@ -183,6 +184,17 @@ class ForestEngine:
         buf = np.frombuffer(blob, dtype=np.uint8)
         check(self._lib.b2f_model_attach_explainer(self._h, ptr(buf), buf.size), "b2f_model_attach_explainer")
         self.explainer_attached = True
+        self.background_rows = 0  # the background belongs to the explainer it was attached to
+
+    def attach_background(self, rows: np.ndarray) -> int:
+        """Attach encoded background rows (N, 24) or packed (N, 16), N >= 1, for ``explain_interventional_rows``; replaces an
+        earlier background.  -> the device bytes of its compressed table."""
+        rows = np.ascontiguousarray(rows)
+        nbytes = C.c_size_t(0)
+        check(self._lib.b2f_model_attach_background(self._h, ptr(rows), rows.shape[0], self._fmt(rows), C.byref(nbytes)),
+              "b2f_model_attach_background")
+        self.background_rows = rows.shape[0]
+        return nbytes.value
 
     def explain_rows(self, rows: np.ndarray, device_ms: bool = False):
         """Encoded rows (N, 24) or packed (N, 16) -> (phi float64 (N, n_cat + n_num), base_value[, device ms]): exact
@@ -203,8 +215,19 @@ class ForestEngine:
         """Enqueue interaction values of device-resident rows into device phi2 (n x fields x fields doubles); ``sync`` waits."""
         check(self._lib.b2f_explain_interactions_device(self._h, rows_dev, n, fmt, phi2_dev), "b2f_explain_interactions_device")
 
+    def explain_interventional_rows(self, rows: np.ndarray, device_ms: bool = False):
+        """Encoded rows (N, 24) or packed (N, 16) -> (phi float64 (N, n_cat + n_num), base_value[, device ms]): exact
+        interventional TreeSHAP against the attached background (``attach_background``), the mean over background rows z of
+        the Shapley values of f(x_S, z_rest).  base_value is the mean prediction over the background, in the output space of
+        ``explain_rows``, and base_value + phi.sum(1) the prediction."""
+        return self._explained("b2f_explain_interventional", 1, rows, device_ms)
+
+    def explain_interventional_device(self, rows_dev: int, n: int, phi_dev: int, fmt: int = ROWS_WORDS24) -> None:
+        """Enqueue interventional values of device-resident rows into device phi (n x fields doubles); ``sync`` waits."""
+        check(self._lib.b2f_explain_interventional_device(self._h, rows_dev, n, fmt, phi_dev), "b2f_explain_interventional_device")
+
     def _explained(self, fn: str, field_axes: int, rows: np.ndarray, device_ms: bool):
-        """C function ``fn`` (b2f_explain / b2f_explain_interactions) on host rows into float64 of shape (N,) + (F,) * field_axes
+        """C function ``fn`` (b2f_explain / b2f_explain_interactions / b2f_explain_interventional) on host rows into float64 of shape (N,) + (F,) * field_axes
         with F = n_cat + n_num -> (values, base_value[, device ms])."""
         rows = np.ascontiguousarray(rows)
         fmt = self._fmt(rows)

@@ -36,13 +36,14 @@ BLOB_FILE = "forest.b2f.npz"
 OUTLIER_BLOB_FILE = "outlier.b2f"
 DRIFT_FILE = "drift_reference.npz"
 EXPLAIN_FILE = "explain.b2f"  # TreeSHAP path table (flatten_explainer); optional
+BACKGROUND_FILE = "explain_background.npz"  # background rows of interventional explanations (raw columns); optional
 OUTLIER_PICKLE = os.path.join("artifacts", "outlier.pkl")  # joblib.dump(outlier, ".../outlier.pkl"), 02-register-model.ipynb:264,326-328
 SKLEARN_PICKLE = os.path.join("artifacts", "classifier", "model", "model.pkl")  # MLflow layout, 02-register-model.ipynb:317-321
 
 
 class B200Model:
     def __init__(self, flat: FlatForest, devices=None, drift=None, proba_dtype=np.float64, outlier_blob: bytes | None = None, host_threads: int = 0,
-                 explain_blob: bytes | None = None):
+                 explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None):
         self.flat = flat
         self.all_features = flat.all_features
         self.categorical_features = list(flat.cat_features)
@@ -66,6 +67,9 @@ class B200Model:
         self.explain_blob = explain_blob
         if explain_blob is not None:
             self.engine.attach_explainer(explain_blob)
+        self.background_rows = 0
+        if explain_background is not None:
+            self.attach_background(explain_background)
         # one scoring replica per GPU for the server's round-robin batcher (each has its own handle,
         # pinned staging and worker thread; the forest is replicated, rows are independent)
         engines = self.group.engines if self.group is not None else [self.engine]
@@ -79,13 +83,19 @@ class B200Model:
 
     # ------------------------------------------------------------------ construction
     @classmethod
-    def from_pipeline(cls, pipeline, reference_frame: pd.DataFrame | None = None, outlier=None, explain: bool = False, **kw) -> "B200Model":
+    def from_pipeline(cls, pipeline, reference_frame: pd.DataFrame | None = None, outlier=None, explain: bool = False,
+                      background: pd.DataFrame | None = None, **kw) -> "B200Model":
         """Fitted sklearn Pipeline (the reference's model.pkl) -> model on the GPU.
 
         ``outlier``: the reference's fitted outlier detector (an alibi-detect ``IForest`` or a bare sklearn
         ``IsolationForest`` plus ``outlier_threshold=``), flattened into a second forest over the same rows.
-        ``explain``: also build the TreeSHAP path table, so that ``explain()`` works."""
+        ``explain``: also build the TreeSHAP path table, so that ``explain()`` works.  ``background``: a frame of raw rows
+        (e.g. the training table) to attach for ``explain_interventional()``; it needs ``explain``."""
+        if background is not None and not explain:
+            raise ValueError("a background is for interventional explanations: pass explain=True with it")
         flat = flatten_pipeline(pipeline)
+        if background is not None:
+            kw["explain_background"] = background
         if explain:
             kw["explain_blob"] = flatten_explainer(pipeline, flat)
         drift = None
@@ -277,6 +287,37 @@ class B200Model:
         predictions from ``replicas[0].score`` with the classifier alone, RuntimeError without an explainer)."""
         return self._explained(model_input, "explain_interactions_rows", "interactions")
 
+    @property
+    def background_attached(self) -> bool:
+        return self.background_rows > 0
+
+    def attach_background(self, frame: pd.DataFrame) -> int:
+        """Attach the background set of ``explain_interventional``: raw rows (at least one) encoded as requests are, compressed
+        once on the first GPU; replaces an earlier background.  -> the device bytes of its table.  RuntimeError without an
+        explainer."""
+        if self.explain_blob is None:
+            raise RuntimeError("a background needs an explainer: build the model with from_pipeline(..., explain=True)")
+        nbytes = self.engine.attach_background(self.encoder.encode_frame(frame))
+        self.background_rows = len(frame)
+        return nbytes
+
+    def explain_interventional(self, model_input) -> dict:
+        """Exact interventional TreeSHAP contributions of every request field against the attached background set (what
+        shap's ``TreeExplainer(model, data)`` computes): the mean, over background rows z, of each field's Shapley value in
+        the game where the fields in S take the row's values and the others z's.  A field the model never reads gets 0, even
+        when it is correlated with one it reads.  With a one-row background this is baseline Shapley against that row.
+
+        -> ``explain``'s keys plus ``"background_rows"``; ``base_value`` is the mean over the background of the probability
+        (RandomForest) or raw margin (GBDT), and ``base_value + contributions[i].sum()`` row i's.  The same rules as
+        ``explain`` apply (first GPU's handle only, predictions from ``replicas[0].score``); RuntimeError without an explainer
+        or a background."""
+        if self.explain_blob is not None and not self.background_attached:
+            raise RuntimeError("this model has no background set: attach_background(frame), from_pipeline(..., background=frame) or a "
+                               f"model directory that holds {BACKGROUND_FILE} (save_model_dir(..., explain_background=frame))")
+        out = self._explained(model_input, "explain_interventional_rows", "contributions")
+        out["background_rows"] = self.background_rows
+        return out
+
     def _explained(self, model_input, method: str, key: str) -> dict:
         """``engine.<method>`` on the encoded rows, answered as ``key`` beside the keys both explanations share."""
         if self.explain_blob is None:
@@ -352,14 +393,17 @@ class _Replica:
 
 # ---------------------------------------------------------------------- loading
 def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | None = None, outlier_blob: bytes | None = None,
-                   explain_blob: bytes | None = None) -> None:
+                   explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None) -> None:
     """Write the GPU-side artefact next to (or instead of) the MLflow pickles.  ``explain_blob``: the TreeSHAP path table
-    (``flatten_explainer``), written as ``explain.b2f`` so that ``load_model`` attaches it."""
+    (``flatten_explainer``), written as ``explain.b2f`` so that ``load_model`` attaches it.  ``explain_background``: raw
+    rows written as ``explain_background.npz``, attached by ``load_model`` with the explainer."""
     os.makedirs(path, exist_ok=True)
     flat.save(os.path.join(path, BLOB_FILE))
     if explain_blob is not None:
         with open(os.path.join(path, EXPLAIN_FILE), "wb") as f:
             f.write(explain_blob)
+    if explain_background is not None:
+        _save_background(os.path.join(path, BACKGROUND_FILE), flat, explain_background)
     if outlier_blob is not None:
         with open(os.path.join(path, OUTLIER_BLOB_FILE), "wb") as f:
             f.write(outlier_blob)
@@ -367,6 +411,46 @@ def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | 
         from .drift import TabularDrift
 
         TabularDrift(reference_frame[flat.all_features], flat.cat_features, device=None).save(os.path.join(path, DRIFT_FILE))
+
+
+def _save_background(path: str, flat: FlatForest, frame: pd.DataFrame) -> None:
+    """The raw columns of ``flat.all_features``: numerics as float64, categories as ``U`` strings with ``null__<name>`` telling
+    a string (0) from None (1) and NaN (2), which the encoder maps differently."""
+    arrays = {}
+    for name in flat.all_features:
+        if name in flat.num_features:
+            arrays[name] = frame[name].to_numpy(dtype=np.float64)
+            continue
+        col = frame[name].to_numpy(dtype=object)
+        null = np.array([_null_kind(name, v) for v in col], dtype=np.uint8)
+        arrays[name] = np.array([v if isinstance(v, str) else "" for v in col], dtype="U")
+        arrays[f"null__{name}"] = null
+    np.savez(path, **arrays)
+
+
+def _null_kind(name: str, v) -> int:
+    if isinstance(v, str):
+        return 0
+    if v is None:
+        return 1
+    if isinstance(v, float) and v != v:
+        return 2
+    raise ValueError(f"background column {name!r}: {v!r} is not a string, None or NaN")
+
+
+def _load_background(path: str, flat: FlatForest) -> pd.DataFrame:
+    with np.load(path, allow_pickle=False) as z:
+        cols = {}
+        for name in flat.all_features:
+            if name in flat.num_features:
+                cols[name] = z[name]
+                continue
+            v = z[name].astype(object)
+            null = z[f"null__{name}"]
+            v[null == 1] = None
+            v[null == 2] = np.nan
+            cols[name] = v
+    return pd.DataFrame(cols)
 
 
 def _load_outlier_blob(path: str, flat: FlatForest):
@@ -427,4 +511,7 @@ def load_model(path: str, devices=None, **kw) -> B200Model:
     if "explain_blob" not in kw and os.path.exists(explain_path) and os.environ.get("B200_EXPLAIN", "gpu") != "off":
         with open(explain_path, "rb") as f:
             kw["explain_blob"] = f.read()
+        background_path = os.path.join(path, BACKGROUND_FILE)
+        if "explain_background" not in kw and os.path.exists(background_path):
+            kw["explain_background"] = _load_background(background_path, flat)
     return B200Model(flat, devices=devices, drift=drift, outlier_blob=outlier_blob, **kw)

@@ -239,15 +239,17 @@ def create_app(model=None, loader=None) -> FastAPI:
 
     app = FastAPI(title=_service_name(), docs_url="/", lifespan=lifespan)
 
-    async def explained(request: Request, method: str, key: str) -> Response:
-        """The body and error rules of /explain and /explain/interactions: parse like /predict, 501 without an explainer, run
-        ``model.<method>`` under the first batcher worker's lock and answer its ``key`` array as nested lists."""
+    async def explained(request: Request, method: str, key: str, attached: str = "explainer_attached", missing: str = "explainer",
+                        extra: tuple = ()) -> Response:
+        """The body and error rules of the /explain routes: parse like /predict, 501 unless ``model.<attached>`` (the model has
+        a ``missing``), run ``model.<method>`` under the first batcher worker's lock and answer its ``key`` array as nested lists,
+        plus its ``extra`` keys."""
         input_df = parser.frame(await request.body())
         if len(input_df) == 0:
             raise KeyError(f"None of {ALL_FEATURES} are in the [columns]")
         m = ml_models["credit_default"]
-        if not getattr(m, "explainer_attached", False):
-            return Response(content=json.dumps({"detail": "this model has no explainer"}), status_code=501, media_type="application/json")
+        if not getattr(m, attached, False):
+            return Response(content=json.dumps({"detail": f"this model has no {missing}"}), status_code=501, media_type="application/json")
         batcher = ml_models["_batcher"]
 
         def run():
@@ -257,6 +259,7 @@ def create_app(model=None, loader=None) -> FastAPI:
         out = await asyncio.get_running_loop().run_in_executor(None, run)
         body = {"feature_names": list(out["feature_names"]), "output": out["output"], "base_value": float(out["base_value"]),
                 "predictions": list(out["predictions"]), key: np.asarray(out[key], dtype=np.float64).tolist()}
+        body.update({k: out[k] for k in extra})
         return Response(content=json.dumps(body, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
 
     @app.post("/explain", openapi_extra={"requestBody": _REQUEST_SCHEMA})
@@ -272,6 +275,15 @@ def create_app(model=None, loader=None) -> FastAPI:
         fields x fields matrix per applicant whose rows sum to /explain's contributions (same output space, base value and
         predictions).  501 when the model was loaded without an explainer."""
         return await explained(request, "explain_interactions", "interactions")
+
+    @app.post("/explain/interventional", openapi_extra={"requestBody": _REQUEST_SCHEMA})
+    async def explain_interventional(request: Request):
+        """Explain each applicant's score against the model's background set: exact interventional TreeSHAP, the mean over
+        background rows of each request field's Shapley value when the applicant's values replace the background row's (same
+        output space as /explain; base_value is the mean prediction over the background, whose size is background_rows).  A
+        field the model never reads gets 0.  501 when the model has no explainer or no background."""
+        return await explained(request, "explain_interventional", "contributions", "background_attached", "background set",
+                               ("background_rows",))
 
     @app.post("/predict", response_model=ModelOutput, openapi_extra={"requestBody": _REQUEST_SCHEMA})
     async def predict(request: Request):

@@ -336,6 +336,21 @@ int b2f_explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_fo
 int b2f_explain_interactions(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi2, double *base_value, float *device_ms);
 /* device-resident form: enqueued on the compute stream (asynchronous, like b2f_explain_device; b2f_sync waits) */
 int b2f_explain_interactions_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi2_dev);
+/* Interventional TreeSHAP against a background set (Lundberg et al., Nat. Mach. Intell. 2020, arXiv:1905.04610; what shap's
+ * TreeExplainer computes when given a dataset): phi[f] is the mean over background rows z of field f's Shapley value in the
+ * game v_z(S) = f(x_S, z_rest), the same players and output space as b2f_explain; with one background row it is baseline
+ * Shapley against that row.  base_value is the mean prediction over the background, and base_value + sum_f phi[f] is the
+ * row's prediction.  A field the model never reads gets exactly 0 however it correlates with the others.
+ * b2f_model_attach_background compresses the rows once: per path, the distinct patterns of the path's conditions the
+ * background rows satisfy, with their counts (*table_bytes, may be NULL: its device size).  rows: n >= 1 host rows,
+ * B2F_ROWS_WORDS24 or B2F_ROWS_PACKED64 (ranked rows or n <= 0: B2F_EINVAL; no explainer: B2F_ESTATE; the table does not
+ * fit: B2F_ENOMEM with its size).  It replaces an earlier background; the background belongs to the explainer, so attaching
+ * another explainer drops it. */
+int b2f_model_attach_background(b2f_model *m, const void *rows, int64_t n, int row_format, size_t *table_bytes);
+/* arguments, output buffers and errors as b2f_explain, plus B2F_ESTATE without a background */
+int b2f_explain_interventional(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi, double *base_value, float *device_ms);
+/* device-resident form: enqueued on the compute stream (asynchronous, like b2f_explain_device; b2f_sync waits) */
+int b2f_explain_interventional_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev);
 
 /* asynchronous form for the request-batching ring: buffers must be pinned and stay valid until
  * b2f_wait(ticket) returns.  proba_is_f64 selects double (1) or float (0) outputs. */
