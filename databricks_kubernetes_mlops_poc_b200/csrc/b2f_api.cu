@@ -771,7 +771,7 @@ static int streams_init(b2f_model *m) {
     CUDA_TRY(cudaStreamCreateWithFlags(&m->compute, cudaStreamNonBlocking));
     CUDA_TRY(cudaFuncSetAttribute(k_feature_moments, cudaFuncAttributeMaxDynamicSharedMemorySize, B2F_MOM_SMEM));
     m->mom_blocks = m->sm_count * 3; /* one full wave: 3 CTAs (3-stage 72 KB ring each) per SM */
-    CUDA_TRY(cudaMalloc(&m->d_mom_partials, (size_t)m->mom_blocks * B2F_MOM_VALUES * sizeof(double)));
+    CUDA_TRY(cudaMalloc(&m->d_mom_partials, (size_t)m->mom_blocks * B2F_MOM_PARTIAL_VALUES * sizeof(double)));
     CUDA_TRY(cudaMalloc(&m->d_mom_ticket, sizeof(unsigned int)));
     CUDA_TRY(cudaMemset(m->d_mom_ticket, 0, sizeof(unsigned int)));
     CUDA_TRY(cudaMalloc(&m->d_mom_out, B2F_MOM_VALUES * sizeof(double)));
