@@ -32,6 +32,7 @@ SCORED_FULL_DTYPE = np.dtype(  # b2f_scored_full, 24 bytes
     [("proba1", np.float64), ("label", np.int32), ("is_outlier", np.int32), ("outlier_score", np.float32), ("reserved", np.int32)]
 )
 MOMENT_VALUES = ROW_WORDS * 3
+PD_PROBE_DTYPE = np.dtype([("word", np.int32), ("grid_offset", np.int32), ("count", np.int32)])  # b2f_pd_probe
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG_DIR, "lib", "libb200forest.so")
@@ -170,6 +171,11 @@ SIGNATURES = {
     "b2f_model_attach_background": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "b2f_explain_interventional": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_float)]),
     "b2f_explain_interventional_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
+    "b2f_partial_dependence": (
+        C.c_int,
+        [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)],
+    ),
+    "b2f_partial_dependence_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "b2f_predict_async_ex": (
         C.c_int,
         [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_uint64)],

@@ -32,6 +32,7 @@
 #include "forest_predict_tile.cuh"
 #include "forest_predict_rank.cuh"
 #include "forest_rank.h"
+#include "partial_dependence.cuh"
 #include "tree_shap.cuh"
 #include "tree_shap_interactions.cuh"
 #include "tree_shap_interventional.cuh"
@@ -162,6 +163,17 @@ struct Explainer {
     ExplainBuf compute; /* b2f_explain_device */
 };
 
+/* partial dependence (b2f_partial_dependence; partial_dependence.cuh).  The forest fields of pp are set at model creation;
+ * segs, grid and points are the current call's. */
+struct Dependence {
+    PdParams pp;
+    int n_segs = 0;
+    std::vector<uint32_t> spec;    /* the call's PdSeg table, then its grid words */
+    ExplainBuf slots[B2F_STREAMS]; /* .out: the curves of a host call's chunk */
+    ExplainBuf host;               /* .scratch: a host call's spec on the device */
+    ExplainBuf compute;            /* .scratch: the device form's spec */
+};
+
 struct TicketRec {
     uint64_t id = 0;
     cudaEvent_t ev[B2F_STREAMS] = {nullptr, nullptr, nullptr, nullptr};
@@ -205,6 +217,7 @@ struct b2f_model {
     void *d_blob = nullptr;
     int64_t forest_bytes = 0;
     Explainer *ex = nullptr; /* attached TreeSHAP path table (b2f_model_attach_explainer) */
+    Dependence pd;
     b2f_model *outlier = nullptr; /* attached isolation forest (b2f_model_attach_outlier_forest): a child handle on the
                                      same device whose kernels are launched on this handle's streams and rows */
     Slot slots[B2F_STREAMS];
@@ -680,6 +693,22 @@ static int warp_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
         kp.g[g].n_leaf_slots = gt[g].n_leaf_slots;
         kp.g[g].depth = gt[g].depth;
     }
+    PdParams &pp = m->pd.pp;
+    memset(&pp, 0, sizeof(pp));
+    pp.chunks = kp.chunks;
+    pp.n_groups = kp.n_groups;
+    pp.agg_mode = kp.agg_mode;
+    pp.n_cat = kp.n_cat;
+    pp.n_num = kp.n_num;
+    pp.init_raw = kp.init_raw;
+    pp.denom = kp.denom;
+    pp.threshold = kp.threshold;
+    memcpy(pp.impute, kp.impute, sizeof(pp.impute));
+    for (uint32_t g = 0; g < m->hdr.n_groups; ++g) {
+        pp.g_off[g] = gt[g].chunk_off;
+        pp.g_slots[g] = gt[g].n_slots;
+        pp.g_trees[g] = gt[g].n_trees;
+    }
 
     /* the packed 64-byte row needs the credit-default shape: exactly 9 categoricals of <= 126 categories, <= 14 numerics */
     m->packed_ok = m->hdr.n_cat == 9 && m->hdr.n_num <= 14; /* the kernels decode word L-7 / q[2+k] for exactly nine 7-bit fields */
@@ -838,6 +867,10 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
     cudaDeviceSynchronize();
     if (m->outlier) b2f_model_destroy(m->outlier);
     if (m->ex) explainer_free(m->ex);
+    for (ExplainBuf *b = m->pd.slots; b <= &m->pd.compute; ++b) {
+        if (b->out) cudaFree(b->out);
+        if (b->scratch) cudaFree(b->scratch);
+    }
     if (m->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(m->comm);
     for (int s = 0; s < B2F_STREAMS; ++s) {
         Slot &sl = m->slots[s];
@@ -1086,11 +1119,22 @@ static int out_launch(b2f_model *m, cudaStream_t st, const void *rows_dev, int64
 #define B2F_OUT_EXPLAIN 16
 #define B2F_OUT_INTERACTIONS 17
 #define B2F_OUT_INTERVENTIONAL 18
+/* B2F_OUT_DEPENDENCE: b2f_partial_dependence's curves, the call's total grid points in doubles per row (partial_dependence.cuh) */
+#define B2F_OUT_DEPENDENCE 19
 /* rows per chunk of an interactions batch (4 232 B of output per row for 23 fields), with no chunk plan: every chunk of
  * 16 384 rows is 512 row tiles, more than the SMs hold at once, so it runs as one range and needs no scratch */
 #define B2F_INTER_CHUNK_ROWS 16384
+/* device bytes of one chunk's partial-dependence curves: the chunk's rows are this over the row's bytes, 1 024 to 16 384 */
+#define B2F_PD_CHUNK_BYTES (64ll << 20)
+static int64_t pd_chunk_rows(const b2f_model *m) {
+    const int64_t rows = B2F_PD_CHUNK_BYTES / ((int64_t)m->pd.pp.points * (int64_t)sizeof(double));
+    return std::max<int64_t>(1024, std::min<int64_t>(B2F_CHUNK_ROWS, rows / 32 * 32));
+}
 /* the fixed rows per chunk of a host batch of this kind, or 0: the model's chunk size and chunk plan */
-static int64_t fixed_chunk_rows(int kind) { return kind == B2F_OUT_INTERACTIONS ? B2F_INTER_CHUNK_ROWS : 0; }
+static int64_t fixed_chunk_rows(const b2f_model *m, int kind) {
+    if (kind == B2F_OUT_DEPENDENCE) return pd_chunk_rows(m);
+    return kind == B2F_OUT_INTERACTIONS ? B2F_INTER_CHUNK_ROWS : 0;
+}
 
 static int explain_fields(const b2f_model *m) { return (int)(m->hdr.n_cat + m->hdr.n_num); }
 static bool explain_kind(int kind) { return kind >= B2F_OUT_EXPLAIN && kind <= B2F_OUT_INTERVENTIONAL; }
@@ -1202,6 +1246,79 @@ static int explain_reserve_out(ExplainBuf &b, cudaStream_t st, int64_t rows, siz
     return B2F_OK;
 }
 
+/* ------------------------------------------------------------------ partial dependence (K6: partial_dependence.cuh)
+ * A call's probes and grid become one spec: a PdSeg per run of up to B2F_PD_SEG points of a probe, then every point's
+ * word in output order (a row's output is its probes' points, concatenated), numerics imputed as the kernels impute rows.
+ * The spec is checked and built on the host, uploaded once per call, and read by every chunk's launch. */
+static int pd_check(const b2f_model *m, int fmt, bool have_out) {
+    (void)m;
+    if (fmt == B2F_ROWS_RANKED)
+        return set_err(B2F_EINVAL, "partial dependence takes float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
+    if (!have_out) return set_err(B2F_EINVAL, "out is NULL");
+    return B2F_OK;
+}
+
+static int pd_prepare(b2f_model *m, const b2f_pd_probe *probes, int n_probes, const uint32_t *grid_words) {
+    const b2f_blob_header &h = m->hdr;
+    if (!probes || !grid_words) return set_err(B2F_EINVAL, "probes or grid_words is NULL");
+    if (n_probes < 1 || n_probes > B2F_PD_MAX_PROBES) return set_err(B2F_EINVAL, "n_probes = %d: expected 1..%d", n_probes, B2F_PD_MAX_PROBES);
+    if (h.max_depth > B2F_PD_STACK) return set_err(B2F_EINVAL, "partial dependence walks trees of depth <= %d; this forest has depth %u", B2F_PD_STACK, h.max_depth);
+    const int fields = (int)(h.n_cat + h.n_num);
+    std::vector<PdSeg> segs;
+    std::vector<uint32_t> words;
+    for (int i = 0; i < n_probes; ++i) {
+        const b2f_pd_probe pr = probes[i];
+        if (pr.word < 0 || pr.word >= fields) return set_err(B2F_EINVAL, "probe %d: row word %d outside the %d fields", i, pr.word, fields);
+        if (pr.count < 1 || pr.count > B2F_PD_MAX_POINTS) return set_err(B2F_EINVAL, "probe %d: %d grid points, expected 1..%d", i, pr.count, B2F_PD_MAX_POINTS);
+        if (pr.grid_offset < 0 || pr.grid_offset > B2F_PD_MAX_PROBES * B2F_PD_MAX_POINTS - pr.count)
+            return set_err(B2F_EINVAL, "probe %d: grid offset %d out of range", i, pr.grid_offset);
+        const bool cat = pr.word < (int)h.n_cat;
+        for (int k = 0; k < pr.count; ++k) {
+            uint32_t w = grid_words[pr.grid_offset + k];
+            if (cat) {
+                const int32_t code = (int32_t)w, vocab = h.vocab[pr.word];
+                if (code < -1 || (vocab > 0 && code >= vocab))
+                    return set_err(B2F_EINVAL, "probe %d point %d: category code %d outside [-1, %d)", i, k, code, vocab);
+            } else {
+                float f;
+                memcpy(&f, &w, sizeof(f));
+                if (std::isinf(f)) return set_err(B2F_ERANGE, "probe %d point %d: value is infinite or overflows float32", i, k);
+                if (std::isnan(f)) memcpy(&w, &h.impute[pr.word], sizeof(w));
+            }
+            if (k % B2F_PD_SEG == 0) segs.push_back(PdSeg{(uint32_t)pr.word, 0u, (uint32_t)words.size(), 0u});
+            segs.back().count++;
+            words.push_back(w);
+        }
+    }
+    Dependence &pd = m->pd;
+    pd.n_segs = (int)segs.size();
+    pd.pp.points = (int32_t)words.size();
+    pd.spec.assign(segs.size() * (sizeof(PdSeg) / sizeof(uint32_t)), 0u);
+    memcpy(pd.spec.data(), segs.data(), segs.size() * sizeof(PdSeg));
+    pd.spec.insert(pd.spec.end(), words.begin(), words.end());
+    return B2F_OK;
+}
+
+static size_t pd_row_bytes(const b2f_model *m) { return (size_t)m->pd.pp.points * sizeof(double); }
+
+/* out_dev[n][points] for n device rows of format fmt on stream st; spec_dev holds the call's spec */
+static int launch_dependence(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, double *out_dev, const void *spec_dev) {
+    if (n <= 0) return B2F_OK;
+    PdParams pp = m->pd.pp;
+    pp.segs = static_cast<const PdSeg *>(spec_dev);
+    pp.grid = reinterpret_cast<const uint32_t *>(pp.segs + m->pd.n_segs);
+    const dim3 grid((unsigned)((n + B2F_PD_WARPS * 32 - 1) / (B2F_PD_WARPS * 32)), (unsigned)m->pd.n_segs);
+    const uint32_t *rows = static_cast<const uint32_t *>(rows_dev);
+    if (fmt == B2F_ROWS_PACKED64)
+        k_partial_dependence<true><<<grid, B2F_PD_WARPS * 32, 0, st>>>(pp, rows, (long long)n, out_dev);
+    else
+        k_partial_dependence<false><<<grid, B2F_PD_WARPS * 32, 0, st>>>(pp, rows, (long long)n, out_dev);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_partial_dependence launch failed: %s", cudaGetErrorString(e));
+    m->launches++;
+    return B2F_OK;
+}
+
 /* ------------------------------------------------------------------ host-buffer pipeline */
 static int slot_reserve(b2f_model *m, Slot &sl, int64_t rows) {
     if (rows <= sl.cap_rows) return B2F_OK;
@@ -1235,16 +1352,17 @@ static int submit_chunk(b2f_model *m, Slot &sl, const void *rows, int fmt, int k
         marks->push_back(e);
     };
     if (marks && marks->empty()) mark();
-    const bool explain = explain_kind(kind);
-    ExplainBuf *eb = explain ? &m->ex->slots[&sl - m->slots] : nullptr;
-    const size_t row_bytes = row_bytes_of(m, fmt), out_bytes = explain ? explain_row_bytes(m, kind) : out_row_bytes(kind);
-    if (explain && (rc = explain_reserve_out(*eb, sl.stream, cnt, out_bytes))) return rc;
-    void *d_out = explain ? static_cast<void *>(eb->out) : sl.d_proba;
+    const bool explain = explain_kind(kind), dep = kind == B2F_OUT_DEPENDENCE;
+    ExplainBuf *eb = explain ? &m->ex->slots[&sl - m->slots] : (dep ? &m->pd.slots[&sl - m->slots] : nullptr);
+    const size_t row_bytes = row_bytes_of(m, fmt), out_bytes = explain ? explain_row_bytes(m, kind) : (dep ? pd_row_bytes(m) : out_row_bytes(kind));
+    if (eb && (rc = explain_reserve_out(*eb, sl.stream, cnt, out_bytes))) return rc;
+    void *d_out = eb ? static_cast<void *>(eb->out) : sl.d_proba;
     const bool records = kind == B2F_OUT_PAIRS || kind == B2F_OUT_FULL;
     CUDA_TRY(cudaMemcpyAsync(sl.d_rows, static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, (size_t)cnt * row_bytes, cudaMemcpyHostToDevice,
                              sl.stream));
     mark();
     rc = explain ? launch_explain(m, sl.stream, sl.d_rows, cnt, fmt, kind, eb->out, *eb)
+         : dep   ? launch_dependence(m, sl.stream, sl.d_rows, cnt, fmt, eb->out, m->pd.host.scratch)
                  : out_launch(m, sl.stream, sl.d_rows, cnt, fmt, kind, out ? sl.d_proba : nullptr, label ? sl.d_label : nullptr);
     if (rc) return rc;
     mark();
@@ -1261,14 +1379,16 @@ static int submit_chunk(b2f_model *m, Slot &sl, const void *rows, int fmt, int k
 static int enqueue_host_batch(b2f_model *m, const void *rows, int64_t n, int fmt, void *out, int kind, int32_t *label, uint32_t *used_mask) {
     *used_mask = 0;
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
-    int rc = explain_kind(kind) ? explain_check(m, fmt, kind, out || n == 0) : out_check(m, kind, fmt, out || n == 0);
+    int rc = explain_kind(kind)            ? explain_check(m, fmt, kind, out || n == 0)
+             : kind == B2F_OUT_DEPENDENCE ? pd_check(m, fmt, out || n == 0)
+                                          : out_check(m, kind, fmt, out || n == 0);
     if (rc) return rc;
     if (n == 0) return B2F_OK;
     if (!rows) return set_err(B2F_EINVAL, "rows is NULL");
     rc = check_row_format(m, fmt);
     if (rc) return rc;
     CUDA_TRY(cudaSetDevice(m->device));
-    const int64_t fixed_chunk = fixed_chunk_rows(kind);
+    const int64_t fixed_chunk = fixed_chunk_rows(m, kind);
     int64_t chunk = fixed_chunk ? fixed_chunk : m->chunk_rows;
     if (n <= chunk + chunk / 2) chunk = n; /* small batch: one H2D, one launch */
     static const bool timeline = getenv("B2F_TIMELINE") != nullptr;
@@ -1524,12 +1644,9 @@ extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_
     return B2F_OK;
 }
 
-/* b2f_explain / b2f_explain_interactions / b2f_explain_interventional: kind B2F_OUT_EXPLAIN, B2F_OUT_INTERACTIONS or
- * B2F_OUT_INTERVENTIONAL */
-static int explain_host(b2f_model *m, const void *rows, int64_t n, int row_format, double *out, int kind, double *base_value, float *device_ms) {
-    if (!m) return set_err(B2F_EINVAL, "model is NULL");
-    if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
-    if (base_value) *base_value = kind == B2F_OUT_INTERVENTIONAL ? m->ex->bg.base_value : m->ex->hdr.base_value;
+/* a synchronous host batch of an explanation or partial-dependence kind; device_ms (may be NULL): from the first H2D to the
+ * end of the last chunk */
+static int timed_host_batch(b2f_model *m, const void *rows, int64_t n, int row_format, double *out, int kind, float *device_ms) {
     if (device_ms) *device_ms = 0.0f;
     CUDA_TRY(cudaSetDevice(m->device));
     struct Events { /* destroyed on every return path */
@@ -1561,6 +1678,15 @@ static int explain_host(b2f_model *m, const void *rows, int64_t n, int row_forma
                 *device_ms = std::max(*device_ms, ms);
             }
     return rc;
+}
+
+/* b2f_explain / b2f_explain_interactions / b2f_explain_interventional: kind B2F_OUT_EXPLAIN, B2F_OUT_INTERACTIONS or
+ * B2F_OUT_INTERVENTIONAL */
+static int explain_host(b2f_model *m, const void *rows, int64_t n, int row_format, double *out, int kind, double *base_value, float *device_ms) {
+    if (!m) return set_err(B2F_EINVAL, "model is NULL");
+    if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
+    if (base_value) *base_value = kind == B2F_OUT_INTERVENTIONAL ? m->ex->bg.base_value : m->ex->hdr.base_value;
+    return timed_host_batch(m, rows, n, row_format, out, kind, device_ms);
 }
 
 extern "C" int b2f_explain(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi, double *base_value, float *device_ms) {
@@ -1672,6 +1798,39 @@ extern "C" int b2f_explain_interventional(b2f_model *m, const void *rows, int64_
 }
 extern "C" int b2f_explain_interventional_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev) {
     return explain_device(m, rows_dev, n, row_format, phi_dev, B2F_OUT_INTERVENTIONAL);
+}
+
+/* the spec goes up once, before the chunks that read it; no earlier host call still reads it (each one synchronises) */
+extern "C" int b2f_partial_dependence(b2f_model *m, const void *rows, int64_t n, int row_format, const b2f_pd_probe *probes, int n_probes,
+                                      const uint32_t *grid_words, double *out, float *device_ms) {
+    if (!m) return set_err(B2F_EINVAL, "model is NULL");
+    if (device_ms) *device_ms = 0.0f;
+    int rc = pd_prepare(m, probes, n_probes, grid_words);
+    if (rc) return rc;
+    if (n > 0) {
+        if ((rc = pd_check(m, row_format, out != nullptr))) return rc;
+        CUDA_TRY(cudaSetDevice(m->device));
+        const size_t bytes = m->pd.spec.size() * sizeof(uint32_t);
+        if ((rc = explain_reserve_scratch(m->pd.host, m->compute, bytes))) return rc;
+        CUDA_TRY(cudaMemcpy(m->pd.host.scratch, m->pd.spec.data(), bytes, cudaMemcpyHostToDevice));
+    }
+    return timed_host_batch(m, rows, n, row_format, out, B2F_OUT_DEPENDENCE, device_ms);
+}
+/* the spec is copied on the compute stream into the device form's own buffer, so it is ordered with the launch */
+extern "C" int b2f_partial_dependence_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const b2f_pd_probe *probes,
+                                             int n_probes, const uint32_t *grid_words, double *out_dev) {
+    if (!m) return set_err(B2F_EINVAL, "model is NULL");
+    if (n < 0) return set_err(B2F_EINVAL, "negative row count");
+    int rc = pd_prepare(m, probes, n_probes, grid_words);
+    if (rc == B2F_OK) rc = pd_check(m, row_format, out_dev != nullptr || n == 0);
+    if (rc == B2F_OK) rc = check_row_format(m, row_format);
+    if (rc) return rc;
+    if (n == 0) return B2F_OK;
+    CUDA_TRY(cudaSetDevice(m->device));
+    const size_t bytes = m->pd.spec.size() * sizeof(uint32_t);
+    if ((rc = explain_reserve_scratch(m->pd.compute, m->compute, bytes))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(m->pd.compute.scratch, m->pd.spec.data(), bytes, cudaMemcpyHostToDevice, m->compute));
+    return launch_dependence(m, m->compute, rows_dev, n, row_format, out_dev, m->pd.compute.scratch);
 }
 
 extern "C" int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned, int proba_is_f64,

@@ -238,6 +238,28 @@ class ForestEngine:
         check(getattr(self._lib, fn)(self._h, ptr(rows), n, fmt, ptr(out), C.byref(base), C.byref(ms)), fn)
         return (out, base.value, ms.value) if device_ms else (out, base.value)
 
+    # ------------------------------------------------------------------ partial dependence (csrc/partial_dependence.cuh)
+    def partial_dependence_rows(self, rows: np.ndarray, probes, grid_words: np.ndarray, device_ms: bool = False):
+        """Encoded rows (N, 24) or packed (N, 16), probes [(row word, grid offset, count)] and the grid's row words ->
+        float64 (N, sum of counts)[, device ms]: column block p holds, for each row, the model's output with word
+        ``probes[p][0]`` replaced by each of its grid words in turn (a row's ICE curves, concatenated in probe order)."""
+        rows = np.ascontiguousarray(rows)
+        pr = _probe_table(probes)
+        grid = np.ascontiguousarray(grid_words, dtype=np.uint32)
+        out = np.empty((rows.shape[0], int(pr["count"].sum())), dtype=np.float64)
+        ms = C.c_float(0.0)
+        check(self._lib.b2f_partial_dependence(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(pr), len(pr), ptr(grid), ptr(out),
+                                               C.byref(ms)), "b2f_partial_dependence")
+        return (out, ms.value) if device_ms else out
+
+    def partial_dependence_device(self, rows_dev: int, n: int, probes, grid_words: np.ndarray, out_dev: int, fmt: int = ROWS_WORDS24) -> None:
+        """Enqueue the curves of device-resident rows into device out (n x sum of counts doubles); probes and grid words are
+        host arrays, as for ``partial_dependence_rows``; ``sync`` waits."""
+        pr = _probe_table(probes)
+        grid = np.ascontiguousarray(grid_words, dtype=np.uint32)
+        check(self._lib.b2f_partial_dependence_device(self._h, rows_dev, n, fmt, ptr(pr), len(pr), ptr(grid), out_dev),
+              "b2f_partial_dependence_device")
+
     # ------------------------------------------------------------------ device-resident interface
     def device_alloc(self, nbytes: int) -> int:
         p = self._lib.b2f_device_alloc(self._h, nbytes)
@@ -426,6 +448,11 @@ def _row_format(rows: np.ndarray, rank_words: int = 0) -> int:
         if rank_words and rows.shape[1] == rank_words:
             return ROWS_RANKED
     raise ValueError(f"rows must be uint32 (N, {ROW_WORDS}), packed (N, {PACKED_ROW_WORDS})" + (f" or ranked (N, {rank_words})" if rank_words else ""))
+
+
+def _probe_table(probes) -> np.ndarray:
+    """[(row word, grid offset, count)] -> b2f_pd_probe records."""
+    return np.array([tuple(int(v) for v in p) for p in probes], dtype=_cabi.PD_PROBE_DTYPE)
 
 
 def moments_merge(parts: np.ndarray) -> np.ndarray:

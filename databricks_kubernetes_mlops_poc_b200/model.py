@@ -26,6 +26,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pandas as pd
 
+from . import dependence
 from ._cabi import OUT_F64, OUT_FULL
 from ._pylists import ListBuilder
 from .encode import RowEncoder
@@ -68,6 +69,8 @@ class B200Model:
         if explain_blob is not None:
             self.engine.attach_explainer(explain_blob)
         self.background_rows = 0
+        self.background = None  # the attached background frame (raw columns)
+        self.dependence_grids = None  # field -> default partial-dependence grid of the background (attach_background)
         if explain_background is not None:
             self.attach_background(explain_background)
         # one scoring replica per GPU for the server's round-robin batcher (each has its own handle,
@@ -299,7 +302,61 @@ class B200Model:
             raise RuntimeError("a background needs an explainer: build the model with from_pipeline(..., explain=True)")
         nbytes = self.engine.attach_background(self.encoder.encode_frame(frame))
         self.background_rows = len(frame)
+        self.background = frame
+        self.dependence_grids = self._default_grids(frame, dependence.DEFAULT_RESOLUTION, dependence.DEFAULT_PERCENTILES)
         return nbytes
+
+    def _default_grids(self, frame: pd.DataFrame, grid_resolution: int, percentiles) -> dict:
+        """field -> its default grid over ``frame`` (``dependence.grid_from_column``); a field without a grid (no present
+        value, coinciding percentiles) is left out."""
+        grids = {}
+        for name in self.all_features:
+            try:
+                grids[name] = dependence.grid_from_column(frame[name], name in self.categorical_features, grid_resolution, percentiles)
+            except ValueError:
+                pass
+        return grids
+
+    def partial_dependence(self, model_input, features, *, kind: str = "average", grid_resolution: int = 100, percentiles=(0.05, 0.95),
+                           custom_values: dict | None = None, grid_frame: pd.DataFrame | None = None) -> dict:
+        """One-way partial dependence and ICE curves of request fields, as scikit-learn's
+        ``partial_dependence(pipeline, model_input, features, kind=..., method="brute", categorical_features=...)`` returns
+        them, one feature at a time.
+
+        -> ``{"feature_names": features, "output": "probability", "grid_values": [grid per feature], "average": [float64
+        (G_f,)], "individual": [float64 (n, G_f)]}``: ``individual[f][i, g]`` is P(class 1) for row i with field f set to
+        ``grid_values[f][g]`` (its own value ignored), bit for bit the tile kernel's score of that row; ``average`` (kind
+        "average" or "both") is its mean over rows, ``individual`` is there for "individual" and "both".  Duplicate names are
+        probed independently.  Grids: ``custom_values[f]`` when given (None / NaN = missing, imputed as in requests; an unknown
+        category behaves as any unknown category), else the default rule of ``dependence.grid_from_column`` over the column of
+        ``grid_frame``, or of ``model_input`` without one; missing values never enter a default grid.  At most 256 points per
+        feature and 23 features per call.  Every model has it, with or without an explainer.  Rows with NaN numerics are
+        accepted (the classifier alone is scored).  It runs on the first GPU's handle only, like ``explain``."""
+        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
+        if len(df.columns) == 0:
+            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        features = dependence.check_request(features, self.all_features, kind)
+        custom_values = dict(custom_values or {})
+        unknown = [f for f in custom_values if f not in self.all_features]
+        if unknown:
+            raise ValueError(f"custom_values for unknown feature(s) {unknown}")
+        source = df if grid_frame is None else grid_frame
+        grids, words, probes, off = [], [], [], 0
+        for name in features:
+            if name in custom_values:
+                grid = list(custom_values[name])
+            else:
+                grid = dependence.grid_from_column(source[name], name in self.categorical_features, grid_resolution, percentiles).tolist()
+            if not 1 <= len(grid) <= dependence.MAX_POINTS:
+                raise ValueError(f"feature {name!r}: {len(grid)} grid points, expected 1..{dependence.MAX_POINTS}")
+            grids.append(grid)
+            words.append(dependence.encode_grid(self.encoder, name, grid))
+            probes.append((dependence.word_of(self.encoder, name), off, len(grid)))
+            off += len(grid)
+        out = self.engine.partial_dependence_rows(self.encoder.encode_frame(df), probes, np.concatenate(words))
+        res = {"feature_names": features, "output": "probability", "grid_values": grids}
+        res.update(dependence.split_output(out, [len(g) for g in grids], kind))
+        return res
 
     def explain_interventional(self, model_input) -> dict:
         """Exact interventional TreeSHAP contributions of every request field against the attached background set (what

@@ -40,6 +40,7 @@ import numpy as np
 import pandas as pd
 from fastapi import FastAPI, Request, Response
 
+from . import dependence
 from .ingest import NativeRequestParser, parse_rows, rows_to_frame  # noqa: F401  (rows_to_frame re-exported)
 from .schema import ALL_FEATURES, LoanApplicant, ModelOutput
 
@@ -206,6 +207,56 @@ def _as_list(a: np.ndarray) -> list:
     return a.tolist()
 
 
+_DEPENDENCE_PARAMETERS = [
+    {"name": "feature", "in": "query", "required": True, "description": "request field to probe; repeat for several (at most 23)",
+     "schema": {"type": "array", "items": {"type": "string"}}, "style": "form", "explode": True},
+    {"name": "kind", "in": "query", "required": False, "schema": {"type": "string", "enum": list(dependence.KINDS), "default": "average"}},
+    {"name": "grid_resolution", "in": "query", "required": False,
+     "schema": {"type": "integer", "minimum": 2, "maximum": dependence.MAX_POINTS, "default": dependence.DEFAULT_RESOLUTION}},
+    {"name": "value", "in": "query", "required": False,
+     "description": "explicit grid point of the one probed field; repeat for several; empty = missing",
+     "schema": {"type": "array", "items": {"type": "string"}}, "style": "form", "explode": True},
+]
+
+
+def _dependence_problem(features, values, kind, grid_resolution) -> str | None:
+    """Why a /explain/dependence query is unprocessable, or None."""
+    if not features:
+        return "at least one feature parameter is needed"
+    if len(features) > dependence.MAX_FEATURES:
+        return f"at most {dependence.MAX_FEATURES} features per request"
+    unknown = [f for f in features if f not in ALL_FEATURES]
+    if unknown:
+        return f"unknown feature(s) {unknown}"
+    if kind not in dependence.KINDS:
+        return f"kind must be one of {list(dependence.KINDS)}"
+    if grid_resolution < 2:
+        return "grid_resolution must be at least 2"
+    if grid_resolution > dependence.MAX_POINTS or len(values) > dependence.MAX_POINTS:
+        return f"at most {dependence.MAX_POINTS} grid points per feature"
+    if values and len(features) != 1:
+        return "explicit values need exactly one feature"
+    return None
+
+
+def _unprocessable(detail: str) -> Response:
+    return Response(content=json.dumps({"detail": detail}), status_code=422, media_type="application/json")
+
+
+def _query_value(v: str, categorical: bool):
+    """A `value` query parameter -> a grid value: the string for a categorical field, else a float; empty = missing."""
+    if v == "":
+        return None
+    return v if categorical else float(v)
+
+
+def _json_value(v):
+    """A grid value for JSON: NaN (missing) -> null, numpy scalars -> Python."""
+    if isinstance(v, (float, np.floating)) and v != v:
+        return None
+    return v.item() if isinstance(v, np.generic) else v
+
+
 def _log_record(kind: str, request_id: str, payload) -> None:
     logging.info(json.dumps({"service_name": _service_name(), "type": kind, "request_id": request_id, "data": payload}))
 
@@ -284,6 +335,51 @@ def create_app(model=None, loader=None) -> FastAPI:
         field the model never reads gets 0.  501 when the model has no explainer or no background."""
         return await explained(request, "explain_interventional", "contributions", "background_attached", "background set",
                                ("background_rows",))
+
+    @app.post("/explain/dependence", openapi_extra={"requestBody": _REQUEST_SCHEMA, "parameters": _DEPENDENCE_PARAMETERS})
+    async def explain_dependence(request: Request):
+        """What-if curves: each applicant's default probability with one request field set to each point of a grid (ICE
+        curves, `individual`) and their mean over the applicants (partial dependence, `average`), one field at a time.  The
+        grid is the repeated `value` parameters (one field only), else the default grid of the model's background set when it
+        has one, else of the request rows.  422 for an unknown field, a bad kind, grid_resolution < 2 or more than 256
+        points."""
+        q = request.query_params
+        features, values, kind = q.getlist("feature"), q.getlist("value"), q.get("kind", "average")
+        try:
+            grid_resolution = int(q.get("grid_resolution", dependence.DEFAULT_RESOLUTION))
+        except ValueError:
+            return _unprocessable("grid_resolution must be an integer")
+        problem = _dependence_problem(features, values, kind, grid_resolution)
+        if problem:
+            return _unprocessable(problem)
+        input_df = parser.frame(await request.body())
+        if len(input_df) == 0:
+            raise KeyError(f"None of {ALL_FEATURES} are in the [columns]")
+        m = ml_models["credit_default"]
+        kw = {"kind": kind, "grid_resolution": grid_resolution}
+        if values:
+            name = features[0]
+            try:
+                kw["custom_values"] = {name: [_query_value(v, name in m.categorical_features) for v in values]}
+            except ValueError:
+                return _unprocessable(f"value parameters of numeric field {name!r} must be numbers")
+        elif getattr(m, "background_attached", False):
+            grids = m.dependence_grids if grid_resolution == dependence.DEFAULT_RESOLUTION else {}
+            kw["custom_values"] = {f: grids[f] for f in features if f in grids}
+            kw["grid_frame"] = m.background
+        batcher = ml_models["_batcher"]
+
+        def run():
+            with batcher.locks[0]:  # the first GPU's handle, which batcher worker 0 drives
+                return m.partial_dependence(input_df, features, **kw)
+
+        out = await asyncio.get_running_loop().run_in_executor(None, run)
+        body = {"feature_names": out["feature_names"], "output": out["output"],
+                "grid_values": [[_json_value(v) for v in g] for g in out["grid_values"]]}
+        for key in ("average", "individual"):
+            if key in out:
+                body[key] = [np.asarray(a, dtype=np.float64).tolist() for a in out[key]]
+        return Response(content=json.dumps(body, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
 
     @app.post("/predict", response_model=ModelOutput, openapi_extra={"requestBody": _REQUEST_SCHEMA})
     async def predict(request: Request):

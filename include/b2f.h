@@ -352,6 +352,33 @@ int b2f_explain_interventional(b2f_model *m, const void *rows, int64_t n, int ro
 /* device-resident form: enqueued on the compute stream (asynchronous, like b2f_explain_device; b2f_sync waits) */
 int b2f_explain_interventional_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev);
 
+/* ---- partial dependence (csrc/partial_dependence.cuh) ----
+ * One-way partial dependence and ICE curves (sklearn's partial_dependence(method="brute") `individual`): for row i and each
+ * point g of a probe, the model's output (b2f_predict_f64's proba1) for row i with row word `word` replaced by the point's
+ * word.  Works for every model, with or without an explainer.  grid_words are 24-word-row words (B2F_ROWS_WORDS24
+ * semantics, whatever the rows' format): a category code (-1 = unknown) or float32 bits (NaN = missing, imputed with the
+ * training median as in rows).  A probe reads grid_words[grid_offset .. grid_offset + count); probes may share points.
+ * out: n x P doubles, row-major, P = the sum of the probes' counts; a row's output is its probes' points, concatenated in
+ * probe order.  Each point equals, bit for bit, the tile kernel's score of the substituted row; rows are independent of
+ * the batch and results are bit-identical from run to run.  Errors: B2F_EINVAL for ranked rows, n < 0, a NULL out with
+ * n > 0, a bad probe (word outside the fields, count outside 1..B2F_PD_MAX_POINTS, more than B2F_PD_MAX_PROBES probes, a
+ * grid range past B2F_PD_MAX_PROBES * B2F_PD_MAX_POINTS words), a category code outside [-1, vocabulary) or a forest deeper
+ * than 32 levels; B2F_ERANGE for an infinite numeric grid word.  Pipelined over the model's streams like b2f_explain, in
+ * chunks of at most 64 MB of output each; device_ms as b2f_explain. */
+#define B2F_PD_MAX_POINTS 256
+#define B2F_PD_MAX_PROBES 23
+typedef struct b2f_pd_probe {
+    int32_t word;        /* row word of the probed field: 0 .. n_cat + n_num - 1 */
+    int32_t grid_offset; /* first point in grid_words */
+    int32_t count;       /* points: 1 .. B2F_PD_MAX_POINTS */
+} b2f_pd_probe;
+int b2f_partial_dependence(b2f_model *m, const void *rows, int64_t n, int row_format, const b2f_pd_probe *probes, int n_probes,
+                           const uint32_t *grid_words, double *out, float *device_ms);
+/* device-resident form: rows_dev and out_dev in device memory, probes and grid_words in host memory; enqueued on the
+ * compute stream (asynchronous, like b2f_explain_device; b2f_sync waits) */
+int b2f_partial_dependence_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const b2f_pd_probe *probes, int n_probes,
+                                  const uint32_t *grid_words, double *out_dev);
+
 /* asynchronous form for the request-batching ring: buffers must be pinned and stay valid until
  * b2f_wait(ticket) returns.  proba_is_f64 selects double (1) or float (0) outputs. */
 int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned,
