@@ -31,6 +31,8 @@ struct b2f_drift {
     int64_t new_cap = 0;
     double *d_rows = nullptr; /* row-scan scratch: [n_num][2][B2F_DRIFT_ROW_STRIDE(n_ref)] */
     int rowscan_max_n = 0, rowscan_smem_max_n = 0;
+    double *d_wide = nullptr; /* wide-band sweep scratch: [n_num][2][wide_ring], grown on demand */
+    int64_t wide_ring = 0;
     size_t finish_smem = 0;
     void *d_out = nullptr; /* p_val[F] | stat[F] | flags[F] */
     void *h_out = nullptr; /* pinned mirror */
@@ -50,6 +52,7 @@ extern "C" void b2f_drift_destroy(b2f_drift *d) {
     if (d->d_new_off) cudaFree(d->d_new_off);
     if (d->d_new_counts) cudaFree(d->d_new_counts);
     if (d->d_rows) cudaFree(d->d_rows);
+    if (d->d_wide) cudaFree(d->d_wide);
     if (d->d_out) cudaFree(d->d_out);
     if (d->h_out) cudaFreeHost(d->h_out);
     if (d->ev0) cudaEventDestroy(d->ev0);
@@ -70,10 +73,13 @@ static int drift_init(b2f_drift *d, const double *ref_sorted, const int32_t *cat
         d->cat_off[c + 1] = d->cat_off[c] + cat_sizes[c];
     }
     d->cat_total = d->cat_off[d->n_cat];
-    for (int f = 0; f < d->n_num; ++f)
+    for (int f = 0; f < d->n_num; ++f) {
+        if (ref_sorted[(int64_t)f * d->n_ref] != ref_sorted[(int64_t)f * d->n_ref]) /* the loop below sees a NaN only after row 0 */
+            return set_err(B2F_EINVAL, "drift: reference column %d holds NaN at row 0", f);
         for (int64_t j = 1; j < d->n_ref; ++j)
             if (!(ref_sorted[(int64_t)f * d->n_ref + j - 1] <= ref_sorted[(int64_t)f * d->n_ref + j]))
                 return set_err(B2F_EINVAL, "drift: reference column %d is not sorted ascending (or holds NaN) at row %lld", f, (long long)j);
+    }
     CUDA_TRY(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
     CUDA_TRY(cudaEventCreate(&d->ev0));
     CUDA_TRY(cudaEventCreate(&d->ev1));
@@ -241,6 +247,32 @@ extern "C" int b2f_drift_score(b2f_drift *d, int64_t n, const double *num_cols, 
         CUDA_TRY(cudaMalloc((void **)&d->d_codes, std::max<size_t>((size_t)cap * d->n_cat * sizeof(int32_t), 8)));
         d->cap_rows = cap;
     }
+    /* the widest sweep ring this batch size can need (h <= lcm: D <= 1); beyond B2F_DRIFT_RING_MAX slots the sweep keeps its two
+     * rings in a global scratch.  Where lcm >= 2^31 (flag 1) no sweep runs. */
+    int64_t wide_need = 0;
+    if (d->n_num > 0) {
+        int64_t g = d->n_ref;
+        for (int64_t b = n; b;) {
+            const int64_t t = g % b;
+            g = b;
+            b = t;
+        }
+        const int64_t mg = std::max(d->n_ref, n) / g, ng = std::min(d->n_ref, n) / g;
+        if ((double)(d->n_ref / g) < 2147483647.0 / (double)(n / g)) {
+            const int64_t width = (2 * mg * ng * g) / (ng + mg) + 2;
+            int64_t ring = 32;
+            while (ring < width + 3) ring <<= 1;
+            if (ring > B2F_DRIFT_RING_MAX) wide_need = ring;
+        }
+    }
+    if (wide_need > d->wide_ring) {
+        CUDA_TRY(cudaStreamSynchronize(d->stream));
+        if (d->d_wide) cudaFree(d->d_wide);
+        d->d_wide = nullptr;
+        d->wide_ring = 0;
+        CUDA_TRY(cudaMalloc((void **)&d->d_wide, (size_t)d->n_num * 2 * (size_t)wide_need * sizeof(double)));
+        d->wide_ring = wide_need;
+    }
     int64_t n_new = 0;
     if (new_offsets) {
         if (!new_counts && new_offsets[d->n_cat] > 0) return set_err(B2F_EINVAL, "drift: new_counts is NULL");
@@ -290,6 +322,8 @@ extern "C" int b2f_drift_score(b2f_drift *d, int64_t n, const double *num_cols, 
     p.rowscan_max_n = d->rowscan_max_n;
     p.rowscan_smem_max_n = (n >= 2 && n <= d->rowscan_smem_max_n) ? d->rowscan_smem_max_n : 0;
     p.rowscan_cap = B2F_DRIFT_ROWSCAN_CAP;
+    p.wide_scratch = d->d_wide;
+    p.wide_ring = d->wide_ring;
     const int64_t total = n * F;
     const unsigned blocks = (unsigned)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, (int64_t)d->sm_count * 8));
     k_drift_count<<<blocks, 256, 0, d->stream>>>(p);

@@ -59,6 +59,8 @@ struct DriftParams {
     int32_t rowscan_max_n;    /* batches of 2 .. this many rows take the row scan through the global scratch (0 = never) */
     int32_t rowscan_smem_max_n; /* batches of 2 .. this many rows take the shared-memory row scan when their band fits (0 = never) */
     int32_t rowscan_cap;      /* doubles of dynamic shared memory available to it */
+    double *wide_scratch;     /* [n_num][2][wide_ring]: the sweep's two ring buffers when the band is wider than B2F_DRIFT_RING_MAX */
+    int64_t wide_ring;        /* slots per buffer there: the widest ring this batch size can need (0: none allocated) */
 };
 
 /* ------------------------------------------------------------------ k_drift_count */
@@ -313,6 +315,57 @@ __device__ __forceinline__ double sweep_block(const SweepConst &c, int tid, int 
         cur = tmp;
     }
     return prev[(int)(c.n & mask)]; /* written before the last barrier */
+}
+
+/* ring > B2F_DRIFT_RING_MAX (large samples, D far from 0): the same sweep with its two ring buffers in a per-feature global
+ * scratch (L2; __syncthreads orders global memory inside the CTA) and no per-slot registers -- a thread owns ring / 1024 slots,
+ * so each slot's cell is recomputed every step from the diagonal's lowest covered j (the closed forms SlotState tracks
+ * incrementally: j = js + ((s - js) mod ring), i = t - j).  All threads of the CTA. */
+__device__ double sweep_wide(const SweepConst &c, int tid, int nt, double *buf0, double *buf1) {
+    const int64_t mask = c.ring - 1;
+    int64_t j_lo = -(c.h / c.den) - 1;
+    while (c.den * j_lo <= -c.h) ++j_lo;
+    int64_t edge = -c.h - c.den * j_lo;
+    int64_t js = j_lo - 1;
+    const SweepF f = sweep_f(c);
+    for (int s = tid; s < c.ring; s += nt) __stcg(buf0 + s, 1.0);
+    __syncthreads();
+    double *prev = buf0, *cur = buf1;
+    for (int64_t t = 0; t <= c.T; ++t) {
+        const double rt = t > 0 ? 1.0 / (double)t : 0.0;
+        for (int s0 = tid; s0 < c.ring; s0 += 4 * nt) { /* four slots' loads in flight before their stores */
+            double up[4], left[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const int s = s0 + k * nt;
+                up[k] = s < c.ring ? __ldcg(prev + s) : 0.0;
+                left[k] = s < c.ring ? __ldcg(prev + ((s - 1) & mask)) : 0.0;
+            }
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const int s = s0 + k * nt;
+                if (s < c.ring) {
+                    const int64_t j = js + ((s - js) & mask);
+                    SlotState st;
+                    st.j = (double)j;
+                    st.i = (double)(t - j);
+                    st.dev = (double)(c.ng * (t - j) - c.mg * j);
+                    st.v = up[k];
+                    __stcg(cur + s, slot_eval(st, left[k], rt, f));
+                }
+            }
+        }
+        edge += c.ng;
+        if (edge >= 0) {
+            edge -= c.den;
+            ++js;
+        }
+        __syncthreads();
+        double *tmp = prev;
+        prev = cur;
+        cur = tmp;
+    }
+    return __ldcg(prev + (c.n & mask));
 }
 
 /* ---- the row-scan form (request-sized batches) ---------------------------------------------------------------------
@@ -636,6 +689,19 @@ __device__ double rows_scan_smem(const SweepConst &c, double *ring, int cap_i, i
     return 0.0;
 }
 
+/* Where the row scans are exact.  Row j is held scaled by 2^-E_j (E_j: the exponent of its largest binomial, 2^E_j <= 2 C(hi_j + j, j)),
+ * so what a cell holds below 2^-1074 of that scale -- a seed C(lo - 1 + j, j) far left of the band, a scaled-down cell -- is lost:
+ * at most 8 * 2^-1074 * 2^E_j per cell and row, w + 2 cells a row (w = hi - lo + 1 <= 2h/ng + 1).  A loss at (i, j) reaches (m, n)
+ * along at most C(m - i + n - j, n - j) paths, and C(hi + j, j) C(m - lo + 1 + n - j, n - j) <= C(m + n + w, n) (Vandermonde), so
+ * relative to C(m + n, n) the error of p is at most  n (w + 2) 2^(4 - 1074) prod_k (m + w + k) / (m + k)
+ *                                                  <= n (w + 2) 2^(4 - 1074) ((m + w + 1) / (m + 1))^n.
+ * A row-scan p-value is kept when it exceeds that bound by 2^40 (relative error <= 1e-12); below (p = 3.4e-183 at n = 1024 against
+ * 30 000 rows, D = 0.45, where the row scan gives half of the true p) the sweep recomputes it. */
+__device__ inline bool rows_scan_trusted(double pv, int64_t m, int64_t n, int64_t w) {
+    const double lg = log2((double)n * (double)(w + 2)) + (4.0 - 1074.0 + 40.0) + (double)n * log2((double)(m + w + 1) / (double)(m + 1));
+    return pv >= exp2(lg);
+}
+
 extern __shared__ unsigned char drift_smem[];
 
 __global__ void __launch_bounds__(B2F_DRIFT_THREADS) k_drift_finish(DriftParams p) {
@@ -742,18 +808,20 @@ __global__ void __launch_bounds__(B2F_DRIFT_THREADS) k_drift_finish(DriftParams 
     else if ((double)(m0 / g) >= 2147483647.0 / (double)(n0 / g)) flag = 1; /* scipy: lcm too big -> asymptotic formula */
     /* widest anti-diagonal of the band: in-band j satisfy |ng*t - (ng+mg)*j| < h */
     const int64_t width = (2 * h) / (ng + mg) + 2;
-    int ring = 32;
-    while (ring < width + 3 && ring < B2F_DRIFT_RING_MAX) ring <<= 1;
-    const bool too_wide = width + 3 > ring; /* only when 2*en*D^2 > ~139: p < 1e-60, below float32 resolution */
+    int64_t ring_need = 32;
+    while (ring_need < width + 3) ring_need <<= 1;
+    /* wider than the shared-memory ring: D * mn/(m+n) > ~2045.  p is not necessarily negligible there (1.6e-264 at
+     * m = n = 30 000, D = 0.142; ~1e-7 at m = n = 10^6, D = 0.004): the sweep then runs through the global scratch */
+    const bool too_wide = ring_need > B2F_DRIFT_RING_MAX;
+    const int ring = (int)min(ring_need, (int64_t)B2F_DRIFT_RING_MAX);
     if (tid == 0) {
         p.stat[out] = dstat;
         p.flags[out] = flag;
         if (flag == 2) p.p_val[out] = nan("");
         else if (flag == 1) p.p_val[out] = -1.0; /* caller applies kstwo.sf(D, round(m*n/(m+n))) */
         else if (h == 0) p.p_val[out] = 1.0;
-        else if (too_wide) p.p_val[out] = 0.0;
     }
-    if (flag != 0 || h == 0 || too_wide) return;
+    if (flag != 0 || h == 0) return;
     if (n == 1) {
         /* single-row request (the common one): the m + 1 lattice paths -- one up-step after k right-steps, k = 0..m --
          * are equally likely, and a path stays strictly inside |i - m*j| < h iff m - h < k < h: no sweep needed */
@@ -773,22 +841,35 @@ __global__ void __launch_bounds__(B2F_DRIFT_THREADS) k_drift_finish(DriftParams 
     c.den = ng + mg;
     c.h = h;
     c.T = m + n;
-    c.ring = ring;
+    c.ring = too_wide ? (int)ring_need : ring;
     double res;
-    if (n >= 2 && n <= (int64_t)p.rowscan_smem_max_n && m == m0 && m >= 1024 && (2 * h) / ng + 2 <= (int64_t)p.rowscan_cap) {
-        /* request-sized batch, band narrow enough for the row to stay in shared memory: n in-place prefix sums */
-        res = rows_scan_smem(c, reinterpret_cast<double *>(drift_smem), p.rowscan_cap, tid, nt);
-        if (tid == 0) p.p_val[out] = fmin(fmax(res, 0.0), 1.0);
-        return;
+    const bool smem_rows = n >= 2 && n <= (int64_t)p.rowscan_smem_max_n && m == m0 && m >= 1024 && (2 * h) / ng + 2 <= (int64_t)p.rowscan_cap;
+    if (smem_rows || (p.row_scratch && n >= 2 && n <= (int64_t)p.rowscan_max_n && m == m0 && m >= 1024)) {
+        __shared__ int s_keep;
+        if (smem_rows) {
+            /* request-sized batch, band narrow enough for the row to stay in shared memory: n in-place prefix sums */
+            res = rows_scan_smem(c, reinterpret_cast<double *>(drift_smem), p.rowscan_cap, tid, nt);
+        } else {
+            /* request-sized batch against the big reference table: n prefix sums instead of m + n dependent steps */
+            double *rows2 = p.row_scratch + (int64_t)f * 2 * B2F_DRIFT_ROW_STRIDE(m0);
+            res = rows_scan(c, rows2, rows2 + B2F_DRIFT_ROW_STRIDE(m0), tid, nt);
+        }
+        if (tid == 0) {
+            res = fmin(fmax(res, 0.0), 1.0);
+            s_keep = rows_scan_trusted(res, m, n, (2 * h) / ng + 1);
+            if (s_keep) p.p_val[out] = res;
+        }
+        __syncthreads(); /* also: the ring's last read is done before a sweep reuses the shared memory */
+        if (s_keep) return;
     }
-    if (p.row_scratch && n >= 2 && n <= (int64_t)p.rowscan_max_n && m == m0 && m >= 1024) {
-        /* request-sized batch against the big reference table: n prefix sums instead of m + n dependent steps */
-        double *rows2 = p.row_scratch + (int64_t)f * 2 * B2F_DRIFT_ROW_STRIDE(m0);
-        res = rows_scan(c, rows2, rows2 + B2F_DRIFT_ROW_STRIDE(m0), tid, nt);
-        if (tid == 0) p.p_val[out] = fmin(fmax(res, 0.0), 1.0);
-        return;
-    }
-    if (ring == 32) {
+    if (too_wide) {
+        double *bufs = p.wide_scratch + (int64_t)f * 2 * p.wide_ring;
+        if (!p.wide_scratch || ring_need > p.wide_ring) { /* the host sizes the scratch for every band this batch size allows */
+            if (tid == 0) p.p_val[out] = nan("");
+            return;
+        }
+        res = sweep_wide(c, tid, nt, bufs, bufs + ring_need);
+    } else if (ring == 32) {
         if (tid >= 32) return;
         res = sweep_warp(c, tid);
     } else {

@@ -44,6 +44,11 @@ class TabularDrift:
         self.num_features = [c for c in self.features if c not in cat_set]
         self.n_ref = len(reference)
         self.ref_sorted = {name: np.sort(reference[name].to_numpy(dtype=np.float64)) for name in self.num_features}
+        for name, col in self.ref_sorted.items():  # np.sort puts NaN last
+            if len(col) and np.isnan(col[-1]):
+                # scipy's K-S (and so alibi-detect) would answer NaN for this feature on every request: refuse the reference instead
+                raise ValueError(f"drift reference column {name!r} holds {int(np.isnan(col).sum())} NaN value(s); "
+                                 "drop or impute them before building the detector")
         self.ref_cats, self.ref_counts = {}, {}
         for name in self.cat_features:
             cats, counts = np.unique(reference[name].astype(str).to_numpy(), return_counts=True)

@@ -47,8 +47,8 @@ def exact_p(m0: int, n0: int, num: int, force_ring: int | None = None, check_boo
         ring = force_ring
     if h == 0:
         return 1.0, 0
-    if width + 3 > ring:
-        return 0.0, 0
+    if width + 3 > ring:  # wider than the shared-memory ring: k_drift_finish runs sweep_wide
+        return exact_p_wide(m0, n0, num, ring_max=RING_MAX)
     if n == 1 and not force_ring:  # single-row request: closed form (m + 1 equally likely paths), as in the kernel
         lo, hi = max(m - h + 1, 0), min(h - 1, m)
         inside = hi - lo + 1 if hi >= lo else 0
@@ -251,3 +251,115 @@ def exact_p_rows_ring(m0: int, n0: int, num: int, cap: int = 26624, nt: int = 10
         hi_p, e_p = hi, e
     total = _binom_scaled(m + n, n, e_p)
     return float(min(max(ring[m % cap] / total, 0.0), 1.0)), 0
+
+
+# ----------------------------------------------------------------------------- which form k_drift_finish runs
+def kernel_limits(path: str | None = None) -> dict:
+    """The router's constants, parsed from ``csrc/drift_stats.cuh`` (so a change there reaches the mirror below)."""
+    import os
+    import re
+
+    if path is None:
+        path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "databricks_kubernetes_mlops_poc_b200", "csrc",
+                            "drift_stats.cuh")
+    src = open(path).read()
+    out = {}
+    for key in ("THREADS", "RING_MAX", "ROWSCAN_MAX", "ROWSCAN_SMEM_MAX", "ROWSCAN_SMEM_LIMIT", "ROWSCAN_CAP"):
+        out[key] = int(re.search(rf"#define\s+B2F_DRIFT_{key}\s+(\d+)", src).group(1))
+    return out
+
+
+def host_limits(env: dict | None = None, limits: dict | None = None) -> dict:
+    """What ``drift_init`` makes of the environment: the largest batch of each row-scan form (0 = off)."""
+    lim = limits or kernel_limits()
+    env = env or {}
+    rows = lim["ROWSCAN_MAX"]
+    if "B2F_DRIFT_ROWSCAN" in env:
+        rows = max(0, min(lim["ROWSCAN_MAX"], int(env["B2F_DRIFT_ROWSCAN"])))
+    smem = 0 if ("B2F_DRIFT_ROWSCAN" in env and rows == 0) else lim["ROWSCAN_SMEM_MAX"]
+    if "B2F_DRIFT_ROWSCAN_SMEM" in env:
+        smem = max(0, min(lim["ROWSCAN_SMEM_LIMIT"], int(env["B2F_DRIFT_ROWSCAN_SMEM"])))
+    return {"rows": rows, "smem": smem, "cap": lim["ROWSCAN_CAP"], "ring_max": lim["RING_MAX"], "threads": lim["THREADS"]}
+
+
+def rows_scan_trusted(p: float, m: int, n: int, w: int) -> bool:
+    """Mirror of ``rows_scan_trusted``: the row scans lose what a row holds below 2^-1074 of its scale; their p-value is kept
+    only where that loss is below 2^-40 of it."""
+    lg = math.log2(n * (w + 2)) + (4.0 - 1074.0 + 40.0) + n * math.log2((m + w + 1) / (m + 1))
+    return p >= 2.0 ** lg if lg > -1100 else True
+
+
+def route(n_ref: int, n0: int, num: int, env: dict | None = None, p: float | None = None, limits: dict | None = None) -> str:
+    """-> the form ``k_drift_finish`` takes for a numeric feature with K-S numerator ``num`` (D = num / (n_ref n0)):
+    'nan' / 'asymptotic' (flags 2 / 1), 'h0' (p = 1), 'n1' (closed form), 'rows_smem', 'rows_global', 'ring32',
+    'ns1' / 'ns2' / 'ns4' (sweep_block<NS>), 'wide' (sweep_wide, rings in global memory).  With ``p`` (the true p-value)
+    a row scan whose result would not be trusted reports the sweep form that recomputes it."""
+    hl = host_limits(env, limits)
+    g = math.gcd(n_ref, n0)
+    m, n = max(n_ref, n0), min(n_ref, n0)
+    mg, ng = m // g, n // g
+    h = num // g
+    if (n_ref // g) >= 2147483647.0 / (n0 // g):
+        return "asymptotic"
+    if h == 0:
+        return "h0"
+    if n == 1:
+        return "n1"
+    width = (2 * h) // (ng + mg) + 2
+    ring = 32
+    while ring < width + 3:
+        ring <<= 1
+    smem_max = hl["smem"] if 2 <= n0 <= hl["smem"] else 0
+    smem_rows = 2 <= n <= smem_max and m == n_ref and m >= 1024 and (2 * h) // ng + 2 <= hl["cap"]
+    global_rows = hl["rows"] > 0 and n_ref >= 1024 and 2 <= n <= hl["rows"] and m == n_ref and m >= 1024
+    if smem_rows or global_rows:
+        if p is None or rows_scan_trusted(p, m, n, (2 * h) // ng + 1):
+            return "rows_smem" if smem_rows else "rows_global"
+    if ring > hl["ring_max"]:
+        return "wide"
+    if ring == 32:
+        return "ring32"
+    return f"ns{ring // min(hl['threads'], ring)}"
+
+
+def exact_p_wide(m0: int, n0: int, num: int, ring_max: int = RING_MAX):
+    """`sweep_wide` step by step: a ring wider than ``ring_max`` in global memory, every slot's cell recomputed each diagonal
+    from the lowest covered j (j = js + ((s - js) mod ring), i = t - j) instead of tracked.  -> (p, flag), or None when the band
+    fits the shared-memory ring (the kernel takes another form)."""
+    g = math.gcd(m0, n0)
+    m, n = max(m0, n0), min(m0, n0)
+    mg, ng = m // g, n // g
+    h = num // g
+    if (m0 // g) >= 2147483647.0 / (n0 // g):
+        return -1.0, 1
+    if h == 0:
+        return 1.0, 0
+    den = ng + mg
+    width = (2 * h) // den + 2
+    ring = 32
+    while ring < width + 3:
+        ring <<= 1
+    if ring <= ring_max:
+        return None
+    mask = ring - 1
+    j_lo = -(h // den) - 1
+    while den * j_lo <= -h:
+        j_lo += 1
+    js, edge = j_lo - 1, -h - den * j_lo
+    s = np.arange(ring, dtype=np.int64)
+    prev = np.ones(ring)
+    for t in range(m + n + 1):
+        j = js + ((s - js) & mask)
+        i = t - j
+        dev = ng * i - mg * j
+        left = prev[(s - 1) & mask]
+        rt = 1.0 / t if t > 0 else 0.0
+        off = (j < 0) | (j > n) | (i < 0) | (i > m) | (np.abs(dev) >= h)
+        scale = np.where(off | (i == 0), 0.0, rt)
+        with np.errstate(invalid="ignore", over="ignore"):
+            prev = (left * j + prev * i) * scale + np.where(off, 1.0, 0.0)
+        edge += ng
+        if edge >= 0:
+            edge -= den
+            js += 1
+    return float(min(max(prev[n & mask], 0.0), 1.0)), 0

@@ -123,7 +123,7 @@ def test_drift_large_batches(curated):
         batch = ref.iloc[rng.integers(0, len(ref), 65536)].reset_index(drop=True)
         _check(det, ref, batch)
         assert det.last_device_ms > 0
-        # a band too wide for the shared-memory ring only occurs where the p-value underflows (here even float64)
+        # a band too wide for the shared-memory ring (D * mn/(m+n) > ~2045): the sweep keeps its rings in global memory
         from databricks_kubernetes_mlops_poc_b200.drift import TabularDrift
 
         one = TabularDrift(ref[[rp.NUMERIC_FEATURES[0]]], [], device=0)
@@ -133,7 +133,7 @@ def test_drift_large_batches(curated):
             r = stats.ks_2samp(col.iloc[:, 0].to_numpy(float), moved.iloc[:, 0].to_numpy(float), alternative="two-sided", method="exact")
             p1, s1, f1 = one.statistics(moved)
             assert f1[0] == 0 and abs(s1[0] - r.statistic) <= 4e-16 and r.statistic > 0.1
-            assert p1[0] == 0.0 and r.pvalue < 1e-300
+            assert abs(p1[0] - r.pvalue) <= RTOL * max(r.pvalue, 1e-300), (p1[0], r.pvalue)
         finally:
             one.close()
         odd = ref.iloc[rng.integers(0, len(ref), 99991)].reset_index(drop=True)  # 30000 * 99991 / gcd >= 2^31
@@ -204,7 +204,7 @@ def test_drift_against_frozen_library_outputs(curated, inference):
 def test_row_scan_and_sweep_agree(curated):
     """Request-sized batches take a row-scan form of the exact p-value -- the row resident in shared memory (2 .. 1024 rows, band
     narrower than the ring), else through the global scratch (2 .. 48 rows) -- larger ones the anti-diagonal sweep; the same
-    batches through all three forms give the same p-values (and all equal scipy's, above)."""
+    batches through all three forms give the same p-values, feature by feature, and each run equals scipy's."""
     import os
 
     from oracle import reference_pipeline as rp
@@ -225,7 +225,7 @@ def test_row_scan_and_sweep_agree(curated):
     det = TabularDrift(ref, rp.CATEGORICAL_FEATURES, device=0)  # shared-memory row scan up to 448 rows, sweep beyond
     try:
         a = [det.statistics(b) for b in batches]
-        for b in batches[:8] + batches[-2:]:
+        for b in batches:
             _check(det, ref, b)
     finally:
         det.close()
@@ -240,6 +240,7 @@ def test_row_scan_and_sweep_agree(curated):
             for b, (p, stat, flags) in zip(batches, a):
                 p2, stat2, flags2 = det.statistics(b)
                 assert (flags == flags2).all() and (stat == stat2).all()
-                assert np.abs(p - p2).max() <= 1e-11 * np.maximum(np.abs(p2), 1e-300).max(), (env, len(b))
+                assert (np.abs(p - p2) <= 1e-11 * np.maximum(np.abs(p), 1e-300)).all(), (env, len(b))  # feature by feature
+                _check(det, ref, b)
         finally:
             det.close()
