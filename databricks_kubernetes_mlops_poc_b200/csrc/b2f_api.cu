@@ -119,59 +119,50 @@ static int nccl_load(void) {
     } while (0)
 
 /* ------------------------------------------------------------------ model */
+/* A device buffer grown on demand and used by one stream at a time.  reserve: when need exceeds the capacity, wait for the
+ * stream st, which orders every use of the buffer, then free it and allocate alloc bytes; a failed allocation leaves it empty. */
+struct DevBuf {
+    void *p = nullptr;
+    size_t bytes = 0;
+    int reserve(cudaStream_t st, size_t need, size_t alloc) {
+        if (need <= bytes) return B2F_OK;
+        CUDA_TRY(cudaStreamSynchronize(st));
+        release();
+        const cudaError_t e = cudaMalloc(&p, alloc);
+        if (e != cudaSuccess) {
+            p = nullptr;
+            return set_err(B2F_ECUDA, "cudaMalloc(%zu bytes) failed: %s", alloc, cudaGetErrorString(e));
+        }
+        bytes = alloc;
+        return B2F_OK;
+    }
+    void release() {
+        if (p) cudaFree(p);
+        p = nullptr;
+        bytes = 0;
+    }
+};
+
+/* one stream of the host pipeline and a chunk's device buffers, whatever the job: chunks on a slot are ordered by its stream */
 struct Slot {
     cudaStream_t stream = nullptr;
-    void *d_rows = nullptr;
-    void *d_proba = nullptr; /* 24 B per row: double, {float, int32} pairs or b2f_scored_full records */
-    int32_t *d_label = nullptr;
-    int64_t cap_rows = 0;
+    DevBuf rows;    /* the chunk's rows, 96 B per row */
+    DevBuf out;     /* its output rows: scores, records, explanations or curves */
+    DevBuf label;   /* its labels */
+    DevBuf scratch; /* per-range partial sums of an explain chunk (launch_explain) */
 };
 
-/* device buffers of one stream's explain launches: phi (or interaction) rows and the per-range partial sums (tree_shap.cuh,
- * tree_shap_interactions.cuh); both kinds share them, grown to the larger request */
-struct ExplainBuf {
-    double *out = nullptr;
-    size_t out_bytes = 0;
-    double *scratch = nullptr;
-    size_t scratch_bytes = 0;
-};
-
-/* the launch shape of one explanation kernel (k_tree_shap, k_tree_shap_interactions or k_tree_shap_interventional) */
-struct ExplainKernel {
-    int smem_bytes = 0;
-    int ctas_per_sm = 1; /* resident CTAs per SM */
-};
-
-/* an attached background set (b2f_model_attach_background; tree_shap_interventional.cuh) */
-struct Background {
-    void *d_table = nullptr; /* offsets[n_paths + 1] int64, then the {mask, count} entries */
-    size_t bytes = 0;
-    int64_t rows = 0;        /* 0: none attached */
-    double base_value = 0.0; /* mean over the background rows of the prediction, in the output space */
-    VParams vp{};            /* vp.s: the explainer's SParams with denom * rows */
-};
-
-/* an attached path table (b2f_model_attach_explainer) */
-struct Explainer {
-    b2f_paths_header hdr;
-    void *d_table = nullptr;
-    IParams ip;   /* k_tree_shap takes ip.s; k_tree_shap_interactions also each warp's fields (inter_assign) */
-    int maxl = 9; /* length bucket of the kernels: 9, 16 or 24 */
-    ExplainKernel kernels[3]; /* [kind - B2F_OUT_EXPLAIN] */
-    Background bg;            /* k_tree_shap_interventional's table (b2f_model_attach_background) */
-    ExplainBuf slots[B2F_STREAMS];
-    ExplainBuf compute; /* b2f_explain_device */
-};
+struct Explainer; /* an attached path table (explain_api.cuh) */
+static void explainer_free(Explainer *ex);
 
 /* partial dependence (b2f_partial_dependence; partial_dependence.cuh).  The forest fields of pp are set at model creation;
  * segs, grid and points are the current call's. */
 struct Dependence {
     PdParams pp;
     int n_segs = 0;
-    std::vector<uint32_t> spec;    /* the call's PdSeg table, then its grid words */
-    ExplainBuf slots[B2F_STREAMS]; /* .out: the curves of a host call's chunk */
-    ExplainBuf host;               /* .scratch: a host call's spec on the device */
-    ExplainBuf compute;            /* .scratch: the device form's spec */
+    std::vector<uint32_t> spec; /* the call's PdSeg table, then its grid words */
+    DevBuf host_spec;           /* a host call's spec on the device */
+    DevBuf device_spec;         /* the device form's: a host call never overwrites a spec an enqueued device-form launch reads */
 };
 
 struct TicketRec {
@@ -222,20 +213,19 @@ struct b2f_model {
                                      same device whose kernels are launched on this handle's streams and rows */
     Slot slots[B2F_STREAMS];
     cudaStream_t compute = nullptr; /* device-resident interface + moments */
+    DevBuf scratch;                 /* per-range partial sums of the explain launches on compute */
     TicketRec tickets[B2F_TICKETS];
     uint64_t next_ticket = 1;
     uint64_t next_slot = 0;
     /* moments */
-    void *d_mom_rows = nullptr;
-    int64_t mom_cap_rows = 0;
+    DevBuf mom_rows;
     double *d_mom_partials = nullptr;
     int mom_blocks = 0;
     unsigned int *d_mom_ticket = nullptr;
     double *d_mom_out = nullptr;
-    double *d_gather = nullptr; /* nranks * 72 doubles */
-    int gather_cap = 0;
+    DevBuf gather; /* (nranks + 1) * 72 doubles */
     /* L2 flush scratch */
-    void *d_flush = nullptr;
+    DevBuf flush;
     /* nccl */
     ncclComm_t comm = nullptr;
     int nranks = 0;
@@ -850,35 +840,18 @@ extern "C" b2f_model *b2f_model_create(const void *forest_blob, size_t nbytes, i
     return m;
 }
 
-/* frees an explainer and its device buffers; nothing on the device may still use them */
-static void explainer_free(Explainer *ex) {
-    for (ExplainBuf *b = ex->slots; b <= &ex->compute; ++b) {
-        if (b->out) cudaFree(b->out);
-        if (b->scratch) cudaFree(b->scratch);
-    }
-    if (ex->d_table) cudaFree(ex->d_table);
-    if (ex->bg.d_table) cudaFree(ex->bg.d_table);
-    delete ex;
-}
-
 extern "C" void b2f_model_destroy(b2f_model *m) {
     if (!m) return;
     cudaSetDevice(m->device);
     cudaDeviceSynchronize();
     if (m->outlier) b2f_model_destroy(m->outlier);
     if (m->ex) explainer_free(m->ex);
-    for (ExplainBuf *b = m->pd.slots; b <= &m->pd.compute; ++b) {
-        if (b->out) cudaFree(b->out);
-        if (b->scratch) cudaFree(b->scratch);
-    }
     if (m->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(m->comm);
-    for (int s = 0; s < B2F_STREAMS; ++s) {
-        Slot &sl = m->slots[s];
-        if (sl.d_rows) cudaFree(sl.d_rows);
-        if (sl.d_proba) cudaFree(sl.d_proba);
-        if (sl.d_label) cudaFree(sl.d_label);
+    for (Slot &sl : m->slots) {
+        for (DevBuf *b : {&sl.rows, &sl.out, &sl.label, &sl.scratch}) b->release();
         if (sl.stream) cudaStreamDestroy(sl.stream);
     }
+    for (DevBuf *b : {&m->scratch, &m->pd.host_spec, &m->pd.device_spec, &m->mom_rows, &m->gather, &m->flush}) b->release();
     for (auto &t : m->tickets)
         for (auto &e : t.ev)
             if (e) cudaEventDestroy(e);
@@ -887,12 +860,9 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
     if (m->d_tile_layout) cudaFree(m->d_tile_layout);
     if (m->d_tile_pieces) cudaFree(m->d_tile_pieces);
     if (m->d_rank_layout) cudaFree(m->d_rank_layout);
-    if (m->d_mom_rows) cudaFree(m->d_mom_rows);
     if (m->d_mom_partials) cudaFree(m->d_mom_partials);
     if (m->d_mom_ticket) cudaFree(m->d_mom_ticket);
     if (m->d_mom_out) cudaFree(m->d_mom_out);
-    if (m->d_gather) cudaFree(m->d_gather);
-    if (m->d_flush) cudaFree(m->d_flush);
     delete m;
 }
 
@@ -1110,239 +1080,43 @@ static int out_launch(b2f_model *m, cudaStream_t st, const void *rows_dev, int64
     return launch_predict(m->outlier, st, rows_dev, n, fmt, false, rec + 16, reinterpret_cast<int32_t *>(rec + 12), B2F_OSTRIDE(6, 6));
 }
 
-/* ------------------------------------------------------------------ explanations (K5: tree_shap.cuh, forest_paths.h)
- * B2F_OUT_EXPLAIN is an output kind of the host pipeline only: b2f_explain passes it to enqueue_host_batch, so explanations
- * ride the same chunking, slots and streams as scores.  It is not a B2F_OUT_* value: out_row_bytes does not know it, so the
- * predict entry points refuse it.  B2F_OUT_INTERACTIONS is its sibling for b2f_explain_interactions (tree_shap_interactions.cuh):
- * F x F doubles per row.  B2F_OUT_INTERVENTIONAL is the third, for b2f_explain_interventional (tree_shap_interventional.cuh):
- * F doubles per row, against the attached background. */
-#define B2F_OUT_EXPLAIN 16
-#define B2F_OUT_INTERACTIONS 17
-#define B2F_OUT_INTERVENTIONAL 18
-/* B2F_OUT_DEPENDENCE: b2f_partial_dependence's curves, the call's total grid points in doubles per row (partial_dependence.cuh) */
-#define B2F_OUT_DEPENDENCE 19
-/* rows per chunk of an interactions batch (4 232 B of output per row for 23 fields), with no chunk plan: every chunk of
- * 16 384 rows is 512 row tiles, more than the SMs hold at once, so it runs as one range and needs no scratch */
-#define B2F_INTER_CHUNK_ROWS 16384
-/* device bytes of one chunk's partial-dependence curves: the chunk's rows are this over the row's bytes, 1 024 to 16 384 */
-#define B2F_PD_CHUNK_BYTES (64ll << 20)
-static int64_t pd_chunk_rows(const b2f_model *m) {
-    const int64_t rows = B2F_PD_CHUNK_BYTES / ((int64_t)m->pd.pp.points * (int64_t)sizeof(double));
-    return std::max<int64_t>(1024, std::min<int64_t>(B2F_CHUNK_ROWS, rows / 32 * 32));
-}
-/* the fixed rows per chunk of a host batch of this kind, or 0: the model's chunk size and chunk plan */
-static int64_t fixed_chunk_rows(const b2f_model *m, int kind) {
-    if (kind == B2F_OUT_DEPENDENCE) return pd_chunk_rows(m);
-    return kind == B2F_OUT_INTERACTIONS ? B2F_INTER_CHUNK_ROWS : 0;
+/* ------------------------------------------------------------------ host-buffer pipeline
+ * A host batch is a job: its entry point checks what the job needs and builds this record once per call.  The pipeline
+ * (enqueue_host_batch, submit_chunk, timed_host_batch) reads nothing else about what the batch computes. */
+struct HostJob {
+    size_t row_bytes;   /* bytes of one output row */
+    int64_t chunk_rows; /* rows per chunk; 0: the model's chunk size and chunk plan */
+    bool label;         /* writes the caller's label array */
+    int kind;           /* passed to launch: a B2F_OUT_* kind for scores, the TreeSHAP variant for explanations */
+    /* one chunk: n device rows of format fmt on stream st into out_dev (NULL: no output) and label_dev (NULL: no labels), with
+     * scratch for partial sums */
+    int (*launch)(b2f_model *m, int kind, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, void *out_dev, int32_t *label_dev,
+                  DevBuf &scratch);
+};
+
+/* the job of a score batch of output kind B2F_OUT_* (checked by out_check) */
+static HostJob score_job(int kind) {
+    return {out_row_bytes(kind), 0, kind == B2F_OUT_F32 || kind == B2F_OUT_F64, kind,
+            [](b2f_model *m, int kind, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, void *out_dev, int32_t *label_dev, DevBuf &) {
+                return out_launch(m, st, rows_dev, n, fmt, kind, out_dev, label_dev);
+            }};
 }
 
-static int explain_fields(const b2f_model *m) { return (int)(m->hdr.n_cat + m->hdr.n_num); }
-static bool explain_kind(int kind) { return kind >= B2F_OUT_EXPLAIN && kind <= B2F_OUT_INTERVENTIONAL; }
-static size_t explain_row_bytes(const b2f_model *m, int kind) {
-    const size_t F = (size_t)explain_fields(m);
-    return (kind == B2F_OUT_INTERACTIONS ? F * F : F) * sizeof(double);
+static int score_check(const b2f_model *m, int64_t n, int kind, int fmt, const void *out) {
+    if (n < 0) return set_err(B2F_EINVAL, "negative row count");
+    return out_check(m, kind, fmt, out || n == 0);
 }
 
-static int explain_check(const b2f_model *m, int fmt, int kind, bool have_out) {
-    if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
-    if (kind == B2F_OUT_INTERVENTIONAL && !m->ex->bg.rows) return set_err(B2F_ESTATE, "no background attached (b2f_model_attach_background)");
-    if (fmt == B2F_ROWS_RANKED)
-        return set_err(B2F_EINVAL, "explanations take float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
-    if (!have_out) return set_err(B2F_EINVAL, kind == B2F_OUT_INTERACTIONS ? "phi2 is NULL" : "phi is NULL");
-    return B2F_OK;
-}
-
-/* row tiles x path ranges of one launch: one range from a full grid of row tiles up; below, enough ranges to fill every SM
- * (at least sixteen paths per range: two per warp for k_tree_shap).  The partials of several ranges take ranges * n * values
- * doubles (values: fields, or F(F+1)/2 triangle slots for interactions); since ranges > 1 only when tiles < target, that is
- * below 2 * target * 32 rows' worth: bounded by the GPU, not by n or the number of paths. */
-static int64_t explain_ranges(const b2f_model *m, int64_t n, int kind) {
-    const int64_t tiles = (n + 31) / 32, target = (int64_t)m->sm_count * m->ex->kernels[kind - B2F_OUT_EXPLAIN].ctas_per_sm;
-    int64_t r = tiles >= target ? 1 : (target + tiles - 1) / tiles;
-    r = std::min<int64_t>(r, std::max<int64_t>(1, (int64_t)m->ex->hdr.n_paths / (2 * B2F_SHAP_WARPS)));
-    return std::max<int64_t>(1, std::min<int64_t>(r, 65535));
-}
-
-static int explain_reserve_scratch(ExplainBuf &b, cudaStream_t st, size_t bytes) {
-    if (bytes <= b.scratch_bytes) return B2F_OK;
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (b.scratch) cudaFree(b.scratch);
-    b.scratch = nullptr;
-    b.scratch_bytes = 0;
-    CUDA_TRY(cudaMalloc((void **)&b.scratch, bytes));
-    b.scratch_bytes = bytes;
-    return B2F_OK;
-}
-
-template <int MAXL>
-static const void *explain_kernel_l(int kind, bool pk) {
-    if (kind == B2F_OUT_INTERACTIONS)
-        return pk ? (const void *)k_tree_shap_interactions<MAXL, true> : (const void *)k_tree_shap_interactions<MAXL, false>;
-    if (kind == B2F_OUT_INTERVENTIONAL)
-        return pk ? (const void *)k_tree_shap_interventional<MAXL, true> : (const void *)k_tree_shap_interventional<MAXL, false>;
-    return pk ? (const void *)k_tree_shap<MAXL, true> : (const void *)k_tree_shap<MAXL, false>;
-}
-/* the kind's kernel for the path-length bucket maxl and the row format.  All take (params, rows, n, out, partials): IParams
- * for interactions, the background's VParams for interventional values, the SParams otherwise. */
-static const void *explain_kernel(int kind, int maxl, bool pk) {
-    return maxl <= 9 ? explain_kernel_l<9>(kind, pk) : (maxl <= 16 ? explain_kernel_l<16>(kind, pk) : explain_kernel_l<24>(kind, pk));
-}
-
-/* out_dev[n] rows of explain_row_bytes (phi, or the F x F interaction matrix) for n device rows of format fmt, on stream st,
- * partial sums (phi, or the triangle) in b's scratch */
-static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, int kind, double *out_dev, ExplainBuf &b) {
-    if (n <= 0) return B2F_OK;
-    Explainer &ex = *m->ex;
-    const bool inter = kind == B2F_OUT_INTERACTIONS, interv = kind == B2F_OUT_INTERVENTIONAL;
-    const char *name = inter ? "k_tree_shap_interactions" : (interv ? "k_tree_shap_interventional" : "k_tree_shap");
-    void *params = inter ? static_cast<void *>(&ex.ip) : (interv ? static_cast<void *>(&ex.bg.vp) : static_cast<void *>(&ex.ip.s));
-    const double denom = interv ? ex.bg.vp.s.denom : ex.hdr.denom; /* phi = sum / denom (interventional: / (denom * rows)) */
-    const int F = explain_fields(m), values = inter ? inter_slots(F) : F; /* partial sums per row */
-    if (ex.hdr.n_paths == 0) { /* every tree a single leaf: nothing moves away from base_value */
-        CUDA_TRY(cudaMemsetAsync(out_dev, 0, (size_t)n * explain_row_bytes(m, kind), st));
-        return B2F_OK;
-    }
-    const int64_t ranges = explain_ranges(m, n, kind);
-    if (ranges > 1) {
-        int rc = explain_reserve_scratch(b, st, (size_t)ranges * (size_t)n * values * sizeof(double));
-        if (rc) return rc;
-    }
-    const uint32_t *rows = static_cast<const uint32_t *>(rows_dev);
-    long long n_rows = n;
-    void *args[] = {params, &rows, &n_rows, &out_dev, &b.scratch};
-    /* a failed launch is also the thread's last error, taken (and cleared) below as after <<< >>> */
-    cudaLaunchKernel(explain_kernel(kind, ex.maxl, fmt == B2F_ROWS_PACKED64), dim3((unsigned)((n + 31) / 32), (unsigned)ranges),
-                     dim3(B2F_SHAP_THREADS), args, (size_t)ex.kernels[kind - B2F_OUT_EXPLAIN].smem_bytes, st);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_err(B2F_ECUDA, "%s launch failed: %s", name, cudaGetErrorString(e));
-    m->launches++;
-    if (ranges > 1) {
-        if (inter) { /* one CTA per row, its triangle in shared memory */
-            const unsigned blocks = (unsigned)std::min<int64_t>(n, (int64_t)m->sm_count * 8);
-            k_tree_shap_interactions_finish<<<blocks, 256, (size_t)values * sizeof(double), st>>>(b.scratch, (int)ranges, n_rows, F, denom,
-                                                                                                  out_dev);
-        } else {
-            const int64_t n_values = n * F;
-            const unsigned blocks = (unsigned)std::min<int64_t>((n_values + 255) / 256, (int64_t)m->sm_count * 8);
-            k_tree_shap_finish<<<blocks, 256, 0, st>>>(b.scratch, (int)ranges, (long long)n_values, denom, out_dev);
-        }
-        e = cudaGetLastError();
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "%s_finish launch failed: %s", name, cudaGetErrorString(e));
-        m->launches++;
-    }
-    return B2F_OK;
-}
-
-/* the output buffer of one slot's chunk: rows of row_bytes (at least 1024 rows' worth) */
-static int explain_reserve_out(ExplainBuf &b, cudaStream_t st, int64_t rows, size_t row_bytes) {
-    if ((size_t)rows * row_bytes <= b.out_bytes) return B2F_OK;
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (b.out) cudaFree(b.out);
-    b.out = nullptr;
-    b.out_bytes = 0;
-    const size_t cap = (size_t)std::max<int64_t>(rows, 1024) * row_bytes;
-    CUDA_TRY(cudaMalloc((void **)&b.out, cap));
-    b.out_bytes = cap;
-    return B2F_OK;
-}
-
-/* ------------------------------------------------------------------ partial dependence (K6: partial_dependence.cuh)
- * A call's probes and grid become one spec: a PdSeg per run of up to B2F_PD_SEG points of a probe, then every point's
- * word in output order (a row's output is its probes' points, concatenated), numerics imputed as the kernels impute rows.
- * The spec is checked and built on the host, uploaded once per call, and read by every chunk's launch. */
-static int pd_check(const b2f_model *m, int fmt, bool have_out) {
-    (void)m;
-    if (fmt == B2F_ROWS_RANKED)
-        return set_err(B2F_EINVAL, "partial dependence takes float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
-    if (!have_out) return set_err(B2F_EINVAL, "out is NULL");
-    return B2F_OK;
-}
-
-static int pd_prepare(b2f_model *m, const b2f_pd_probe *probes, int n_probes, const uint32_t *grid_words) {
-    const b2f_blob_header &h = m->hdr;
-    if (!probes || !grid_words) return set_err(B2F_EINVAL, "probes or grid_words is NULL");
-    if (n_probes < 1 || n_probes > B2F_PD_MAX_PROBES) return set_err(B2F_EINVAL, "n_probes = %d: expected 1..%d", n_probes, B2F_PD_MAX_PROBES);
-    if (h.max_depth > B2F_PD_STACK) return set_err(B2F_EINVAL, "partial dependence walks trees of depth <= %d; this forest has depth %u", B2F_PD_STACK, h.max_depth);
-    const int fields = (int)(h.n_cat + h.n_num);
-    std::vector<PdSeg> segs;
-    std::vector<uint32_t> words;
-    for (int i = 0; i < n_probes; ++i) {
-        const b2f_pd_probe pr = probes[i];
-        if (pr.word < 0 || pr.word >= fields) return set_err(B2F_EINVAL, "probe %d: row word %d outside the %d fields", i, pr.word, fields);
-        if (pr.count < 1 || pr.count > B2F_PD_MAX_POINTS) return set_err(B2F_EINVAL, "probe %d: %d grid points, expected 1..%d", i, pr.count, B2F_PD_MAX_POINTS);
-        if (pr.grid_offset < 0 || pr.grid_offset > B2F_PD_MAX_PROBES * B2F_PD_MAX_POINTS - pr.count)
-            return set_err(B2F_EINVAL, "probe %d: grid offset %d out of range", i, pr.grid_offset);
-        const bool cat = pr.word < (int)h.n_cat;
-        for (int k = 0; k < pr.count; ++k) {
-            uint32_t w = grid_words[pr.grid_offset + k];
-            if (cat) {
-                const int32_t code = (int32_t)w, vocab = h.vocab[pr.word];
-                if (code < -1 || (vocab > 0 && code >= vocab))
-                    return set_err(B2F_EINVAL, "probe %d point %d: category code %d outside [-1, %d)", i, k, code, vocab);
-            } else {
-                float f;
-                memcpy(&f, &w, sizeof(f));
-                if (std::isinf(f)) return set_err(B2F_ERANGE, "probe %d point %d: value is infinite or overflows float32", i, k);
-                if (std::isnan(f)) memcpy(&w, &h.impute[pr.word], sizeof(w));
-            }
-            if (k % B2F_PD_SEG == 0) segs.push_back(PdSeg{(uint32_t)pr.word, 0u, (uint32_t)words.size(), 0u});
-            segs.back().count++;
-            words.push_back(w);
-        }
-    }
-    Dependence &pd = m->pd;
-    pd.n_segs = (int)segs.size();
-    pd.pp.points = (int32_t)words.size();
-    pd.spec.assign(segs.size() * (sizeof(PdSeg) / sizeof(uint32_t)), 0u);
-    memcpy(pd.spec.data(), segs.data(), segs.size() * sizeof(PdSeg));
-    pd.spec.insert(pd.spec.end(), words.begin(), words.end());
-    return B2F_OK;
-}
-
-static size_t pd_row_bytes(const b2f_model *m) { return (size_t)m->pd.pp.points * sizeof(double); }
-
-/* out_dev[n][points] for n device rows of format fmt on stream st; spec_dev holds the call's spec */
-static int launch_dependence(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, double *out_dev, const void *spec_dev) {
-    if (n <= 0) return B2F_OK;
-    PdParams pp = m->pd.pp;
-    pp.segs = static_cast<const PdSeg *>(spec_dev);
-    pp.grid = reinterpret_cast<const uint32_t *>(pp.segs + m->pd.n_segs);
-    const dim3 grid((unsigned)((n + B2F_PD_WARPS * 32 - 1) / (B2F_PD_WARPS * 32)), (unsigned)m->pd.n_segs);
-    const uint32_t *rows = static_cast<const uint32_t *>(rows_dev);
-    if (fmt == B2F_ROWS_PACKED64)
-        k_partial_dependence<true><<<grid, B2F_PD_WARPS * 32, 0, st>>>(pp, rows, (long long)n, out_dev);
-    else
-        k_partial_dependence<false><<<grid, B2F_PD_WARPS * 32, 0, st>>>(pp, rows, (long long)n, out_dev);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_partial_dependence launch failed: %s", cudaGetErrorString(e));
-    m->launches++;
-    return B2F_OK;
-}
-
-/* ------------------------------------------------------------------ host-buffer pipeline */
-static int slot_reserve(b2f_model *m, Slot &sl, int64_t rows) {
-    if (rows <= sl.cap_rows) return B2F_OK;
-    CUDA_TRY(cudaStreamSynchronize(sl.stream));
-    if (sl.d_rows) cudaFree(sl.d_rows);
-    if (sl.d_proba) cudaFree(sl.d_proba);
-    if (sl.d_label) cudaFree(sl.d_label);
-    sl.d_rows = sl.d_proba = nullptr;
-    sl.d_label = nullptr;
-    sl.cap_rows = 0;
-    int64_t cap = std::max<int64_t>(rows, 1024);
-    CUDA_TRY(cudaMalloc(&sl.d_rows, (size_t)cap * B2F_ROW_BYTES));
-    CUDA_TRY(cudaMalloc(&sl.d_proba, (size_t)cap * sizeof(b2f_scored_full)));
-    CUDA_TRY(cudaMalloc((void **)&sl.d_label, (size_t)cap * sizeof(int32_t)));
-    sl.cap_rows = cap;
-    return B2F_OK;
-}
-
-/* One chunk on one slot: rows [lo, lo + cnt) of the caller's host rows -> H2D -> the output kind's launches -> D2H into the
- * caller's host output(s) at row lo.  marks (B2F_TIMELINE, may be NULL) gets an event before the first chunk's H2D, then one
- * after each of its H2D, launches and D2H. */
-static int submit_chunk(b2f_model *m, Slot &sl, const void *rows, int fmt, int kind, void *out, int32_t *label, int64_t lo, int64_t cnt,
+/* One chunk on one slot: rows [lo, lo + cnt) of the caller's host rows -> H2D -> the job's launch -> D2H into the caller's
+ * host output(s) at row lo.  marks (B2F_TIMELINE, may be NULL) gets an event before the first chunk's H2D, then one after
+ * each of its H2D, launches and D2H. */
+static int submit_chunk(b2f_model *m, Slot &sl, const HostJob &job, const void *rows, int fmt, void *out, int32_t *label, int64_t lo, int64_t cnt,
                         std::vector<cudaEvent_t> *marks) {
-    int rc = slot_reserve(m, sl, cnt);
+    if (!job.label) label = nullptr;
+    const size_t row_bytes = row_bytes_of(m, fmt), cap = (size_t)std::max<int64_t>(cnt, 1024); /* rows each buffer holds */
+    int rc = sl.rows.reserve(sl.stream, (size_t)cnt * B2F_ROW_BYTES, cap * B2F_ROW_BYTES);
+    if (rc == B2F_OK && out) rc = sl.out.reserve(sl.stream, (size_t)cnt * job.row_bytes, cap * job.row_bytes);
+    if (rc == B2F_OK && label) rc = sl.label.reserve(sl.stream, (size_t)cnt * sizeof(int32_t), cap * sizeof(int32_t));
     if (rc) return rc;
     auto mark = [&] {
         if (!marks) return;
@@ -1352,51 +1126,39 @@ static int submit_chunk(b2f_model *m, Slot &sl, const void *rows, int fmt, int k
         marks->push_back(e);
     };
     if (marks && marks->empty()) mark();
-    const bool explain = explain_kind(kind), dep = kind == B2F_OUT_DEPENDENCE;
-    ExplainBuf *eb = explain ? &m->ex->slots[&sl - m->slots] : (dep ? &m->pd.slots[&sl - m->slots] : nullptr);
-    const size_t row_bytes = row_bytes_of(m, fmt), out_bytes = explain ? explain_row_bytes(m, kind) : (dep ? pd_row_bytes(m) : out_row_bytes(kind));
-    if (eb && (rc = explain_reserve_out(*eb, sl.stream, cnt, out_bytes))) return rc;
-    void *d_out = eb ? static_cast<void *>(eb->out) : sl.d_proba;
-    const bool records = kind == B2F_OUT_PAIRS || kind == B2F_OUT_FULL;
-    CUDA_TRY(cudaMemcpyAsync(sl.d_rows, static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, (size_t)cnt * row_bytes, cudaMemcpyHostToDevice,
+    CUDA_TRY(cudaMemcpyAsync(sl.rows.p, static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, (size_t)cnt * row_bytes, cudaMemcpyHostToDevice,
                              sl.stream));
     mark();
-    rc = explain ? launch_explain(m, sl.stream, sl.d_rows, cnt, fmt, kind, eb->out, *eb)
-         : dep   ? launch_dependence(m, sl.stream, sl.d_rows, cnt, fmt, eb->out, m->pd.host.scratch)
-                 : out_launch(m, sl.stream, sl.d_rows, cnt, fmt, kind, out ? sl.d_proba : nullptr, label ? sl.d_label : nullptr);
+    rc = job.launch(m, job.kind, sl.stream, sl.rows.p, cnt, fmt, out ? sl.out.p : nullptr, label ? static_cast<int32_t *>(sl.label.p) : nullptr,
+                    sl.scratch);
     if (rc) return rc;
     mark();
     if (out)
-        CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(out) + (size_t)lo * out_bytes, d_out, (size_t)cnt * out_bytes, cudaMemcpyDeviceToHost,
-                                 sl.stream));
-    if (label && !records) CUDA_TRY(cudaMemcpyAsync(label + lo, sl.d_label, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, sl.stream));
+        CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(out) + (size_t)lo * job.row_bytes, sl.out.p, (size_t)cnt * job.row_bytes,
+                                 cudaMemcpyDeviceToHost, sl.stream));
+    if (label) CUDA_TRY(cudaMemcpyAsync(label + lo, sl.label.p, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, sl.stream));
     mark();
     return B2F_OK;
 }
 
-/* enqueue the whole batch; on return used_mask tells which slot streams carry work.
+/* enqueue the whole batch of n >= 0 rows; on return used_mask tells which slot streams carry work.
  * B2F_TIMELINE=1 (debug): record an event after every operation and print the schedule to stderr. */
-static int enqueue_host_batch(b2f_model *m, const void *rows, int64_t n, int fmt, void *out, int kind, int32_t *label, uint32_t *used_mask) {
+static int enqueue_host_batch(b2f_model *m, const HostJob &job, const void *rows, int64_t n, int fmt, void *out, int32_t *label,
+                              uint32_t *used_mask) {
     *used_mask = 0;
-    if (n < 0) return set_err(B2F_EINVAL, "negative row count");
-    int rc = explain_kind(kind)            ? explain_check(m, fmt, kind, out || n == 0)
-             : kind == B2F_OUT_DEPENDENCE ? pd_check(m, fmt, out || n == 0)
-                                          : out_check(m, kind, fmt, out || n == 0);
-    if (rc) return rc;
     if (n == 0) return B2F_OK;
     if (!rows) return set_err(B2F_EINVAL, "rows is NULL");
-    rc = check_row_format(m, fmt);
+    int rc = check_row_format(m, fmt);
     if (rc) return rc;
     CUDA_TRY(cudaSetDevice(m->device));
-    const int64_t fixed_chunk = fixed_chunk_rows(m, kind);
-    int64_t chunk = fixed_chunk ? fixed_chunk : m->chunk_rows;
+    int64_t chunk = job.chunk_rows ? job.chunk_rows : m->chunk_rows;
     if (n <= chunk + chunk / 2) chunk = n; /* small batch: one H2D, one launch */
     static const bool timeline = getenv("B2F_TIMELINE") != nullptr;
     std::vector<cudaEvent_t> tev;
     /* chunk schedule: equal chunks by default; a plan (B2F_CHUNK_PLAN="a,b,c": fractions of the batch in
      * 1/1024ths, the last chunk takes the remainder) front-loads the copies so the un-overlapped tail --
      * the last chunk's kernel and D2H -- is short */
-    const bool planned = !fixed_chunk && !m->chunk_plan.empty() && chunk != n && n >= 2 * m->chunk_rows;
+    const bool planned = !job.chunk_rows && !m->chunk_plan.empty() && chunk != n && n >= 2 * m->chunk_rows;
     int c = 0;
     for (int64_t off = 0; off < n; ++c) {
         int64_t cnt = std::min(chunk, n - off);
@@ -1407,7 +1169,7 @@ static int enqueue_host_batch(b2f_model *m, const void *rows, int64_t n, int fmt
         /* slots rotate ACROSS calls too, so with several batches in flight (async ring, stream dealer) the next
          * batch's H2D does not wait for the previous batch's kernel to release the same staging buffer */
         const int slot_idx = (int)((m->next_slot + (uint64_t)c) % B2F_STREAMS);
-        rc = submit_chunk(m, m->slots[slot_idx], rows, fmt, kind, out, label, off, cnt, timeline ? &tev : nullptr);
+        rc = submit_chunk(m, m->slots[slot_idx], job, rows, fmt, out, label, off, cnt, timeline ? &tev : nullptr);
         if (rc) return rc;
         *used_mask |= 1u << slot_idx;
         off += cnt;
@@ -1436,7 +1198,8 @@ static int sync_mask(b2f_model *m, uint32_t mask) {
 static int predict_host(b2f_model *m, const void *rows, int64_t n, int fmt, void *out, int kind, int32_t *label) {
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
     uint32_t mask = 0;
-    int rc = enqueue_host_batch(m, rows, n, fmt, out, kind, label, &mask);
+    int rc = score_check(m, n, kind, fmt, out);
+    if (rc == B2F_OK) rc = enqueue_host_batch(m, score_job(kind), rows, n, fmt, out, label, &mask);
     int rc2 = sync_mask(m, mask);
     return rc ? rc : rc2;
 }
@@ -1478,192 +1241,35 @@ extern "C" int b2f_predict_full(b2f_model *m, const void *rows, int64_t n, int r
     return predict_host(m, rows, n, row_format, out, B2F_OUT_FULL, nullptr);
 }
 
-/* ------------------------------------------------------------------ explainer: path table check, attach, explain */
-static int validate_paths(const uint8_t *t, size_t nbytes, b2f_paths_header *hdr_out) {
-    if (!t || nbytes < sizeof(b2f_paths_header)) return set_err(B2F_EINVAL, "path table too small (%zu bytes)", nbytes);
-    b2f_paths_header h;
-    memcpy(&h, t, sizeof(h));
-    if (memcmp(h.magic, B2F_PATHS_MAGIC, 8) != 0) return set_err(B2F_EINVAL, "path table: bad magic");
-    if (h.version != B2F_PATHS_VERSION) return set_err(B2F_EINVAL, "path table: version %u, expected %u", h.version, B2F_PATHS_VERSION);
-    if (h.header_bytes != B2F_PATHS_HEADER_BYTES) return set_err(B2F_EINVAL, "path table: header_bytes=%u unsupported", h.header_bytes);
-    if (h.agg_mode != B2F_AGG_RF_MEAN && h.agg_mode != B2F_AGG_GBDT_LOGISTIC)
-        return set_err(B2F_EINVAL, "path table: agg_mode %u (only RandomForest and GBDT classifiers are explained)", h.agg_mode);
-    if (h.n_cat + h.n_num > B2F_SENTINEL_WORD || h.n_cat + h.n_num == 0)
-        return set_err(B2F_EINVAL, "path table: n_cat+n_num=%u out of range [1,%u]", h.n_cat + h.n_num, B2F_SENTINEL_WORD);
-    if (h.n_trees == 0 || h.n_trees > B2F_MAX_TREES) return set_err(B2F_EINVAL, "path table: n_trees=%u out of range", h.n_trees);
-    if (h.max_len > B2F_PATHS_MAX_LEN) return set_err(B2F_EINVAL, "path table: max_len=%u exceeds %u", h.max_len, B2F_PATHS_MAX_LEN);
-    if (!(h.denom > 0.0) || !std::isfinite(h.base_value)) return set_err(B2F_EINVAL, "path table: bad denom or base_value");
-    const uint64_t elems_off = (h.paths_off + (uint64_t)h.n_paths * sizeof(b2f_path) + 15) / 16 * 16;
-    if (h.paths_off != B2F_PATHS_HEADER_BYTES || h.elems_off != elems_off || h.total_bytes != nbytes ||
-        h.elems_off + (uint64_t)h.n_elems * sizeof(b2f_path_elem) != nbytes)
-        return set_err(B2F_EINVAL, "path table: sections do not match its size (%zu bytes; truncated?)", nbytes);
-    const b2f_path *P = reinterpret_cast<const b2f_path *>(t + h.paths_off);
-    const b2f_path_elem *E = reinterpret_cast<const b2f_path_elem *>(t + h.elems_off);
-    const uint32_t F = h.n_cat + h.n_num;
-    uint64_t next = 0;
-    uint32_t longest = 0;
-    for (uint32_t p = 0; p < h.n_paths; ++p) {
-        b2f_path pr;
-        memcpy(&pr, &P[p], sizeof(pr));
-        if (pr.first != next || pr.len < 2 || pr.len > h.max_len || (uint64_t)pr.first + pr.len > h.n_elems || pr.tree >= h.n_trees ||
-            !std::isfinite(pr.leaf))
-            return set_err(B2F_EINVAL, "path table: path %u malformed (first %u, len %u)", p, pr.first, pr.len);
-        next += pr.len;
-        longest = std::max(longest, pr.len);
-        uint32_t seen = 0;
-        for (uint32_t k = 0; k < pr.len; ++k) {
-            b2f_path_elem e;
-            memcpy(&e, &E[pr.first + k], sizeof(e));
-            if (k == 0) {
-                if (e.field != B2F_PATH_BIAS_FIELD || e.kind != B2F_PE_BIAS) return set_err(B2F_EINVAL, "path table: path %u has no bias element", p);
-                continue;
-            }
-            const bool cat = e.kind == B2F_PE_CAT, num = (e.kind & ~B2F_PE_HAS_HI) == B2F_PE_NUM;
-            if (e.field >= F || (cat && e.field >= h.n_cat) || (num && e.field < h.n_cat) || !(cat || num))
-                return set_err(B2F_EINVAL, "path table: path %u element %u: field %u / kind %u invalid", p, k, e.field, e.kind);
-            if (seen & (1u << e.field)) return set_err(B2F_EINVAL, "path table: path %u tests field %u twice (elements must be merged)", p, e.field);
-            seen |= 1u << e.field;
-            if (!(e.zero_fraction > 0.0 && e.zero_fraction <= 1.0) || !(e.inv_zero_fraction >= 1.0) || !std::isfinite(e.inv_zero_fraction))
-                return set_err(B2F_EINVAL, "path table: path %u element %u: bad zero fraction", p, k);
-        }
+/* CUDA events, destroyed on every return path */
+struct Events {
+    std::vector<cudaEvent_t> e;
+    int create(size_t n) {
+        e.assign(n, nullptr);
+        for (cudaEvent_t &x : e) CUDA_TRY(cudaEventCreate(&x));
+        return B2F_OK;
     }
-    if (next != h.n_elems || longest != h.max_len) return set_err(B2F_EINVAL, "path table: element count or max_len inconsistent");
-    *hdr_out = h;
-    return B2F_OK;
-}
-
-extern "C" int b2f_paths_validate(const void *paths, size_t nbytes) {
-    b2f_paths_header h;
-    return validate_paths(static_cast<const uint8_t *>(paths), nbytes, &h);
-}
-
-/* flatten.py blob_fingerprint: sum of splitmix64(w_i ^ i * golden) over the blob's 64-bit words */
-static uint64_t blob_fingerprint(const uint8_t *blob, size_t nbytes) {
-    uint64_t sum = 0;
-    for (size_t i = 0; i < nbytes / 8; ++i) {
-        uint64_t z;
-        memcpy(&z, blob + 8 * i, 8);
-        z ^= (uint64_t)i * 0x9E3779B97F4A7C15ull;
-        z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-        z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-        sum += z ^ (z >> 31);
+    ~Events() {
+        for (cudaEvent_t x : e)
+            if (x) cudaEventDestroy(x);
     }
-    return sum;
-}
+};
 
-/* the fields each warp of k_tree_shap_interactions owns, balancing the counted pair work: per path of d elements that holds
- * field f, its owner unwinds f (d steps) and takes the unwound sum of every element of a higher field (d - 1 steps each).
- * Longest work first, each field to the warp with the least work so far (ties: the lower field, the lower warp). */
-static void inter_assign(const uint8_t *t, const b2f_paths_header &h, uint32_t own[B2F_SHAP_WARPS]) {
-    const int F = (int)(h.n_cat + h.n_num);
-    const b2f_path *P = reinterpret_cast<const b2f_path *>(t + h.paths_off);
-    const b2f_path_elem *E = reinterpret_cast<const b2f_path_elem *>(t + h.elems_off);
-    std::vector<double> work(F, 0.0);
-    for (uint32_t p = 0; p < h.n_paths; ++p) {
-        b2f_path pr;
-        memcpy(&pr, &P[p], sizeof(pr));
-        uint32_t fields[B2F_PATHS_MAX_LEN];
-        for (uint32_t k = 1; k < pr.len; ++k) memcpy(&fields[k], &E[pr.first + k].field, sizeof(uint32_t));
-        const double d = pr.len - 1.0;
-        for (uint32_t k = 1; k < pr.len; ++k) {
-            int higher = 0;
-            for (uint32_t j = 1; j < pr.len; ++j) higher += fields[j] > fields[k];
-            work[fields[k]] += d + higher * (d - 1.0);
-        }
-    }
-    std::vector<int> order(F);
-    for (int f = 0; f < F; ++f) order[f] = f;
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return work[a] > work[b]; });
-    double load[B2F_SHAP_WARPS] = {};
-    for (int w = 0; w < B2F_SHAP_WARPS; ++w) own[w] = 0;
-    for (int f : order) {
-        const int w = (int)(std::min_element(load, load + B2F_SHAP_WARPS) - load);
-        own[w] |= 1u << f;
-        load[w] += work[f];
-    }
-}
-
-extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_t nbytes) {
-    if (!m) return set_err(B2F_EINVAL, "model is NULL");
-    b2f_paths_header h;
-    int rc = validate_paths(static_cast<const uint8_t *>(paths), nbytes, &h);
-    if (rc) return rc;
-    if (h.n_cat != m->hdr.n_cat || h.n_num != m->hdr.n_num || h.agg_mode != m->hdr.agg_mode || h.n_trees != m->hdr.n_trees)
-        return set_err(B2F_EINVAL, "path table: shape (%u cat, %u num, agg %u, %u trees) differs from the model's (%u, %u, %u, %u)", h.n_cat, h.n_num,
-                       h.agg_mode, h.n_trees, m->hdr.n_cat, m->hdr.n_num, m->hdr.agg_mode, m->hdr.n_trees);
-    CUDA_TRY(cudaSetDevice(m->device));
-    std::vector<uint8_t> blob(m->hdr.total_bytes);
-    CUDA_TRY(cudaMemcpy(blob.data(), m->d_blob, blob.size(), cudaMemcpyDeviceToHost));
-    if (blob_fingerprint(blob.data(), blob.size()) != h.fingerprint)
-        return set_err(B2F_EINVAL, "path table: built from another forest (fingerprint mismatch)");
-    /* replacing an explainer: nothing may still read the old table.  Waited for before anything new is allocated, so a
-     * failure here leaves the model as it was and leaks nothing. */
-    if (m->ex) CUDA_TRY(cudaDeviceSynchronize());
-    Explainer *ex = new (std::nothrow) Explainer();
-    if (!ex) return set_err(B2F_ENOMEM, "out of host memory");
-    auto fail = [&](int code) {
-        explainer_free(ex);
-        return code;
-    };
-    ex->hdr = h;
-    if (cudaMalloc(&ex->d_table, nbytes) != cudaSuccess || cudaMemcpy(ex->d_table, paths, nbytes, cudaMemcpyHostToDevice) != cudaSuccess)
-        return fail(set_err(B2F_ENOMEM, "path table upload (%zu bytes) failed: %s", nbytes, cudaGetErrorString(cudaGetLastError())));
-    SParams &sp = ex->ip.s;
-    memset(&sp, 0, sizeof(sp));
-    sp.paths = reinterpret_cast<const b2f_path *>(static_cast<uint8_t *>(ex->d_table) + h.paths_off);
-    sp.elems = reinterpret_cast<const b2f_path_elem *>(static_cast<uint8_t *>(ex->d_table) + h.elems_off);
-    sp.n_paths = (int)h.n_paths;
-    sp.n_cat = (int)h.n_cat;
-    sp.n_num = (int)h.n_num;
-    sp.denom = h.denom;
-    memcpy(sp.impute, m->hdr.impute, sizeof(sp.impute));
-    ex->maxl = h.max_len <= 9 ? 9 : (h.max_len <= 16 ? 16 : 24);
-    inter_assign(static_cast<const uint8_t *>(paths), h, ex->ip.own);
-    /* the EXTEND / UNWIND factors (no division in the kernel) */
-    double tab[4][B2F_SHAP_TAB_L][B2F_SHAP_TAB_L]; /* per call: concurrent attaches (other handles) share nothing on the host */
-    for (int l = 0; l < B2F_SHAP_TAB_L; ++l)
-        for (int i = 0; i < B2F_SHAP_TAB_L; ++i) {
-            tab[0][l][i] = (i + 1.0) / (l + 1.0);
-            tab[1][l][i] = (l - i) / (l + 1.0);
-            tab[2][l][i] = (l + 1.0) / (i + 1.0);
-            tab[3][l][i] = l > i ? (l + 1.0) / (l - i) : 0.0;
-        }
-    cudaError_t e = cudaMemcpyToSymbol(c_shap_tab, tab, sizeof(tab));
-    for (int kind : {B2F_OUT_EXPLAIN, B2F_OUT_INTERACTIONS, B2F_OUT_INTERVENTIONAL}) {
-        ExplainKernel &k = ex->kernels[kind - B2F_OUT_EXPLAIN];
-        const int F = sp.n_cat + sp.n_num;
-        k.smem_bytes = kind == B2F_OUT_INTERACTIONS ? inter_smem_bytes(F) : (kind == B2F_OUT_INTERVENTIONAL ? interv_smem_bytes(F) : shap_smem_bytes(F));
-        for (bool pk : {false, true})
-            if (e == cudaSuccess) e = cudaFuncSetAttribute(explain_kernel(kind, ex->maxl, pk), cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem_bytes);
-        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k.ctas_per_sm, explain_kernel(kind, ex->maxl, false), B2F_SHAP_THREADS, k.smem_bytes);
-        k.ctas_per_sm = std::max(1, k.ctas_per_sm);
-    }
-    if (e != cudaSuccess) return fail(set_err(B2F_ECUDA, "explainer set-up failed: %s", cudaGetErrorString(e)));
-    if (m->ex) explainer_free(m->ex); /* the device was synchronised above */
-    m->ex = ex;
-    return B2F_OK;
-}
-
-/* a synchronous host batch of an explanation or partial-dependence kind; device_ms (may be NULL): from the first H2D to the
- * end of the last chunk */
-static int timed_host_batch(b2f_model *m, const void *rows, int64_t n, int row_format, double *out, int kind, float *device_ms) {
+/* a synchronous host batch of n >= 0 rows of a checked job; device_ms (may be NULL): from the first H2D to the end of the last
+ * chunk */
+static int timed_host_batch(b2f_model *m, const HostJob &job, const void *rows, int64_t n, int row_format, double *out, float *device_ms) {
     if (device_ms) *device_ms = 0.0f;
     CUDA_TRY(cudaSetDevice(m->device));
-    struct Events { /* destroyed on every return path */
-        cudaEvent_t e[1 + B2F_STREAMS] = {};
-        ~Events() {
-            for (cudaEvent_t x : e)
-                if (x) cudaEventDestroy(x);
-        }
-    } evs;
-    cudaEvent_t *ev = evs.e;
+    Events evs;
     const int first = (int)(m->next_slot % B2F_STREAMS);
     if (device_ms && n > 0) {
-        for (int i = 0; i <= B2F_STREAMS; ++i) CUDA_TRY(cudaEventCreate(&ev[i]));
-        CUDA_TRY(cudaEventRecord(ev[0], m->slots[first].stream));
+        int rc = evs.create(1 + B2F_STREAMS);
+        if (rc) return rc;
+        CUDA_TRY(cudaEventRecord(evs.e[0], m->slots[first].stream));
     }
+    cudaEvent_t *ev = evs.e.data();
     uint32_t mask = 0;
-    int rc = enqueue_host_batch(m, rows, n, row_format, out, kind, nullptr, &mask);
+    int rc = enqueue_host_batch(m, job, rows, n, row_format, out, nullptr, &mask);
     if (device_ms && n > 0 && rc == B2F_OK)
         for (int s = 0; s < B2F_STREAMS && rc == B2F_OK; ++s)
             if ((mask & (1u << s)) && cudaEventRecord(ev[1 + s], m->slots[s].stream) != cudaSuccess)
@@ -1678,159 +1284,6 @@ static int timed_host_batch(b2f_model *m, const void *rows, int64_t n, int row_f
                 *device_ms = std::max(*device_ms, ms);
             }
     return rc;
-}
-
-/* b2f_explain / b2f_explain_interactions / b2f_explain_interventional: kind B2F_OUT_EXPLAIN, B2F_OUT_INTERACTIONS or
- * B2F_OUT_INTERVENTIONAL */
-static int explain_host(b2f_model *m, const void *rows, int64_t n, int row_format, double *out, int kind, double *base_value, float *device_ms) {
-    if (!m) return set_err(B2F_EINVAL, "model is NULL");
-    if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
-    if (base_value) *base_value = kind == B2F_OUT_INTERVENTIONAL ? m->ex->bg.base_value : m->ex->hdr.base_value;
-    return timed_host_batch(m, rows, n, row_format, out, kind, device_ms);
-}
-
-extern "C" int b2f_explain(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi, double *base_value, float *device_ms) {
-    return explain_host(m, rows, n, row_format, phi, B2F_OUT_EXPLAIN, base_value, device_ms);
-}
-extern "C" int b2f_explain_interactions(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi2, double *base_value,
-                                        float *device_ms) {
-    return explain_host(m, rows, n, row_format, phi2, B2F_OUT_INTERACTIONS, base_value, device_ms);
-}
-
-/* b2f_explain_device / b2f_explain_interactions_device / b2f_explain_interventional_device */
-static int explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *out_dev, int kind) {
-    if (!m) return set_err(B2F_EINVAL, "model is NULL");
-    if (n < 0) return set_err(B2F_EINVAL, "negative row count");
-    int rc = explain_check(m, row_format, kind, out_dev != nullptr || n == 0);
-    if (rc == B2F_OK) rc = check_row_format(m, row_format);
-    if (rc) return rc;
-    CUDA_TRY(cudaSetDevice(m->device));
-    return launch_explain(m, m->compute, rows_dev, n, row_format, kind, out_dev, m->ex->compute);
-}
-extern "C" int b2f_explain_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev) {
-    return explain_device(m, rows_dev, n, row_format, phi_dev, B2F_OUT_EXPLAIN);
-}
-extern "C" int b2f_explain_interactions_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi2_dev) {
-    return explain_device(m, rows_dev, n, row_format, phi2_dev, B2F_OUT_INTERACTIONS);
-}
-
-/* The background table of n host rows (tree_shap_interventional.cuh): the rows' imputed words in tiles, a counting pass,
- * the offsets (scanned on the host), one allocation sized from them, a fill pass.  base_value = the path table's
- * path-dependent base value plus each path's move to the background mean (k_background_table), added in path order. */
-extern "C" int b2f_model_attach_background(b2f_model *m, const void *rows, int64_t n, int row_format, size_t *table_bytes) {
-    if (!m) return set_err(B2F_EINVAL, "model is NULL");
-    if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
-    if (n <= 0) return set_err(B2F_EINVAL, "background needs at least one row (n = %lld)", (long long)n);
-    if (!rows) return set_err(B2F_EINVAL, "rows is NULL");
-    if (row_format == B2F_ROWS_RANKED)
-        return set_err(B2F_EINVAL, "a background takes float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
-    int rc = check_row_format(m, row_format);
-    if (rc) return rc;
-    CUDA_TRY(cudaSetDevice(m->device));
-    Explainer &ex = *m->ex;
-    const int64_t P = ex.hdr.n_paths, tiles = (n + 31) / 32;
-    const int F = explain_fields(m);
-    const bool pk = row_format == B2F_ROWS_PACKED64;
-    Background bg;
-    bg.rows = n;
-    bg.vp.s = ex.ip.s;
-    bg.vp.s.denom = ex.hdr.denom * (double)n;
-    void *d_rows = nullptr, *d_words = nullptr, *d_counts = nullptr, *d_moved = nullptr;
-    auto done = [&](int code) { /* frees the scratch, and the new table unless it was attached */
-        for (void *b : {d_rows, d_words, d_counts, d_moved})
-            if (b) cudaFree(b);
-        if (code != B2F_OK && bg.d_table) cudaFree(bg.d_table);
-        return code;
-    };
-    auto cuda_fail = [&](const char *what) {
-        return done(set_err(B2F_ECUDA, "background %s failed: %s", what, cudaGetErrorString(cudaGetLastError())));
-    };
-    const size_t rows_bytes = (size_t)n * row_bytes_of(m, row_format), words_bytes = (size_t)tiles * F * 32 * sizeof(uint32_t);
-    if (cudaMalloc(&d_rows, rows_bytes) != cudaSuccess || cudaMalloc(&d_words, words_bytes) != cudaSuccess ||
-        cudaMalloc(&d_counts, (size_t)std::max<int64_t>(P, 1) * sizeof(long long)) != cudaSuccess ||
-        cudaMalloc(&d_moved, (size_t)std::max<int64_t>(P, 1) * sizeof(double)) != cudaSuccess)
-        return done(set_err(B2F_ENOMEM, "background scratch (%zu bytes of rows, %zu of words) allocation failed: %s", rows_bytes, words_bytes,
-                            cudaGetErrorString(cudaGetLastError())));
-    if (cudaMemcpy(d_rows, rows, rows_bytes, cudaMemcpyHostToDevice) != cudaSuccess) return cuda_fail("upload");
-    const uint32_t *rw = static_cast<const uint32_t *>(d_rows);
-    uint32_t *words = static_cast<uint32_t *>(d_words);
-    long long *counts = static_cast<long long *>(d_counts);
-    double *moved = static_cast<double *>(d_moved);
-    if (pk)
-        k_background_words<true><<<(unsigned)tiles, B2F_SHAP_THREADS>>>(bg.vp.s, rw, (long long)n, words);
-    else
-        k_background_words<false><<<(unsigned)tiles, B2F_SHAP_THREADS>>>(bg.vp.s, rw, (long long)n, words);
-    const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>(P, (int64_t)m->sm_count * 32));
-    if (P) k_background_table<false><<<grid, B2F_SHAP_THREADS>>>(bg.vp, words, (long long)n, counts, nullptr, nullptr);
-    if (cudaGetLastError() != cudaSuccess) return cuda_fail("counting pass");
-    std::vector<long long> off((size_t)P + 1, 0);
-    if (P && cudaMemcpy(off.data() + 1, counts, (size_t)P * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess)
-        return cuda_fail("counting pass");
-    for (int64_t p = 0; p < P; ++p) off[p + 1] += off[p];
-    const size_t off_bytes = off.size() * sizeof(long long);
-    bg.bytes = off_bytes + (size_t)off[P] * sizeof(uint2);
-    if (cudaMalloc(&bg.d_table, bg.bytes) != cudaSuccess) {
-        bg.d_table = nullptr;
-        return done(set_err(B2F_ENOMEM, "background table (%zu bytes) allocation failed: %s", bg.bytes, cudaGetErrorString(cudaGetLastError())));
-    }
-    bg.vp.offsets = static_cast<const long long *>(bg.d_table);
-    bg.vp.entries = reinterpret_cast<const uint2 *>(static_cast<uint8_t *>(bg.d_table) + off_bytes);
-    if (cudaMemcpy(bg.d_table, off.data(), off_bytes, cudaMemcpyHostToDevice) != cudaSuccess) return cuda_fail("offsets upload");
-    if (P)
-        k_background_table<true><<<grid, B2F_SHAP_THREADS>>>(bg.vp, words, (long long)n, nullptr, const_cast<uint2 *>(bg.vp.entries), moved);
-    if (cudaGetLastError() != cudaSuccess) return cuda_fail("fill pass");
-    std::vector<double> mv((size_t)P);
-    if (P && cudaMemcpy(mv.data(), moved, (size_t)P * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) return cuda_fail("fill pass");
-    double sum = 0.0;
-    for (double v : mv) sum += v;
-    bg.base_value = ex.hdr.base_value + sum / ex.hdr.denom;
-    /* replacing a background: nothing may still read the old table */
-    if (cudaDeviceSynchronize() != cudaSuccess) return cuda_fail("synchronise");
-    if (ex.bg.d_table) cudaFree(ex.bg.d_table);
-    ex.bg = bg;
-    if (table_bytes) *table_bytes = bg.bytes;
-    return done(B2F_OK);
-}
-
-extern "C" int b2f_explain_interventional(b2f_model *m, const void *rows, int64_t n, int row_format, double *phi, double *base_value,
-                                          float *device_ms) {
-    return explain_host(m, rows, n, row_format, phi, B2F_OUT_INTERVENTIONAL, base_value, device_ms);
-}
-extern "C" int b2f_explain_interventional_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, double *phi_dev) {
-    return explain_device(m, rows_dev, n, row_format, phi_dev, B2F_OUT_INTERVENTIONAL);
-}
-
-/* the spec goes up once, before the chunks that read it; no earlier host call still reads it (each one synchronises) */
-extern "C" int b2f_partial_dependence(b2f_model *m, const void *rows, int64_t n, int row_format, const b2f_pd_probe *probes, int n_probes,
-                                      const uint32_t *grid_words, double *out, float *device_ms) {
-    if (!m) return set_err(B2F_EINVAL, "model is NULL");
-    if (device_ms) *device_ms = 0.0f;
-    int rc = pd_prepare(m, probes, n_probes, grid_words);
-    if (rc) return rc;
-    if (n > 0) {
-        if ((rc = pd_check(m, row_format, out != nullptr))) return rc;
-        CUDA_TRY(cudaSetDevice(m->device));
-        const size_t bytes = m->pd.spec.size() * sizeof(uint32_t);
-        if ((rc = explain_reserve_scratch(m->pd.host, m->compute, bytes))) return rc;
-        CUDA_TRY(cudaMemcpy(m->pd.host.scratch, m->pd.spec.data(), bytes, cudaMemcpyHostToDevice));
-    }
-    return timed_host_batch(m, rows, n, row_format, out, B2F_OUT_DEPENDENCE, device_ms);
-}
-/* the spec is copied on the compute stream into the device form's own buffer, so it is ordered with the launch */
-extern "C" int b2f_partial_dependence_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const b2f_pd_probe *probes,
-                                             int n_probes, const uint32_t *grid_words, double *out_dev) {
-    if (!m) return set_err(B2F_EINVAL, "model is NULL");
-    if (n < 0) return set_err(B2F_EINVAL, "negative row count");
-    int rc = pd_prepare(m, probes, n_probes, grid_words);
-    if (rc == B2F_OK) rc = pd_check(m, row_format, out_dev != nullptr || n == 0);
-    if (rc == B2F_OK) rc = check_row_format(m, row_format);
-    if (rc) return rc;
-    if (n == 0) return B2F_OK;
-    CUDA_TRY(cudaSetDevice(m->device));
-    const size_t bytes = m->pd.spec.size() * sizeof(uint32_t);
-    if ((rc = explain_reserve_scratch(m->pd.compute, m->compute, bytes))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(m->pd.compute.scratch, m->pd.spec.data(), bytes, cudaMemcpyHostToDevice, m->compute));
-    return launch_dependence(m, m->compute, rows_dev, n, row_format, out_dev, m->pd.compute.scratch);
 }
 
 extern "C" int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned, int proba_is_f64,
@@ -1848,7 +1301,8 @@ extern "C" int b2f_predict_async_ex(b2f_model *m, const void *rows_pinned, int64
             if (t.used_mask & (1u << s)) CUDA_TRY(cudaEventSynchronize(t.ev[s]));
     }
     uint32_t mask = 0;
-    int rc = enqueue_host_batch(m, rows_pinned, n, row_format, proba1_pinned, proba_is_f64, label_pinned, &mask);
+    int rc = score_check(m, n, proba_is_f64, row_format, proba1_pinned);
+    if (rc == B2F_OK) rc = enqueue_host_batch(m, score_job(proba_is_f64), rows_pinned, n, row_format, proba1_pinned, label_pinned, &mask);
     if (rc) {
         sync_mask(m, mask);
         return rc;
@@ -1891,9 +1345,10 @@ extern "C" int b2f_predict_multi_ex(b2f_model **models, int n_models, const void
     for (int i = 0; i < n_models && rc == B2F_OK; ++i) {
         const int64_t lo = n * i / n_models, hi = n * (i + 1) / n_models;
         if (hi <= lo) continue;
-        rc = enqueue_host_batch(models[i], static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, hi - lo, row_format,
-                                proba1 ? static_cast<uint8_t *>(proba1) + (size_t)lo * out_bytes : nullptr, proba_is_f64, label ? label + lo : nullptr,
-                                &masks[i]);
+        rc = out_check(models[i], proba_is_f64, row_format, proba1 != nullptr);
+        if (rc == B2F_OK)
+            rc = enqueue_host_batch(models[i], score_job(proba_is_f64), static_cast<const uint8_t *>(rows) + (size_t)lo * row_bytes, hi - lo, row_format,
+                                    proba1 ? static_cast<uint8_t *>(proba1) + (size_t)lo * out_bytes : nullptr, label ? label + lo : nullptr, &masks[i]);
     }
     for (int i = 0; i < n_models; ++i) {
         cudaSetDevice(models[i]->device);
@@ -1997,8 +1452,31 @@ extern "C" int b2f_sync(b2f_model *m) {
     return B2F_OK;
 }
 
-static int ensure_flush(b2f_model *m) {
-    if (!m->d_flush) CUDA_TRY(cudaMalloc(&m->d_flush, B2F_FLUSH_BYTES));
+/* iters launches on the compute stream, timed by events this function owns.  ms_each: an event pair around each launch, after
+ * a memset that flushes L2 when flush_l2 is set.  ms_total: one pair around the whole loop.  Without ms_each nothing is
+ * recorded between launches: an event record between two launches keeps them from overlapping (programmatic dependent launch
+ * of the rank kernel).  launch(i) enqueues launch i. */
+template <typename Launch>
+static int timed_launches(b2f_model *m, int iters, bool flush_l2, float *ms_each, float *ms_total, Launch launch) {
+    const cudaStream_t st = m->compute;
+    int rc = flush_l2 ? m->flush.reserve(st, B2F_FLUSH_BYTES, B2F_FLUSH_BYTES) : B2F_OK;
+    Events ev;
+    const size_t n_each = ms_each ? 2 * (size_t)iters : 0;
+    if (rc == B2F_OK) rc = ev.create(n_each + (ms_total ? 2 : 0));
+    if (rc) return rc;
+    cudaEvent_t *each = ev.e.data(), *region = each + n_each;
+    if (ms_total) CUDA_TRY(cudaEventRecord(region[0], st));
+    for (int i = 0; i < iters && rc == B2F_OK; ++i) {
+        if (flush_l2) CUDA_TRY(cudaMemsetAsync(m->flush.p, i & 0xff, B2F_FLUSH_BYTES, st));
+        if (ms_each) CUDA_TRY(cudaEventRecord(each[2 * i], st));
+        rc = launch(i);
+        if (ms_each) CUDA_TRY(cudaEventRecord(each[2 * i + 1], st));
+    }
+    if (ms_total) CUDA_TRY(cudaEventRecord(region[1], st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (rc) return rc;
+    for (int i = 0; ms_each && i < iters; ++i) CUDA_TRY(cudaEventElapsedTime(&ms_each[i], each[2 * i], each[2 * i + 1]));
+    if (ms_total) CUDA_TRY(cudaEventElapsedTime(ms_total, region[0], region[1]));
     return B2F_OK;
 }
 
@@ -2006,28 +1484,14 @@ extern "C" int b2f_predict_device_timed(b2f_model *m, const void *rows_dev, int6
                                         int iters, int flush_l2, float *ms_each) {
     if (!m || iters <= 0 || !ms_each) return set_err(B2F_EINVAL, "bad argument");
     CUDA_TRY(cudaSetDevice(m->device));
-    if (flush_l2) {
-        int rc = ensure_flush(m);
-        if (rc) return rc;
-    }
-    std::vector<cudaEvent_t> ev(2 * (size_t)iters);
-    for (auto &e : ev) CUDA_TRY(cudaEventCreate(&e));
-    int rc = B2F_OK;
-    for (int i = 0; i < iters && rc == B2F_OK; ++i) {
-        if (flush_l2) CUDA_TRY(cudaMemsetAsync(m->d_flush, i & 0xff, B2F_FLUSH_BYTES, m->compute));
-        CUDA_TRY(cudaEventRecord(ev[2 * i], m->compute));
-        rc = out_launch(m, m->compute, rows_dev, n, B2F_ROWS_WORDS24, proba_is_f64 ? B2F_OUT_F64 : B2F_OUT_F32, proba1_dev, label_dev);
-        CUDA_TRY(cudaEventRecord(ev[2 * i + 1], m->compute));
-    }
-    CUDA_TRY(cudaStreamSynchronize(m->compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(cudaEventElapsedTime(&ms_each[i], ev[2 * i], ev[2 * i + 1]));
-    for (auto &e : ev) cudaEventDestroy(e);
-    return rc;
+    const int kind = proba_is_f64 ? B2F_OUT_F64 : B2F_OUT_F32;
+    return timed_launches(m, iters, flush_l2, ms_each, nullptr,
+                          [&](int) { return out_launch(m, m->compute, rows_dev, n, B2F_ROWS_WORDS24, kind, proba1_dev, label_dev); });
 }
 
 /* Streaming measurement: `steps` launches over a pool of `pool` distinct device-resident batches
  * (batch i%pool), so consecutive steps read different HBM lines (pool * n * 96 B should exceed L2).
- * Per-launch events and one region event pair, all on the launching stream. */
+ * Per-launch events (when ms_each is not NULL) and one region event pair, all on the launching stream. */
 extern "C" int b2f_predict_stream_timed(b2f_model *m, const void *rows_dev, int64_t n, int pool, void *proba1_dev, int proba_is_f64,
                                         int32_t *label_dev, int steps, float *ms_each, float *ms_total) {
     return b2f_predict_stream_timed_ex(m, rows_dev, n, B2F_ROWS_WORDS24, pool, proba1_dev, proba_is_f64, label_dev, steps, ms_each, ms_total);
@@ -2042,30 +1506,13 @@ extern "C" int b2f_predict_stream_timed_ex(b2f_model *m, const void *rows_dev, i
     }
     const size_t row_bytes = row_bytes_of(m, row_format);
     CUDA_TRY(cudaSetDevice(m->device));
-    /* per-launch events only when the caller asks for per-launch times: an event record between two launches keeps
-     * them from overlapping (programmatic dependent launch of the rank kernel), so the region time is measured without */
-    const bool each = ms_each != nullptr;
-    std::vector<cudaEvent_t> ev(each ? 2 * (size_t)steps + 2 : 2);
-    for (auto &e : ev) CUDA_TRY(cudaEventCreate(&e));
     const int kind = proba_is_f64 ? B2F_OUT_F64 : B2F_OUT_F32;
     const size_t out_bytes = out_row_bytes(kind);
-    const size_t i0 = ev.size() - 2, i1 = ev.size() - 1;
-    int rc = B2F_OK;
-    CUDA_TRY(cudaEventRecord(ev[i0], m->compute));
-    for (int i = 0; i < steps && rc == B2F_OK; ++i) {
+    return timed_launches(m, steps, false, ms_each, ms_total, [&](int i) {
         const size_t b = (size_t)(i % pool);
-        if (each) CUDA_TRY(cudaEventRecord(ev[2 * i], m->compute));
-        rc = out_launch(m, m->compute, static_cast<const uint8_t *>(rows_dev) + b * (size_t)n * row_bytes, n, row_format, kind,
-                        proba1_dev ? static_cast<uint8_t *>(proba1_dev) + b * (size_t)n * out_bytes : nullptr, label_dev ? label_dev + b * (size_t)n : nullptr);
-        if (each) CUDA_TRY(cudaEventRecord(ev[2 * i + 1], m->compute));
-    }
-    CUDA_TRY(cudaEventRecord(ev[i1], m->compute));
-    CUDA_TRY(cudaStreamSynchronize(m->compute));
-    if (each)
-        for (int i = 0; i < steps; ++i) CUDA_TRY(cudaEventElapsedTime(&ms_each[i], ev[2 * i], ev[2 * i + 1]));
-    CUDA_TRY(cudaEventElapsedTime(ms_total, ev[i0], ev[i1]));
-    for (auto &e : ev) cudaEventDestroy(e);
-    return rc;
+        return out_launch(m, m->compute, static_cast<const uint8_t *>(rows_dev) + b * (size_t)n * row_bytes, n, row_format, kind,
+                          proba1_dev ? static_cast<uint8_t *>(proba1_dev) + b * (size_t)n * out_bytes : nullptr, label_dev ? label_dev + b * (size_t)n : nullptr);
+    });
 }
 
 /* ------------------------------------------------------------------ moments */
@@ -2094,15 +1541,9 @@ extern "C" int b2f_moments_device(b2f_model *m, const void *rows_dev, int64_t n,
 }
 
 static int moments_stage(b2f_model *m, const void *rows, int64_t n) {
-    if (n > m->mom_cap_rows) {
-        CUDA_TRY(cudaStreamSynchronize(m->compute));
-        if (m->d_mom_rows) cudaFree(m->d_mom_rows);
-        m->d_mom_rows = nullptr;
-        m->mom_cap_rows = 0;
-        CUDA_TRY(cudaMalloc(&m->d_mom_rows, (size_t)std::max<int64_t>(n, 1024) * B2F_ROW_BYTES));
-        m->mom_cap_rows = std::max<int64_t>(n, 1024);
-    }
-    if (n > 0) CUDA_TRY(cudaMemcpyAsync(m->d_mom_rows, rows, (size_t)n * B2F_ROW_BYTES, cudaMemcpyHostToDevice, m->compute));
+    int rc = m->mom_rows.reserve(m->compute, (size_t)n * B2F_ROW_BYTES, (size_t)std::max<int64_t>(n, 1024) * B2F_ROW_BYTES);
+    if (rc) return rc;
+    if (n > 0) CUDA_TRY(cudaMemcpyAsync(m->mom_rows.p, rows, (size_t)n * B2F_ROW_BYTES, cudaMemcpyHostToDevice, m->compute));
     return B2F_OK;
 }
 
@@ -2111,30 +1552,17 @@ extern "C" int b2f_moments(b2f_model *m, const void *rows, int64_t n, double *ou
     CUDA_TRY(cudaSetDevice(m->device));
     int rc = moments_stage(m, rows, n);
     if (rc) return rc;
-    return b2f_moments_device(m, m->d_mom_rows, n, out);
+    return b2f_moments_device(m, m->mom_rows.p, n, out);
 }
 
 extern "C" int b2f_moments_device_timed(b2f_model *m, const void *rows_dev, int64_t n, int iters, int flush_l2, float *ms_each, double *out) {
     if (!m || iters <= 0 || !ms_each) return set_err(B2F_EINVAL, "bad argument");
     CUDA_TRY(cudaSetDevice(m->device));
-    if (flush_l2) {
-        int rc = ensure_flush(m);
-        if (rc) return rc;
-    }
-    std::vector<cudaEvent_t> ev(2 * (size_t)iters);
-    for (auto &e : ev) CUDA_TRY(cudaEventCreate(&e));
-    int rc = B2F_OK;
-    for (int i = 0; i < iters && rc == B2F_OK; ++i) {
-        if (flush_l2) CUDA_TRY(cudaMemsetAsync(m->d_flush, i & 0xff, B2F_FLUSH_BYTES, m->compute));
-        CUDA_TRY(cudaEventRecord(ev[2 * i], m->compute));
-        rc = launch_moments(m, rows_dev, n);
-        CUDA_TRY(cudaEventRecord(ev[2 * i + 1], m->compute));
-    }
-    if (out) CUDA_TRY(cudaMemcpyAsync(out, m->d_mom_out, B2F_MOM_VALUES * sizeof(double), cudaMemcpyDeviceToHost, m->compute));
+    int rc = timed_launches(m, iters, flush_l2, ms_each, nullptr, [&](int) { return launch_moments(m, rows_dev, n); });
+    if (rc || !out) return rc;
+    CUDA_TRY(cudaMemcpyAsync(out, m->d_mom_out, B2F_MOM_VALUES * sizeof(double), cudaMemcpyDeviceToHost, m->compute));
     CUDA_TRY(cudaStreamSynchronize(m->compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(cudaEventElapsedTime(&ms_each[i], ev[2 * i], ev[2 * i + 1]));
-    for (auto &e : ev) cudaEventDestroy(e);
-    return rc;
+    return B2F_OK;
 }
 
 /* Chan et al. pairwise merge of (count, mean, M2), in part order */
@@ -2174,13 +1602,8 @@ extern "C" int b2f_comm_unique_id(void *id_out128) {
 }
 
 static int comm_buffers(b2f_model *m, int nranks) {
-    if (nranks > m->gather_cap) {
-        if (m->d_gather) cudaFree(m->d_gather);
-        m->d_gather = nullptr;
-        CUDA_TRY(cudaMalloc(&m->d_gather, (size_t)(nranks + 1) * B2F_MOM_VALUES * sizeof(double)));
-        m->gather_cap = nranks;
-    }
-    return B2F_OK;
+    const size_t bytes = (size_t)(nranks + 1) * B2F_MOM_VALUES * sizeof(double);
+    return m->gather.reserve(m->compute, bytes, bytes);
 }
 
 extern "C" int b2f_comm_init_rank(b2f_model *m, int nranks, int rank, const void *id128) {
@@ -2219,11 +1642,11 @@ extern "C" int b2f_moments_allgather(b2f_model *m, const double *local, double *
     if (!m || !local || !merged) return set_err(B2F_EINVAL, "null argument");
     if (!m->comm) return set_err(B2F_ESTATE, "communicator not initialised (call b2f_comm_init_rank)");
     CUDA_TRY(cudaSetDevice(m->device));
-    double *send = m->d_gather + (size_t)m->nranks * B2F_MOM_VALUES;
+    double *gather = static_cast<double *>(m->gather.p), *send = gather + (size_t)m->nranks * B2F_MOM_VALUES;
     CUDA_TRY(cudaMemcpyAsync(send, local, B2F_MOM_VALUES * sizeof(double), cudaMemcpyHostToDevice, m->compute));
-    NCCL_TRY(g_nccl.AllGather(send, m->d_gather, B2F_MOM_VALUES, ncclDouble, m->comm, m->compute));
+    NCCL_TRY(g_nccl.AllGather(send, gather, B2F_MOM_VALUES, ncclDouble, m->comm, m->compute));
     std::vector<double> parts((size_t)m->nranks * B2F_MOM_VALUES);
-    CUDA_TRY(cudaMemcpyAsync(parts.data(), m->d_gather, parts.size() * sizeof(double), cudaMemcpyDeviceToHost, m->compute));
+    CUDA_TRY(cudaMemcpyAsync(parts.data(), gather, parts.size() * sizeof(double), cudaMemcpyDeviceToHost, m->compute));
     CUDA_TRY(cudaStreamSynchronize(m->compute));
     b2f_moments_merge(parts.data(), m->nranks, merged);
     return B2F_OK;
@@ -2238,7 +1661,7 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
         const int64_t lo = n * i / n_models, hi = n * (i + 1) / n_models;
         CUDA_TRY(cudaSetDevice(m->device));
         rc = moments_stage(m, static_cast<const uint8_t *>(rows) + (size_t)lo * B2F_ROW_BYTES, hi - lo);
-        if (rc == B2F_OK) rc = launch_moments(m, m->d_mom_rows, hi - lo);
+        if (rc == B2F_OK) rc = launch_moments(m, m->mom_rows.p, hi - lo);
     }
     if (rc) return rc;
     const bool use_nccl = models[0]->comm != nullptr && models[0]->nranks == n_models;
@@ -2248,7 +1671,7 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
         NCCL_TRY(g_nccl.GroupStart());
         for (int i = 0; i < n_models; ++i) {
             b2f_model *m = models[i];
-            ncclResult_t r = g_nccl.AllGather(m->d_mom_out, m->d_gather, B2F_MOM_VALUES, ncclDouble, m->comm, m->compute);
+            ncclResult_t r = g_nccl.AllGather(m->d_mom_out, m->gather.p, B2F_MOM_VALUES, ncclDouble, m->comm, m->compute);
             if (r != ncclSuccess) {
                 g_nccl.GroupEnd();
                 return set_err(B2F_ENCCL, "ncclAllGather failed: %s", g_nccl.GetErrorString(r));
@@ -2256,7 +1679,7 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
         }
         NCCL_TRY(g_nccl.GroupEnd());
         CUDA_TRY(cudaSetDevice(models[0]->device));
-        CUDA_TRY(cudaMemcpyAsync(parts.data(), models[0]->d_gather, parts.size() * sizeof(double), cudaMemcpyDeviceToHost, models[0]->compute));
+        CUDA_TRY(cudaMemcpyAsync(parts.data(), models[0]->gather.p, parts.size() * sizeof(double), cudaMemcpyDeviceToHost, models[0]->compute));
         for (int i = 0; i < n_models; ++i) {
             CUDA_TRY(cudaSetDevice(models[i]->device));
             CUDA_TRY(cudaStreamSynchronize(models[i]->compute));
@@ -2279,3 +1702,9 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
 
 /* ------------------------------------------------------------------ batch drift detector (K3) */
 #include "drift_api.cuh"
+
+/* ------------------------------------------------------------------ explanations (K5) */
+#include "explain_api.cuh"
+
+/* ------------------------------------------------------------------ partial dependence (K6) */
+#include "dependence_api.cuh"

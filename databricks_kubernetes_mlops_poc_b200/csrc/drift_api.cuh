@@ -23,16 +23,12 @@ struct b2f_drift {
     int64_t *d_ref_counts = nullptr;
     void *d_hist = nullptr; /* hist_a | hist_b | nan_count | cat_hist, one memset */
     size_t hist_bytes = 0;
-    double *d_x = nullptr;
-    int32_t *d_codes = nullptr;
-    int64_t cap_rows = 0;
+    DevBuf x, codes; /* the batch's numeric columns and category codes, n + n/2 rows' worth */
     int32_t *d_new_off = nullptr;
-    int64_t *d_new_counts = nullptr;
-    int64_t new_cap = 0;
+    DevBuf new_counts;
     double *d_rows = nullptr; /* row-scan scratch: [n_num][2][B2F_DRIFT_ROW_STRIDE(n_ref)] */
     int rowscan_max_n = 0, rowscan_smem_max_n = 0;
-    double *d_wide = nullptr; /* wide-band sweep scratch: [n_num][2][wide_ring], grown on demand */
-    int64_t wide_ring = 0;
+    DevBuf wide; /* wide-band sweep scratch: [n_num][2][ring slots] for the widest ring a batch needed so far */
     size_t finish_smem = 0;
     void *d_out = nullptr; /* p_val[F] | stat[F] | flags[F] */
     void *h_out = nullptr; /* pinned mirror */
@@ -47,12 +43,9 @@ extern "C" void b2f_drift_destroy(b2f_drift *d) {
     if (d->d_cat_off) cudaFree(d->d_cat_off);
     if (d->d_ref_counts) cudaFree(d->d_ref_counts);
     if (d->d_hist) cudaFree(d->d_hist);
-    if (d->d_x) cudaFree(d->d_x);
-    if (d->d_codes) cudaFree(d->d_codes);
+    for (DevBuf *b : {&d->x, &d->codes, &d->new_counts, &d->wide}) b->release();
     if (d->d_new_off) cudaFree(d->d_new_off);
-    if (d->d_new_counts) cudaFree(d->d_new_counts);
     if (d->d_rows) cudaFree(d->d_rows);
-    if (d->d_wide) cudaFree(d->d_wide);
     if (d->d_out) cudaFree(d->d_out);
     if (d->h_out) cudaFreeHost(d->h_out);
     if (d->ev0) cudaEventDestroy(d->ev0);
@@ -235,18 +228,10 @@ extern "C" int b2f_drift_score(b2f_drift *d, int64_t n, const double *num_cols, 
     if ((d->n_num > 0 && !num_cols) || (d->n_cat > 0 && !cat_codes) || !p_val) return set_err(B2F_EINVAL, "drift: NULL argument");
     if (n > (1 << 26)) return set_err(B2F_EINVAL, "drift: batch too large");
     CUDA_TRY(cudaSetDevice(d->device));
-    if (n > d->cap_rows) {
-        CUDA_TRY(cudaStreamSynchronize(d->stream));
-        if (d->d_x) cudaFree(d->d_x);
-        if (d->d_codes) cudaFree(d->d_codes);
-        d->d_x = nullptr;
-        d->d_codes = nullptr;
-        d->cap_rows = 0;
-        const int64_t cap = std::max<int64_t>(n + n / 2, 1024);
-        CUDA_TRY(cudaMalloc((void **)&d->d_x, std::max<size_t>((size_t)cap * d->n_num * sizeof(double), 8)));
-        CUDA_TRY(cudaMalloc((void **)&d->d_codes, std::max<size_t>((size_t)cap * d->n_cat * sizeof(int32_t), 8)));
-        d->cap_rows = cap;
-    }
+    const size_t cap = (size_t)std::max<int64_t>(n + n / 2, 1024), x_row = d->n_num * sizeof(double), codes_row = d->n_cat * sizeof(int32_t);
+    int rc = d->x.reserve(d->stream, std::max<size_t>(n * x_row, 8), std::max<size_t>(cap * x_row, 8));
+    if (rc == B2F_OK) rc = d->codes.reserve(d->stream, std::max<size_t>(n * codes_row, 8), std::max<size_t>(cap * codes_row, 8));
+    if (rc) return rc;
     /* the widest sweep ring this batch size can need (h <= lcm: D <= 1); beyond B2F_DRIFT_RING_MAX slots the sweep keeps its two
      * rings in a global scratch.  Where lcm >= 2^31 (flag 1) no sweep runs. */
     int64_t wide_need = 0;
@@ -265,14 +250,8 @@ extern "C" int b2f_drift_score(b2f_drift *d, int64_t n, const double *num_cols, 
             if (ring > B2F_DRIFT_RING_MAX) wide_need = ring;
         }
     }
-    if (wide_need > d->wide_ring) {
-        CUDA_TRY(cudaStreamSynchronize(d->stream));
-        if (d->d_wide) cudaFree(d->d_wide);
-        d->d_wide = nullptr;
-        d->wide_ring = 0;
-        CUDA_TRY(cudaMalloc((void **)&d->d_wide, (size_t)d->n_num * 2 * (size_t)wide_need * sizeof(double)));
-        d->wide_ring = wide_need;
-    }
+    const size_t wide_slot = (size_t)d->n_num * 2 * sizeof(double); /* bytes per ring slot over the features */
+    if ((rc = d->wide.reserve(d->stream, wide_slot * wide_need, wide_slot * wide_need))) return rc;
     int64_t n_new = 0;
     if (new_offsets) {
         if (!new_counts && new_offsets[d->n_cat] > 0) return set_err(B2F_EINVAL, "drift: new_counts is NULL");
@@ -281,21 +260,15 @@ extern "C" int b2f_drift_score(b2f_drift *d, int64_t n, const double *num_cols, 
             if (k < 0 || k + (d->cat_off[c + 1] - d->cat_off[c]) > B2F_DRIFT_MAX_CATS) return set_err(B2F_EINVAL, "drift: too many categories for feature %d", c);
         }
         n_new = new_offsets[d->n_cat];
-        if (n_new > d->new_cap) {
-            CUDA_TRY(cudaStreamSynchronize(d->stream));
-            if (d->d_new_counts) cudaFree(d->d_new_counts);
-            d->d_new_counts = nullptr;
-            CUDA_TRY(cudaMalloc((void **)&d->d_new_counts, (size_t)(n_new + 64) * sizeof(int64_t)));
-            d->new_cap = n_new + 64;
-        }
+        if ((rc = d->new_counts.reserve(d->stream, (size_t)n_new * sizeof(int64_t), (size_t)(n_new + 64) * sizeof(int64_t)))) return rc;
         CUDA_TRY(cudaMemcpyAsync(d->d_new_off, new_offsets, (d->n_cat + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, d->stream));
-        if (n_new) CUDA_TRY(cudaMemcpyAsync(d->d_new_counts, new_counts, (size_t)n_new * sizeof(int64_t), cudaMemcpyHostToDevice, d->stream));
+        if (n_new) CUDA_TRY(cudaMemcpyAsync(d->new_counts.p, new_counts, (size_t)n_new * sizeof(int64_t), cudaMemcpyHostToDevice, d->stream));
     }
     const int F = d->n_num + d->n_cat;
     CUDA_TRY(cudaEventRecord(d->ev0, d->stream));
     /* the batch arrives feature-major with stride n: one copy per kind */
-    if (d->n_num) CUDA_TRY(cudaMemcpyAsync(d->d_x, num_cols, (size_t)n * d->n_num * sizeof(double), cudaMemcpyHostToDevice, d->stream));
-    if (d->n_cat) CUDA_TRY(cudaMemcpyAsync(d->d_codes, cat_codes, (size_t)n * d->n_cat * sizeof(int32_t), cudaMemcpyHostToDevice, d->stream));
+    if (d->n_num) CUDA_TRY(cudaMemcpyAsync(d->x.p, num_cols, (size_t)n * d->n_num * sizeof(double), cudaMemcpyHostToDevice, d->stream));
+    if (d->n_cat) CUDA_TRY(cudaMemcpyAsync(d->codes.p, cat_codes, (size_t)n * d->n_cat * sizeof(int32_t), cudaMemcpyHostToDevice, d->stream));
     CUDA_TRY(cudaMemsetAsync(d->d_hist, 0, d->hist_bytes, d->stream));
     DriftParams p;
     memset(&p, 0, sizeof(p));
@@ -304,8 +277,8 @@ extern "C" int b2f_drift_score(b2f_drift *d, int64_t n, const double *num_cols, 
     p.n_num = d->n_num;
     p.n_cat = d->n_cat;
     p.ref_sorted = d->d_ref;
-    p.x = d->d_x;
-    p.codes = d->d_codes;
+    p.x = static_cast<double *>(d->x.p);
+    p.codes = static_cast<int32_t *>(d->codes.p);
     uint32_t *hp = static_cast<uint32_t *>(d->d_hist);
     p.hist_a = hp;
     p.hist_b = hp + (size_t)d->n_num * (d->n_ref + 1);
@@ -314,7 +287,7 @@ extern "C" int b2f_drift_score(b2f_drift *d, int64_t n, const double *num_cols, 
     p.cat_off = d->d_cat_off;
     p.ref_counts = d->d_ref_counts;
     p.new_off = new_offsets ? d->d_new_off : nullptr;
-    p.new_counts = d->d_new_counts;
+    p.new_counts = static_cast<int64_t *>(d->new_counts.p);
     p.p_val = static_cast<double *>(d->d_out);
     p.stat = p.p_val + F;
     p.flags = reinterpret_cast<int32_t *>(p.stat + F);
@@ -322,8 +295,8 @@ extern "C" int b2f_drift_score(b2f_drift *d, int64_t n, const double *num_cols, 
     p.rowscan_max_n = d->rowscan_max_n;
     p.rowscan_smem_max_n = (n >= 2 && n <= d->rowscan_smem_max_n) ? d->rowscan_smem_max_n : 0;
     p.rowscan_cap = B2F_DRIFT_ROWSCAN_CAP;
-    p.wide_scratch = d->d_wide;
-    p.wide_ring = d->wide_ring;
+    p.wide_scratch = static_cast<double *>(d->wide.p);
+    p.wide_ring = d->n_num ? (int64_t)(d->wide.bytes / wide_slot) : 0;
     const int64_t total = n * F;
     const unsigned blocks = (unsigned)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, (int64_t)d->sm_count * 8));
     k_drift_count<<<blocks, 256, 0, d->stream>>>(p);

@@ -251,7 +251,8 @@ struct b2f_scorer {
     int64_t n = 0, chunk_rows = 0;
     int64_t chunk_lo[B2F_SCORER_MAX_CHUNKS + 1] = {}; /* chunk c = rows [chunk_lo[c], chunk_lo[c + 1]) */
     int n_chunks = 0, parts_per_chunk = 1;
-    int row_format = 0, out_mode = B2F_OUT_F64;
+    int row_format = 0;
+    HostJob job{}; /* score_job of the output kind */
     const b2f_str_column *cats = nullptr;
     const double *const *nums = nullptr;
     const int64_t *strides = nullptr;
@@ -287,7 +288,7 @@ static void scorer_submit_chunk(b2f_scorer *s, int c) {
     {
         std::lock_guard<std::mutex> lk(s->mu);
         Slot &sl = m->slots[c % B2F_STREAMS];
-        rc = submit_chunk(m, sl, s->h_rows, s->row_format, s->out_mode, s->h_out, nullptr, lo, cnt, nullptr);
+        rc = submit_chunk(m, sl, s->job, s->h_rows, s->row_format, s->h_out, nullptr, lo, cnt, nullptr);
         const cudaError_t e = rc == B2F_OK ? cudaEventRecord(s->ev[c], sl.stream) : cudaSuccess;
         if (e != cudaSuccess) {
             snprintf(s->err, sizeof(s->err), "CUDA error while submitting chunk %d: %s", c, cudaGetErrorString(e));
@@ -472,7 +473,7 @@ extern "C" int b2f_scorer_start(b2f_scorer *s, int64_t n, const b2f_str_column *
     s->chunk_rows = chunk_rows;
     s->n_chunks = n_chunks;
     s->row_format = row_format;
-    s->out_mode = out_mode;
+    s->job = score_job(out_mode);
     s->cats = cat_cols;
     s->nums = num_cols;
     s->strides = num_strides;

@@ -213,17 +213,39 @@ def test_errors_leave_the_handle_working(rf100d6, curated):
 
 
 def test_interleaved_calls(rf100d6, curated):
+    from databricks_kubernetes_mlops_poc_b200.engine import ForestEngine
     from oracle import reference_pipeline as rp
 
-    flat, eng, enc, _ = _engine(rf100d6)
+    flat, eng, enc, table = _engine(rf100d6)
+    probes, grid = [(12, 0, 64)], np.linspace(-5.0, 5e5, 64, dtype=np.float32).view(np.uint32)
     try:
         rows = enc.encode_frame(curated[rp.FEATURES].iloc[:5000])
         alone = (eng.predict_rows(rows, np.float64)[0], eng.explain_rows(rows)[0], eng.explain_interactions_rows(rows)[0])
+        pd_alone = eng.partial_dependence_rows(rows, probes, grid)
         for _ in range(2):
             p2 = eng.explain_interactions_rows(rows)[0]
             p = eng.predict_rows(rows, np.float64)[0]
             phi = eng.explain_rows(rows)[0]
             assert np.array_equal(p, alone[0]) and np.array_equal(phi, alone[1]) and np.array_equal(p2, alone[2])
+    finally:
+        eng.close()
+    # every slot stream carries a score batch still in flight when explain, interactions and partial dependence grow the
+    # output and scratch buffers those batches share: each buffer is freed only after its stream has finished with it
+    eng = ForestEngine(flat, 0)
+    try:
+        eng.attach_explainer(table)
+        n = len(rows)
+        staged, proba, label = eng.staging(4 * n)
+        proba[:] = -1
+        tickets = []
+        for k in range(4):
+            staged[k * n : (k + 1) * n] = rows
+            tickets.append(eng.predict_rows_async(staged[k * n : (k + 1) * n], proba[k * n : (k + 1) * n], label[k * n : (k + 1) * n]))
+        got = (eng.explain_rows(rows)[0], eng.explain_interactions_rows(rows)[0], eng.partial_dependence_rows(rows, probes, grid))
+        for t in tickets:
+            eng.wait(t)
+        assert np.array_equal(proba, np.tile(alone[0], 4))
+        assert np.array_equal(got[0], alone[1]) and np.array_equal(got[1], alone[2]) and np.array_equal(got[2], pd_alone)
     finally:
         eng.close()
 
