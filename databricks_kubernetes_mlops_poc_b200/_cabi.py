@@ -33,6 +33,9 @@ SCORED_FULL_DTYPE = np.dtype(  # b2f_scored_full, 24 bytes
 )
 MOMENT_VALUES = ROW_WORDS * 3
 PD_PROBE_DTYPE = np.dtype([("word", np.int32), ("grid_offset", np.int32), ("count", np.int32)])  # b2f_pd_probe
+COUNTERFACTUAL_DTYPE = np.dtype(  # struct b2f_counterfactual, 32 bytes
+    [("lower_p1", np.float64), ("upper_p1", np.float64), ("lower", np.float32), ("upper", np.float32), ("value", np.float32), ("reserved", np.int32)]
+)
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG_DIR, "lib", "libb200forest.so")
@@ -120,6 +123,7 @@ SIGNATURES = {
     "b2f_last_error": (C.c_char_p, []),
     "b2f_device_count": (C.c_int, []),
     "b2f_blob_validate": (C.c_int, [C.c_void_p, C.c_size_t]),
+    "b2f_blob_split_values": (C.c_int64, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_int64]),
     "b2f_model_create": (C.c_void_p, [C.c_void_p, C.c_size_t, C.c_int]),
     "b2f_model_destroy": (None, [C.c_void_p]),
     "b2f_model_info": (C.c_int, [C.c_void_p, C.POINTER(Info)]),
@@ -176,6 +180,14 @@ SIGNATURES = {
         [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)],
     ),
     "b2f_partial_dependence_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "b2f_counterfactual": (
+        C.c_int,
+        [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)],
+    ),
+    "b2f_counterfactual_device": (
+        C.c_int,
+        [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_void_p],
+    ),
     "b2f_predict_async_ex": (
         C.c_int,
         [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_uint64)],

@@ -33,6 +33,7 @@
 #include "forest_predict_rank.cuh"
 #include "forest_rank.h"
 #include "partial_dependence.cuh"
+#include "counterfactual.cuh"
 #include "tree_shap.cuh"
 #include "tree_shap_interactions.cuh"
 #include "tree_shap_interventional.cuh"
@@ -165,6 +166,15 @@ struct Dependence {
     DevBuf device_spec;         /* the device form's: a host call never overwrites a spec an enqueued device-form launch reads */
 };
 
+/* nearest single-field counterfactuals (b2f_counterfactual; counterfactual.cuh).  The split-value table is built on the
+ * first call; the forest fields of cp are set at model creation, the probe fields are the current call's. */
+struct Counterfactual {
+    CfParams cp;
+    bool built = false;
+    std::vector<uint32_t> table; /* offset[24], count[24] per row word, then the float32 split values */
+    DevBuf dev;                  /* the table on the device */
+};
+
 struct TicketRec {
     uint64_t id = 0;
     cudaEvent_t ev[B2F_STREAMS] = {nullptr, nullptr, nullptr, nullptr};
@@ -209,6 +219,7 @@ struct b2f_model {
     int64_t forest_bytes = 0;
     Explainer *ex = nullptr; /* attached TreeSHAP path table (b2f_model_attach_explainer) */
     Dependence pd;
+    Counterfactual cf;
     b2f_model *outlier = nullptr; /* attached isolation forest (b2f_model_attach_outlier_forest): a child handle on the
                                      same device whose kernels are launched on this handle's streams and rows */
     Slot slots[B2F_STREAMS];
@@ -699,6 +710,8 @@ static int warp_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
         pp.g_slots[g] = gt[g].n_slots;
         pp.g_trees[g] = gt[g].n_trees;
     }
+    memset(&m->cf.cp, 0, sizeof(m->cf.cp));
+    m->cf.cp.pd = pp;
 
     /* the packed 64-byte row needs the credit-default shape: exactly 9 categoricals of <= 126 categories, <= 14 numerics */
     m->packed_ok = m->hdr.n_cat == 9 && m->hdr.n_num <= 14; /* the kernels decode word L-7 / q[2+k] for exactly nine 7-bit fields */
@@ -851,7 +864,7 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
         for (DevBuf *b : {&sl.rows, &sl.out, &sl.label, &sl.scratch}) b->release();
         if (sl.stream) cudaStreamDestroy(sl.stream);
     }
-    for (DevBuf *b : {&m->scratch, &m->pd.host_spec, &m->pd.device_spec, &m->mom_rows, &m->gather, &m->flush}) b->release();
+    for (DevBuf *b : {&m->scratch, &m->pd.host_spec, &m->pd.device_spec, &m->cf.dev, &m->mom_rows, &m->gather, &m->flush}) b->release();
     for (auto &t : m->tickets)
         for (auto &e : t.ev)
             if (e) cudaEventDestroy(e);
@@ -1708,3 +1721,6 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
 
 /* ------------------------------------------------------------------ partial dependence (K6) */
 #include "dependence_api.cuh"
+
+/* ------------------------------------------------------------------ counterfactuals (K7) */
+#include "counterfactual_api.cuh"

@@ -126,6 +126,35 @@ static int tree_depth(const Tree &t, uint32_t s, int d, int limit) {
 
 }  // namespace rankdetail
 
+/* The sorted distinct split values t' of each numeric feature over the whole forest, at any depth: thr[k] for row word
+ * n_cat + k.  -0.0 and +0.0 collapse (float ==), as the comparison sees them.  Every lane of a group below its tree count is
+ * read, node slot by node slot.  Returns NULL, or why the forest has no such table (thr is then unspecified). */
+static const char *forest_split_values(const uint8_t *blob, const b2f_blob_header &h, std::vector<std::vector<float>> &thr) {
+    const int n_cat = (int)h.n_cat, n_num = (int)h.n_num;
+    thr.assign(n_num, {});
+    const b2f_blob_group *gt = reinterpret_cast<const b2f_blob_group *>(blob + h.groups_off);
+    for (uint32_t t = 0; t < h.n_trees; ++t) {
+        const b2f_blob_group &gr = gt[t / 32];
+        const uint32_t *N = reinterpret_cast<const uint32_t *>(blob + h.chunks_off + gr.chunk_off);
+        for (uint32_t s = 0; s < gr.n_slots; ++s) {
+            const uint32_t T = N[(s * 32 + t % 32) * 2], M = N[(s * 32 + t % 32) * 2 + 1];
+            if ((M & B2F_META_SLOT_MASK) == s || (M & B2F_META_CAT)) continue; /* leaf, categorical test */
+            const uint32_t w = M >> B2F_META_FEAT_SHIFT;
+            if (w == B2F_SENTINEL_WORD) continue; /* "always second child" node */
+            if ((int)w < n_cat || (int)w >= n_cat + n_num) return "numeric test on a non-numeric row word";
+            float f;
+            memcpy(&f, &T, 4);
+            if (f != f) return "NaN split value";
+            thr[w - n_cat].push_back(f);
+        }
+    }
+    for (auto &v : thr) {
+        std::sort(v.begin(), v.end());
+        v.erase(std::unique(v.begin(), v.end()), v.end());
+    }
+    return nullptr;
+}
+
 /* rank tables (host_simd.cpp): lvl[j][i] = largest value of the i-th chunk at level j; +inf padding.  Upper levels fan out
  * 16 ways, the last one 16..64 ways, chosen as the shallowest / narrowest shape whose capacity exceeds the value count. */
 static void rank_tab_shape(size_t m, int *levels, int32_t fan[4]) {
@@ -214,26 +243,17 @@ static bool ranker_build(b2f_ranker *r, const uint8_t *blob, const b2f_blob_head
     if (depth < 1) depth = 1;
     r->depth = depth;
 
-    /* distinct split values per numeric feature */
-    r->thr.assign(r->n_num, {});
+    /* tested (categorical feature, category) pairs; distinct split values per numeric feature */
     r->pairs.clear();
     for (const Tree &t : trees)
         for (uint32_t s = 0; s < t.T.size(); ++s) {
-            if (is_leaf(t, s)) continue;
+            if (is_leaf(t, s) || !(t.M[s] & B2F_META_CAT)) continue;
             const uint32_t w = t.M[s] >> B2F_META_FEAT_SHIFT;
-            if (t.M[s] & B2F_META_CAT) {
-                if (t.T[s] == 0x7FFFFFFFu) continue; /* "never equal" */
-                if ((int)w >= r->n_cat || t.T[s] > 65533u) return fail("categorical test outside the schema");
-                r->pairs.push_back((w << 16) | t.T[s]);
-                continue;
-            }
-            if (w == B2F_SENTINEL_WORD) continue; /* "always second child" node */
-            if ((int)w < r->n_cat || (int)w >= r->n_cat + r->n_num) return fail("numeric test on a non-numeric row word");
-            float f;
-            memcpy(&f, &t.T[s], 4);
-            if (f != f) return fail("NaN split value");
-            r->thr[w - r->n_cat].push_back(f);
+            if (t.T[s] == 0x7FFFFFFFu) continue; /* "never equal" */
+            if ((int)w >= r->n_cat || t.T[s] > 65533u) return fail("categorical test outside the schema");
+            r->pairs.push_back((w << 16) | t.T[s]);
         }
+    if (const char *why = forest_split_values(blob, h, r->thr)) return fail(why);
     std::sort(r->pairs.begin(), r->pairs.end());
     r->pairs.erase(std::unique(r->pairs.begin(), r->pairs.end()), r->pairs.end());
     if (rank_onehot_base(r->n_num) + (int)r->pairs.size() > B2F_RANK_MAX_FEATS) return fail("more than 128 numeric features + tested categories");
@@ -241,9 +261,7 @@ static bool ranker_build(b2f_ranker *r, const uint8_t *blob, const b2f_blob_head
         if ((pr & 0xFFFFu) >= 64u) return fail("a tested category code does not fit the kernel's 64-bit per-feature mask");
     r->nan_rank.assign(r->n_num, 0);
     for (int k = 0; k < r->n_num; ++k) {
-        auto &v = r->thr[k];
-        std::sort(v.begin(), v.end());
-        v.erase(std::unique(v.begin(), v.end()), v.end()); /* float ==: -0.0 and +0.0 collapse, as the comparison sees them */
+        const auto &v = r->thr[k];
         if (v.size() > B2F_RANK_MAX_THRESHOLDS) return fail("more than 65534 distinct split values on one feature");
         const float imp = r->impute[r->n_cat + k];
         r->nan_rank[k] = (imp != imp) ? (uint16_t)v.size() : (uint16_t)(std::upper_bound(v.begin(), v.end(), imp) - v.begin());

@@ -21,6 +21,8 @@
  * Arithmetic: every point's payloads are added in tree order, from the GBDT init value (or 0), then aggregate() -- the
  * tile kernel's order -- so a point equals, bit for bit, k_forest_predict_tile on the row with the word replaced.  No
  * atomics; a row's outputs depend on nothing but the row, the forest and the grid.
+ *
+ * The mask walk is pd_mask_walk, which K7 (counterfactual.cuh) calls as well.
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -59,6 +61,95 @@ struct PdParams {
     uint32_t g_trees[B2F_MAX_GROUPS]; /* real trees of the group */
 };
 
+/* Stage this lane's row into xw[word][lane] (its warp's tile): decode, impute the numerics, sentinel above the fields
+ * (k_forest_predict_tile's staging).  A dead lane stages sentinels.  k_partial_dependence keeps its own inline copy of
+ * these lines: through this function its SASS would change (same work, another instruction schedule). */
+template <bool PACKED>
+__device__ __forceinline__ void pd_stage_row(const PdParams &p, const uint32_t *__restrict__ rows, long long row, bool live,
+                                             uint32_t (*xw)[32], int lane) {
+    uint32_t w[B2F_ROW_WORDS];
+#pragma unroll
+    for (int k = 0; k < B2F_ROW_WORDS; ++k) w[k] = B2F_SENTINEL_BITS;
+    if (live) {
+        if constexpr (PACKED) {
+            const uint4 *src = reinterpret_cast<const uint4 *>(rows + row * B2F_PACKED_ROW_WORDS);
+            uint32_t q[B2F_PACKED_ROW_WORDS];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const uint4 v = __ldg(src + k);
+                q[4 * k + 0] = v.x, q[4 * k + 1] = v.y, q[4 * k + 2] = v.z, q[4 * k + 3] = v.w;
+            }
+            const unsigned long long codes = (((unsigned long long)q[1]) << 32) | q[0];
+#pragma unroll
+            for (int k = 0; k < 9; ++k) w[k] = ((uint32_t)(codes >> (7 * k)) & 0x7fu) - 1u;
+#pragma unroll
+            for (int k = 0; k < 14; ++k) w[9 + k] = q[2 + k];
+        } else {
+            const uint4 *src = reinterpret_cast<const uint4 *>(rows + row * B2F_ROW_WORDS);
+#pragma unroll
+            for (int k = 0; k < 6; ++k) {
+                const uint4 v = __ldg(src + k);
+                w[4 * k + 0] = v.x, w[4 * k + 1] = v.y, w[4 * k + 2] = v.z, w[4 * k + 3] = v.w;
+            }
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < B2F_ROW_WORDS; ++k) {
+        uint32_t v = w[k];
+        if (k >= p.n_cat && k < p.n_cat + p.n_num && isnan(__uint_as_float(v))) v = __float_as_uint(p.impute[k]);
+        if (k >= (int)B2F_SENTINEL_WORD) v = B2F_SENTINEL_BITS;
+        xw[k][lane] = v;
+    }
+}
+
+/* The mask walk: acc[k] += every leaf payload that point k of a segment reaches, tree by tree in tree order.  One walk per
+ * (row, tree) forks only at splits on row word `word`, with gv[k] (shared) the word point k puts there and `full` the mask
+ * of the segment's points; xw = the warp's staged rows; stk = the block's walk stacks, column threadIdx.x this thread's. */
+__device__ __forceinline__ void pd_mask_walk(const PdParams &p, uint32_t word, uint32_t full, const uint32_t *gv, const uint32_t (*xw)[32],
+                                             int lane, unsigned long long (*stk)[B2F_PD_WARPS * 32], double (&acc)[B2F_PD_SEG]) {
+    for (int g = 0; g < p.n_groups; ++g) {
+        const uint8_t *chunk = p.chunks + p.g_off[g];
+        const size_t leaf_area = (size_t)p.g_slots[g] * B2F_NODE_STRIDE;
+        const int n_trees = (int)p.g_trees[g];
+        for (int l = 0; l < n_trees; ++l) { /* tree 32 g + l: tree order */
+            const uint8_t *nodes = chunk + l * 8;
+            uint32_t node = 0, mask = full;
+            int sp = 0;
+            while (true) {
+                const uint2 tm = __ldg(reinterpret_cast<const uint2 *>(nodes + (size_t)node * B2F_NODE_STRIDE));
+                const uint32_t first = tm.y & B2F_META_SLOT_MASK;
+                if (first == node) { /* a leaf is the only node that is its own first child */
+                    const double v = __ldg(reinterpret_cast<const double *>(nodes + leaf_area + (size_t)tm.x * B2F_NODE_STRIDE));
+#pragma unroll
+                    for (int k = 0; k < B2F_PD_SEG; ++k)
+                        if ((mask >> k) & 1u) acc[k] += v;
+                    if (sp == 0) break;
+                    const unsigned long long e = stk[--sp][threadIdx.x];
+                    node = (uint32_t)e;
+                    mask = (uint32_t)(e >> 32);
+                    continue;
+                }
+                const uint32_t feat = tm.y >> B2F_META_FEAT_SHIFT;
+                if (feat == word) {
+                    uint32_t sec = 0;
+#pragma unroll
+                    for (int k = 0; k < B2F_PD_SEG; ++k) sec |= (take_second(gv[k], tm.x, tm.y) ? 1u : 0u) << k;
+                    const uint32_t m2 = mask & sec, m1 = mask & ~sec;
+                    if (m1 && m2) { /* fork: the second child waits on the stack */
+                        stk[sp++][threadIdx.x] = ((unsigned long long)m2 << 32) | (first + 1u);
+                        node = first;
+                        mask = m1;
+                    } else {
+                        node = first + (m2 ? 1u : 0u);
+                    }
+                } else {
+                    node = first + (take_second(xw[feat][lane], tm.x, tm.y) ? 1u : 0u);
+                }
+            }
+        }
+    }
+}
+
 template <bool PACKED>
 __global__ void __launch_bounds__(B2F_PD_WARPS * 32)
     k_partial_dependence(const __grid_constant__ PdParams p, const uint32_t *__restrict__ rows, long long n, double *__restrict__ out) {
@@ -71,7 +162,6 @@ __global__ void __launch_bounds__(B2F_PD_WARPS * 32)
     if (threadIdx.x < B2F_PD_SEG) gv[threadIdx.x] = threadIdx.x < sg.count ? p.grid[sg.off + threadIdx.x] : 0u;
     const long long row = ((long long)blockIdx.x * B2F_PD_WARPS + warp) * 32 + lane;
     const bool live = row < n;
-
     /* stage this lane's row: decode, impute, sentinel above the fields (k_forest_predict_tile's staging) */
     {
         uint32_t w[B2F_ROW_WORDS];
@@ -115,48 +205,7 @@ __global__ void __launch_bounds__(B2F_PD_WARPS * 32)
     double acc[B2F_PD_SEG];
 #pragma unroll
     for (int k = 0; k < B2F_PD_SEG; ++k) acc[k] = p.agg_mode == B2F_AGG_GBDT_LOGISTIC ? p.init_raw : 0.0;
-
-    for (int g = 0; g < p.n_groups; ++g) {
-        const uint8_t *chunk = p.chunks + p.g_off[g];
-        const size_t leaf_area = (size_t)p.g_slots[g] * B2F_NODE_STRIDE;
-        const int n_trees = (int)p.g_trees[g];
-        for (int l = 0; l < n_trees; ++l) { /* tree 32 g + l: tree order */
-            const uint8_t *nodes = chunk + l * 8;
-            uint32_t node = 0, mask = full;
-            int sp = 0;
-            while (true) {
-                const uint2 tm = __ldg(reinterpret_cast<const uint2 *>(nodes + (size_t)node * B2F_NODE_STRIDE));
-                const uint32_t first = tm.y & B2F_META_SLOT_MASK;
-                if (first == node) { /* a leaf is the only node that is its own first child */
-                    const double v = __ldg(reinterpret_cast<const double *>(nodes + leaf_area + (size_t)tm.x * B2F_NODE_STRIDE));
-#pragma unroll
-                    for (int k = 0; k < B2F_PD_SEG; ++k)
-                        if ((mask >> k) & 1u) acc[k] += v;
-                    if (sp == 0) break;
-                    const unsigned long long e = stk[--sp][threadIdx.x];
-                    node = (uint32_t)e;
-                    mask = (uint32_t)(e >> 32);
-                    continue;
-                }
-                const uint32_t feat = tm.y >> B2F_META_FEAT_SHIFT;
-                if (feat == sg.word) {
-                    uint32_t sec = 0;
-#pragma unroll
-                    for (int k = 0; k < B2F_PD_SEG; ++k) sec |= (take_second(gv[k], tm.x, tm.y) ? 1u : 0u) << k;
-                    const uint32_t m2 = mask & sec, m1 = mask & ~sec;
-                    if (m1 && m2) { /* fork: the second child waits on the stack */
-                        stk[sp++][threadIdx.x] = ((unsigned long long)m2 << 32) | (first + 1u);
-                        node = first;
-                        mask = m1;
-                    } else {
-                        node = first + (m2 ? 1u : 0u);
-                    }
-                } else {
-                    node = first + (take_second(xs[warp][feat][lane], tm.x, tm.y) ? 1u : 0u);
-                }
-            }
-        }
-    }
+    pd_mask_walk(p, sg.word, full, gv, xs[warp], lane, stk, acc);
 
     double *o = out + row * (long long)p.points + sg.off;
 #pragma unroll

@@ -260,6 +260,28 @@ class ForestEngine:
         check(self._lib.b2f_partial_dependence_device(self._h, rows_dev, n, fmt, ptr(pr), len(pr), ptr(grid), out_dev),
               "b2f_partial_dependence_device")
 
+    # ------------------------------------------------------------------ counterfactuals (csrc/counterfactual.cuh)
+    def counterfactual_rows(self, rows: np.ndarray, words, cutoff: float = 0.5, device_ms: bool = False):
+        """Encoded rows (N, 24) or packed (N, 16) and numeric row words -> (proba float64 (N,), records (N, len(words)) of
+        ``COUNTERFACTUAL_DTYPE``[, device ms]): per row and word, the nearest float32 values below and above the row's value
+        whose decision ``p1 > cutoff`` differs from the row's, with p1 there (NaN: none on that side)."""
+        rows = np.ascontiguousarray(rows)
+        w = np.ascontiguousarray(words, dtype=np.int32)
+        n = rows.shape[0]
+        proba = np.empty(n, dtype=np.float64)
+        out = np.empty((n, len(w)), dtype=_cabi.COUNTERFACTUAL_DTYPE)
+        ms = C.c_float(0.0)
+        check(self._lib.b2f_counterfactual(self._h, ptr(rows), n, self._fmt(rows), ptr(w), len(w), float(cutoff), ptr(proba), ptr(out),
+                                           C.byref(ms)), "b2f_counterfactual")
+        return (proba, out, ms.value) if device_ms else (proba, out)
+
+    def counterfactual_device(self, rows_dev: int, n: int, words, cutoff: float, proba_dev: int, out_dev: int, fmt: int = ROWS_WORDS24) -> None:
+        """Enqueue the counterfactuals of device-resident rows into device proba (n doubles; 0: not written) and out (n x
+        len(words) records); ``sync`` waits."""
+        w = np.ascontiguousarray(words, dtype=np.int32)
+        check(self._lib.b2f_counterfactual_device(self._h, rows_dev, n, fmt, ptr(w), len(w), float(cutoff), proba_dev, out_dev),
+              "b2f_counterfactual_device")
+
     # ------------------------------------------------------------------ device-resident interface
     def device_alloc(self, nbytes: int) -> int:
         p = self._lib.b2f_device_alloc(self._h, nbytes)
@@ -448,6 +470,18 @@ def _row_format(rows: np.ndarray, rank_words: int = 0) -> int:
         if rank_words and rows.shape[1] == rank_words:
             return ROWS_RANKED
     raise ValueError(f"rows must be uint32 (N, {ROW_WORDS}), packed (N, {PACKED_ROW_WORDS})" + (f" or ranked (N, {rank_words})" if rank_words else ""))
+
+
+def blob_split_values(blob: bytes, word: int) -> np.ndarray:
+    """The sorted distinct float32 split values of numeric row word ``word`` over a forest blob (``b2f_blob_split_values``;
+    needs no GPU)."""
+    lib = _cabi.load_library()
+    buf = np.frombuffer(blob, dtype=np.uint8)
+    n = lib.b2f_blob_split_values(ptr(buf), buf.size, int(word), None, 0)
+    check(min(int(n), 0), "b2f_blob_split_values")
+    out = np.empty(int(n), dtype=np.float32)
+    check(min(int(lib.b2f_blob_split_values(ptr(buf), buf.size, int(word), ptr(out), out.size)), 0), "b2f_blob_split_values")
+    return out
 
 
 def _probe_table(probes) -> np.ndarray:

@@ -358,6 +358,77 @@ class B200Model:
         res.update(dependence.split_output(out, [len(g) for g in grids], kind))
         return res
 
+    def counterfactuals(self, model_input, features=None, *, cutoff: float = 0.5) -> dict:
+        """What would change the decision: per applicant and request field, the nearest value of that field alone at which
+        the decision ``P(class 1) > cutoff`` differs from the applicant's own.
+
+        -> ``{"feature_names", "output": "probability", "cutoff", "predictions": float64 (n,), "decisions": bool (n,),
+        "counterfactuals": [one dict per field, in order]}``.  A numeric field's dict holds float64 (n,) arrays ``value`` (the
+        value as scored: a missing value is the training median), ``lower`` / ``upper`` (the largest float32 below / smallest
+        above ``value`` whose decision differs; NaN when no value on that side does) and ``lower_prediction`` /
+        ``upper_prediction`` (P(class 1) there, bit for bit the tile kernel's score of the row with the field set to that
+        value).  These are exact float32 boundaries: sent back as request values they reproduce the flip, and the float32
+        one step toward ``value`` keeps the decision.  A categorical field has no order: its dict holds ``value`` (the
+        category, None when missing or unknown) and ``flips``, per row the list of ``(category, P(class 1))`` of the
+        vocabulary categories, in code order, whose decision differs.  At cutoff 0.5 the decision is the model's label except
+        where P(class 1) rounds to exactly 0.5.  ``features=None`` probes every field; unknown or repeated names raise
+        ValueError, as does a cutoff outside [0, 1].  Every model has it, with or without an explainer; rows with NaN
+        numerics are accepted.  It runs on the first GPU's handle only, like ``partial_dependence``."""
+        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
+        if len(df.columns) == 0:
+            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        features = list(self.all_features) if features is None else ([features] if isinstance(features, str) else list(features))
+        if not features:
+            raise ValueError("at least one feature is needed")
+        unknown = [f for f in features if f not in self.all_features]
+        if unknown:
+            raise ValueError(f"unknown feature(s) {unknown}; expected names from {list(self.all_features)}")
+        if len(set(features)) != len(features):
+            raise ValueError(f"repeated feature(s) {sorted({f for f in features if features.count(f) > 1})}")
+        if isinstance(cutoff, bool) or not isinstance(cutoff, (int, float, np.integer, np.floating)) or not 0.0 <= float(cutoff) <= 1.0:
+            raise ValueError(f"cutoff={cutoff!r}: expected a number in [0, 1]")
+        cutoff = float(cutoff)
+        rows = self.encoder.encode_frame(df)
+        n = rows.shape[0]
+        cats = [f for f in features if f in self.categorical_features]
+        nums = [f for f in features if f not in self.categorical_features]
+        proba, rec = None, None
+        if nums:
+            proba, rec = self.engine.counterfactual_rows(rows, [dependence.word_of(self.encoder, f) for f in nums], cutoff)
+        # categoricals: K6 ICE points over the whole vocabulary, at most 256 points per probe; without a numeric field the
+        # predictions are the ICE point at each row's own code (-1 added to the first field's grid for unknown categories)
+        probes, words, spans = [], [], {}
+        for f in cats:
+            word, vocab = dependence.word_of(self.encoder, f), len(self.flat.categories[self.categorical_features.index(f)])
+            codes = list(range(-1 if (proba is None and not probes) else 0, vocab))
+            spans[f] = (len(words), codes)
+            for lo in range(0, len(codes), dependence.MAX_POINTS):
+                probes.append((word, len(words) + lo, min(dependence.MAX_POINTS, len(codes) - lo)))
+            words.extend(codes)
+        ice = self.engine.partial_dependence_rows(rows, probes, np.asarray(words, dtype=np.int32).view(np.uint32)) if probes else None
+        if proba is None:
+            f0 = cats[0]
+            own = rows[:, dependence.word_of(self.encoder, f0)].view(np.int32).astype(np.int64)
+            proba = ice[np.arange(n), spans[f0][0] + own + 1] if n else np.empty(0, dtype=np.float64)
+        decisions = proba > cutoff
+        out, k = [], 0
+        for f in features:
+            if f in spans:
+                start, codes = spans[f]
+                vocab = self.flat.categories[self.categorical_features.index(f)]
+                own = rows[:, dependence.word_of(self.encoder, f)].view(np.int32)
+                first = start + (1 if codes[0] == -1 else 0)
+                curve = ice[:, first:start + len(codes)]
+                flips = [[(vocab[c], float(curve[i, c])) for c in np.flatnonzero((curve[i] > cutoff) != decisions[i])] for i in range(n)]
+                out.append({"value": [vocab[c] if c >= 0 else None for c in own.tolist()], "flips": flips})
+            else:
+                r = rec[:, k]
+                k += 1
+                out.append({"value": r["value"].astype(np.float64), "lower": r["lower"].astype(np.float64), "lower_prediction": r["lower_p1"].copy(),
+                            "upper": r["upper"].astype(np.float64), "upper_prediction": r["upper_p1"].copy()})
+        return {"feature_names": features, "output": "probability", "cutoff": cutoff, "predictions": proba, "decisions": decisions,
+                "counterfactuals": out}
+
     def explain_interventional(self, model_input) -> dict:
         """Exact interventional TreeSHAP contributions of every request field against the attached background set (what
         shap's ``TreeExplainer(model, data)`` computes): the mean, over background rows z, of each field's Shapley value in

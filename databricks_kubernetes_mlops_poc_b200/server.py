@@ -219,6 +219,39 @@ _DEPENDENCE_PARAMETERS = [
 ]
 
 
+_COUNTERFACTUAL_PARAMETERS = [
+    {"name": "feature", "in": "query", "required": False,
+     "description": "request field to probe; repeat for several, each at most once; none = every field",
+     "schema": {"type": "array", "items": {"type": "string"}}, "style": "form", "explode": True},
+    {"name": "cutoff", "in": "query", "required": False, "description": "the decision is P(class 1) > cutoff",
+     "schema": {"type": "number", "minimum": 0, "maximum": 1, "default": 0.5}},
+]
+
+
+def _counterfactual_problem(features, cutoff: str) -> str | None:
+    """Why a /explain/counterfactual query is unprocessable, or None."""
+    unknown = [f for f in features if f not in ALL_FEATURES]
+    if unknown:
+        return f"unknown feature(s) {unknown}"
+    if len(set(features)) != len(features):
+        return f"repeated feature(s) {sorted({f for f in features if features.count(f) > 1})}"
+    try:
+        c = float(cutoff)
+    except ValueError:
+        c = float("nan")
+    if not 0.0 <= c <= 1.0:
+        return "cutoff must be a number in [0, 1]"
+    return None
+
+
+def _counterfactual_json(name: str, cf: dict) -> dict:
+    """One field's counterfactuals for JSON: NaN (none) -> null."""
+    if "flips" in cf:
+        return {"feature": name, "value": cf["value"], "flips": [[[c, p] for c, p in row] for row in cf["flips"]]}
+    return {"feature": name, **{k: [None if v != v else v for v in np.asarray(cf[k], dtype=np.float64).tolist()]
+                                for k in ("value", "lower", "lower_prediction", "upper", "upper_prediction")}}
+
+
 def _dependence_problem(features, values, kind, grid_resolution) -> str | None:
     """Why a /explain/dependence query is unprocessable, or None."""
     if not features:
@@ -379,6 +412,35 @@ def create_app(model=None, loader=None) -> FastAPI:
         for key in ("average", "individual"):
             if key in out:
                 body[key] = [np.asarray(a, dtype=np.float64).tolist() for a in out[key]]
+        return Response(content=json.dumps(body, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
+
+    @app.post("/explain/counterfactual", openapi_extra={"requestBody": _REQUEST_SCHEMA, "parameters": _COUNTERFACTUAL_PARAMETERS})
+    async def explain_counterfactual(request: Request):
+        """What would change the decision: for each applicant and probed field (every field without a `feature` parameter),
+        the nearest value of that field alone at which the decision P(class 1) > cutoff flips.  A numeric field answers the
+        largest value below (`lower`) and the smallest above (`upper`) the applicant's `value` that flip it, exact float32
+        boundaries, with the probability there; null when no value on that side flips it.  A categorical field answers the
+        categories that flip it (`flips`: [category, probability] pairs).  422 for an unknown or repeated field or a cutoff
+        that is not a number in [0, 1]."""
+        q = request.query_params
+        features, cutoff = q.getlist("feature"), q.get("cutoff", "0.5")
+        problem = _counterfactual_problem(features, cutoff)
+        if problem:
+            return _unprocessable(problem)
+        input_df = parser.frame(await request.body())
+        if len(input_df) == 0:
+            raise KeyError(f"None of {ALL_FEATURES} are in the [columns]")
+        m = ml_models["credit_default"]
+        batcher = ml_models["_batcher"]
+
+        def run():
+            with batcher.locks[0]:  # the first GPU's handle, which batcher worker 0 drives
+                return m.counterfactuals(input_df, features or None, cutoff=float(cutoff))
+
+        out = await asyncio.get_running_loop().run_in_executor(None, run)
+        body = {"feature_names": list(out["feature_names"]), "output": out["output"], "cutoff": out["cutoff"],
+                "predictions": np.asarray(out["predictions"], dtype=np.float64).tolist(), "decisions": np.asarray(out["decisions"]).tolist(),
+                "counterfactuals": [_counterfactual_json(f, cf) for f, cf in zip(out["feature_names"], out["counterfactuals"])]}
         return Response(content=json.dumps(body, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
 
     @app.post("/predict", response_model=ModelOutput, openapi_extra={"requestBody": _REQUEST_SCHEMA})

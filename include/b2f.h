@@ -149,6 +149,10 @@ int b2f_device_count(void); /* number of CUDA devices, or B2F_ENODEV */
 /* structural check of a forest blob (header, group table, every node word keeps the walk in bounds);
  * needs no GPU.  b2f_model_create() runs the same check. */
 int b2f_blob_validate(const void *forest_blob, size_t nbytes);
+/* the sorted distinct float32 split values t' = nextup(floor32(threshold)) of numeric row word `word` over the whole forest,
+ * at any depth (-0.0 and +0.0 count once): min(count, cap) of them into out; returns the count, or B2F_EINVAL for a
+ * malformed blob, a word outside the numerics or a NaN split value.  Needs no GPU. */
+int64_t b2f_blob_split_values(const void *forest_blob, size_t nbytes, int word, float *out, int64_t cap);
 b2f_model *b2f_model_create(const void *forest_blob, size_t nbytes, int device); /* NULL on error */
 void b2f_model_destroy(b2f_model *m);
 int b2f_model_info(const b2f_model *m, b2f_info *out);
@@ -378,6 +382,37 @@ int b2f_partial_dependence(b2f_model *m, const void *rows, int64_t n, int row_fo
  * compute stream (asynchronous, like b2f_explain_device; b2f_sync waits) */
 int b2f_partial_dependence_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const b2f_pd_probe *probes, int n_probes,
                                   const uint32_t *grid_words, double *out_dev);
+
+/* ---- nearest single-field counterfactuals (csrc/counterfactual.cuh) ----
+ * "What is the smallest change to this one field that changes the decision?"  For row i and probed numeric row word w with
+ * the forest's split values t'_0 < ... < t'_{m-1} (b2f_blob_split_values), every float32 value of a piece [t'_{k-1}, t'_k)
+ * scores the same; the row's own piece is j = #{t' <= x}, x the value as scored (NaN: the training median).  The decision
+ * is p1 > cutoff, p1 the tile-order probability b2f_partial_dependence returns (at cutoff 0.5 this is the model's label,
+ * except where p1 rounds to exactly 0.5).  out[i * n_words + f] holds `value` = x, `upper` = t'_{k-1} for the least k > j
+ * whose decision differs from the row's (the smallest float32 above x that flips it), `lower` = nextdown(t'_k) for the
+ * greatest such k < j (the largest float32 below x that flips it), and the p1 there; NaN on a side with no flip.  Each
+ * returned p1 equals, bit for bit, the tile kernel's score of the row with the word set to the returned value, and the
+ * float32 one step toward x keeps the row's decision.  proba (may be NULL): the row's own p1, from the same sums.
+ * words: 1..23 numeric row words (a categorical field has no order: score its vocabulary with b2f_partial_dependence).
+ * Rows are independent of the batch and results bit-identical from run to run.  Errors: B2F_EINVAL for ranked rows, n < 0,
+ * a NULL out with n > 0, n_words outside 1..23, a word outside the numerics, a cutoff that is not a number in [0, 1], or a
+ * forest deeper than 32 levels.  The split-value table goes to the device on a model's first call.  Pipelined over the
+ * model's streams like b2f_explain, in chunks of at most 64 MB of per-segment candidates; device_ms as b2f_explain.
+ * (The record's tag is not a typedef: b2f_counterfactual is also the function's name, as with POSIX `struct stat`.) */
+struct b2f_counterfactual {
+    double lower_p1; /* p1 at `lower` (NaN: none) */
+    double upper_p1; /* p1 at `upper` (NaN: none) */
+    float lower;
+    float upper;
+    float value;
+    int32_t reserved;
+};
+int b2f_counterfactual(b2f_model *m, const void *rows, int64_t n, int row_format, const int32_t *words, int n_words, double cutoff,
+                       double *proba, struct b2f_counterfactual *out, float *device_ms);
+/* device-resident form: rows_dev, proba_dev (may be NULL) and out_dev in device memory, words in host memory; enqueued on
+ * the compute stream (asynchronous, like b2f_partial_dependence_device; b2f_sync waits) */
+int b2f_counterfactual_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const int32_t *words, int n_words,
+                              double cutoff, double *proba_dev, struct b2f_counterfactual *out_dev);
 
 /* asynchronous form for the request-batching ring: buffers must be pinned and stay valid until
  * b2f_wait(ticket) returns.  proba_is_f64 selects double (1) or float (0) outputs. */
