@@ -19,15 +19,17 @@ when a reference table is supplied; without one every score is 0.0.
 
 from __future__ import annotations
 
+import contextlib
 import os
 import threading
+import time
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import pandas as pd
 
 from . import dependence
-from ._cabi import OUT_F64, OUT_FULL
+from ._cabi import OUT_F64, OUT_FULL, ROWS_PACKED64, ROWS_WORDS24
 from ._pylists import ListBuilder
 from .encode import RowEncoder
 from .engine import EngineGroup, ForestEngine
@@ -43,7 +45,7 @@ SKLEARN_PICKLE = os.path.join("artifacts", "classifier", "model", "model.pkl")  
 
 
 class B200Model:
-    def __init__(self, flat: FlatForest, devices=None, drift=None, proba_dtype=np.float64, outlier_blob: bytes | None = None, host_threads: int = 0,
+    def __init__(self, flat: FlatForest, devices=None, drift=None, outlier_blob: bytes | None = None, host_threads: int = 0,
                  explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None):
         self.flat = flat
         self.all_features = flat.all_features
@@ -58,7 +60,6 @@ class B200Model:
             self.group = EngineGroup(flat, devices)
             self.engine = self.group.engines[0]
         self.drift = drift
-        self.proba_dtype = np.dtype(proba_dtype)
         self.classes = np.asarray(flat.classes)
         self._pool = ThreadPoolExecutor(max_workers=2, thread_name_prefix="b200-drift") if drift is not None else None
         self.outlier_blob = outlier_blob
@@ -68,21 +69,17 @@ class B200Model:
         self.explain_blob = explain_blob
         if explain_blob is not None:
             self.engine.attach_explainer(explain_blob)
+        # encoder threads of each GPU's request pipeline (csrc/scorer.h); 0: the library's default for the GPU
+        self.host_threads = int(host_threads or os.environ.get("B200_HOST_THREADS", 0))
+        # one scoring replica per GPU: the only code that scores on that GPU's handle (predict, the server's round-robin
+        # batcher, explain); the forest is replicated, rows are independent
+        engines = self.group.engines if self.group is not None else [self.engine]
+        self.replicas = [_Replica(self.encoder, e, outlier_blob is not None, self.numeric_features, self.host_threads) for e in engines]
         self.background_rows = 0
         self.background = None  # the attached background frame (raw columns)
         self.dependence_grids = None  # field -> default partial-dependence grid of the background (attach_background)
         if explain_background is not None:
             self.attach_background(explain_background)
-        # one scoring replica per GPU for the server's round-robin batcher (each has its own handle,
-        # pinned staging and worker thread; the forest is replicated, rows are independent)
-        engines = self.group.engines if self.group is not None else [self.engine]
-        self.replicas = [_Replica(self.encoder, e, outlier_blob is not None, self.numeric_features) for e in engines]
-        # the columnar request pipeline of the first GPU (csrc/scorer.h): created on first use
-        self._scorer = None
-        self._scorer_lock = threading.Lock()
-        self.host_threads = int(os.environ.get("B200_HOST_THREADS", host_threads or 0))  # 0: half the CPUs of the GPU's NUMA node
-        self._scorer_failed = os.environ.get("B200_SCORER", "1") == "0"
-        self.last_timing = None  # seconds spent in the stages of the last large predict(): columns / first chunk / lists
 
     # ------------------------------------------------------------------ construction
     @classmethod
@@ -119,9 +116,6 @@ class B200Model:
             if r._scorer is not None:
                 r._scorer.close()
                 r._scorer = None
-        if self._scorer is not None:
-            self._scorer.close()
-            self._scorer = None
         if self._pool is not None:
             self._pool.shutdown(wait=True)
         if self.drift is not None:
@@ -132,94 +126,29 @@ class B200Model:
             self.engine.close()
 
     # ------------------------------------------------------------------ scoring
-    def _score(self, df: pd.DataFrame, want_outliers: bool = False):
-        """-> (proba1, label, is_outlier or None); one H2D copy of the encoded rows whichever outputs are wanted."""
-        n = len(df)
-        # large requests travel as 64-byte packed rows (one third fewer PCIe bytes), encoded natively in one pass
-        packed = self.encoder.packed_ok and n > self.encoder.SMALL_BATCH
-        rows, proba, label = self.engine.staging(n, packed=packed)
-        if packed:
-            self.encoder.encode_frame_packed(df, out=rows)
-        else:
-            self.encoder.encode_frame(df, out=rows)
-        target = self.group if self.group is not None else self.engine
-        if want_outliers and self.outlier_blob is not None:
-            _reject_nan(df, self.numeric_features)
-            rec = target.predict_full(rows, out=self.engine.staging_full(n))
-            return rec["proba1"], rec["label"], rec["is_outlier"]
-        if self.proba_dtype != np.float64:
-            proba = proba.view(np.float32)[:n]
-        target.predict_rows(rows, proba_dtype=self.proba_dtype, out_proba=proba, out_label=label)
-        return proba, label, None
+    @property
+    def last_timing(self) -> dict | None:
+        """Seconds spent in the stages of the last job on the first GPU's request pipeline: columns / first chunk / chunks."""
+        return self.replicas[0].last_timing
+
+    def _staged(self, df: pd.DataFrame, full: bool = False):
+        """The general path, copied out of the first GPU's pinned staging -> (proba1, label, is_outlier or None).  On several
+        GPUs it is one group call (``b2f_predict_multi``) that slices the rows over every GPU, so it holds every replica's lock,
+        taken in index order: a batcher worker holds one lock and ``explain`` the first, so neither can deadlock against it."""
+        with contextlib.ExitStack() as held:
+            for r in self.replicas if self.group is not None else self.replicas[:1]:
+                held.enter_context(r.lock)
+            return tuple(None if a is None else np.array(a) for a in self.replicas[0]._staged(df, full, self.group))
 
     def predict_proba1(self, df: pd.DataFrame) -> np.ndarray:
         """``classifier.predict_proba(df[all_features])[:, 1]`` (02-register-model.ipynb:335-337)."""
-        return np.array(self._score(df)[0], dtype=np.float64)
+        if self.group is None:
+            return self.replicas[0].score(df, want_outliers=False)[0]
+        return self._staged(df)[0]
 
     def predict_label(self, df: pd.DataFrame) -> np.ndarray:
         """``pipeline.predict(df)`` (hard labels, 01-train-model.ipynb:290)."""
-        return self.classes[np.array(self._score(df)[1])]
-
-    PIPELINE_MIN_ROWS = int(os.environ.get("B200_PIPELINE_MIN_ROWS", "1"))  # from here up a request goes through the columnar pipeline
-
-    def _pipeline(self, df: pd.DataFrame):
-        """Large requests on one GPU: the DataFrame's column buffers go to the native scorer in ONE call; chunks come back while
-        later chunks are still being encoded / copied / scored, and each chunk's Python floats are built as it lands.
-        -> (predictions list, outlier-flag list or None), or None when this request has to take the general path."""
-        if self._scorer_failed or self.group is not None or len(df) < self.PIPELINE_MIN_ROWS:
-            return None
-        import time
-
-        t0 = time.perf_counter()
-        if self._scorer is None:
-            try:
-                self._scorer = self.engine.scorer(self.encoder, self.host_threads)
-            except Exception:
-                self._scorer_failed = True
-                return None
-        cols = self.encoder.frame_columns(df)
-        if cols is None:
-            return None
-        sc = self._scorer
-        n = len(df)
-        full = self.outlier_blob is not None
-        with self._scorer_lock:  # one job at a time per scorer: concurrent predict() calls on one model take turns
-            return self._pipeline_locked(sc, df, n, full, cols, t0)
-
-    def _pipeline_locked(self, sc, df, n, full, cols, t0):
-        import time
-
-        if full:
-            _reject_nan(df, self.numeric_features)
-        t1 = time.perf_counter()
-        # classifier only: the scorer's own choice (64-byte float32 rows: cheapest to encode; ranked rows with B200_SCORER_ROWS=ranked);
-        # with the outlier forest on the same rows: float32 rows (ranks are relative to ONE forest's split values)
-        n_chunks = sc.start(n, cols, out_mode=OUT_FULL if full else OUT_F64, fmt=(1 if self.encoder.packed_ok else 0) if full else None)
-        out = sc.results()
-        bounds = sc.bounds
-        # Python lists are built chunk by chunk while later chunks are in flight (float objects recycled: _pylists.py); what does
-        # not depend on the results -- the empty lists, the all-zero outlier list of a classifier-only model -- is made while
-        # the first chunk is on its way
-        preds = ListBuilder(n)
-        flags = ListBuilder(n) if full else None
-        zeros = None if full else [0] * n
-        t_first = None
-        for c in range(n_chunks):
-            sc.wait(c)
-            if t_first is None:
-                t_first = time.perf_counter()
-            lo = bounds[c]
-            part = out[lo:bounds[c + 1]]
-            if full:
-                preds.fill(lo, part["proba1"])
-                flags.fill(lo, part["is_outlier"])
-            else:
-                preds.fill(lo, part)
-        preds, flags = preds.items, (flags.items if full else zeros)
-        t2 = time.perf_counter()
-        self.last_timing = {"columns_s": t1 - t0, "first_chunk_s": (t_first or t2) - t1, "chunks_and_lists_s": t2 - t1, "chunks": n_chunks,
-                            "threads": sc.threads, "row_format": sc.last_fmt}
-        return preds, flags
+        return self.classes[self._staged(df)[1]]
 
     def predict(self, model_input) -> dict:
         """Mirror of ``CustomModel.predict(context, model_input)`` (02-register-model.ipynb:330-353)."""
@@ -243,13 +172,24 @@ class B200Model:
 
     def _predictions(self, df: pd.DataFrame):
         """-> (predictions list, outlier-flag list): what ``predict`` returns for these rows, without the drift scores."""
-        n = len(df)
-        fast = self._pipeline(df)
-        if fast is not None:
-            preds, flags = fast
-            return preds, flags if flags is not None else [0] * n
-        proba, _, fl = self._score(df, want_outliers=True)
-        return proba.tolist(), fl.tolist() if fl is not None else [0] * n
+        n, full = len(df), self.outlier_blob is not None
+        if self.group is not None:
+            proba, _, flags = self._staged(df, full)
+            return proba.tolist(), flags.tolist() if full else [0] * n
+        # one GPU: each chunk's Python floats are built as it lands, while later chunks are still being encoded / copied /
+        # scored (float objects recycled: _pylists.py)
+        chunks = self.replicas[0]._chunks(df, full)
+        next(chunks)
+        # the job is in flight: what does not depend on its results -- the empty lists, the all-zero outlier list of a
+        # classifier-only model -- is made while the first chunk is on its way
+        preds = ListBuilder(n)
+        flags = ListBuilder(n) if full else None
+        zeros = None if full else [0] * n
+        for lo, proba, outlier in chunks:
+            preds.fill(lo, proba)
+            if full:
+                flags.fill(lo, outlier)
+        return preds.items, flags.items if full else zeros
 
     # ------------------------------------------------------------------ explanations
     @property
@@ -275,8 +215,7 @@ class B200Model:
         with the classifier alone.  So a row with a NaN numeric is explained even when an outlier forest is attached (the
         outlier detector, not the classifier, refuses NaN in ``predict``).  On one GPU the predictions are the numbers
         ``predict`` returns; a multi-GPU ``predict`` slices the batch over all GPUs and may differ from them in the last bits.
-        Calls on one handle must not overlap: a caller that also scores on ``replicas[0]`` from other threads serialises the
-        two (the HTTP server takes the first batcher worker's lock)."""
+        It holds ``replicas[0].lock`` across both calls, so it may run beside ``predict`` and the HTTP batcher's workers."""
         return self._explained(model_input, "explain_rows", "contributions")
 
     def explain_interactions(self, model_input) -> dict:
@@ -300,7 +239,9 @@ class B200Model:
         explainer."""
         if self.explain_blob is None:
             raise RuntimeError("a background needs an explainer: build the model with from_pipeline(..., explain=True)")
-        nbytes = self.engine.attach_background(self.encoder.encode_frame(frame))
+        rows = self.encoder.encode_frame(frame)
+        with self.replicas[0].lock:
+            nbytes = self.engine.attach_background(rows)
         self.background_rows = len(frame)
         self.background = frame
         self.dependence_grids = self._default_grids(frame, dependence.DEFAULT_RESOLUTION, dependence.DEFAULT_PERCENTILES)
@@ -353,7 +294,9 @@ class B200Model:
             words.append(dependence.encode_grid(self.encoder, name, grid))
             probes.append((dependence.word_of(self.encoder, name), off, len(grid)))
             off += len(grid)
-        out = self.engine.partial_dependence_rows(self.encoder.encode_frame(df), probes, np.concatenate(words))
+        rows = self.encoder.encode_frame(df)
+        with self.replicas[0].lock:
+            out = self.engine.partial_dependence_rows(rows, probes, np.concatenate(words))
         res = {"feature_names": features, "output": "probability", "grid_values": grids}
         res.update(dependence.split_output(out, [len(g) for g in grids], kind))
         return res
@@ -394,7 +337,8 @@ class B200Model:
         nums = [f for f in features if f not in self.categorical_features]
         proba, rec = None, None
         if nums:
-            proba, rec = self.engine.counterfactual_rows(rows, [dependence.word_of(self.encoder, f) for f in nums], cutoff)
+            with self.replicas[0].lock:
+                proba, rec = self.engine.counterfactual_rows(rows, [dependence.word_of(self.encoder, f) for f in nums], cutoff)
         # categoricals: K6 ICE points over the whole vocabulary, at most 256 points per probe; without a numeric field the
         # predictions are the ICE point at each row's own code (-1 added to the first field's grid for unknown categories)
         probes, words, spans = [], [], {}
@@ -405,7 +349,10 @@ class B200Model:
             for lo in range(0, len(codes), dependence.MAX_POINTS):
                 probes.append((word, len(words) + lo, min(dependence.MAX_POINTS, len(codes) - lo)))
             words.extend(codes)
-        ice = self.engine.partial_dependence_rows(rows, probes, np.asarray(words, dtype=np.int32).view(np.uint32)) if probes else None
+        ice = None
+        if probes:
+            with self.replicas[0].lock:
+                ice = self.engine.partial_dependence_rows(rows, probes, np.asarray(words, dtype=np.int32).view(np.uint32))
         if proba is None:
             f0 = cats[0]
             own = rows[:, dependence.word_of(self.encoder, f0)].view(np.int32).astype(np.int64)
@@ -454,8 +401,10 @@ class B200Model:
         df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
         if len(df.columns) == 0:
             raise KeyError(f"None of {self.all_features} are in the [columns]")
-        values, base = getattr(self.engine, method)(self.encoder.encode_frame(df))
-        proba, _ = self.replicas[0].score(df, want_outliers=False)
+        rows = self.encoder.encode_frame(df)
+        with self.replicas[0].lock:
+            values, base = getattr(self.engine, method)(rows)
+            proba, _ = self.replicas[0].score(df, want_outliers=False)
         return {"feature_names": list(self.all_features), "output": self.explain_output, "base_value": float(base),
                 key: values, "predictions": proba.tolist()}
 
@@ -469,54 +418,92 @@ def _reject_nan(df: pd.DataFrame, numeric_features) -> None:
 
 
 class _Replica:
-    """One GPU's view of the model: encode into that engine's pinned staging and score there."""
+    """One GPU's scoring path, and the only code that scores on its engine's handle: the columnar request pipeline
+    (``csrc/scorer.h``, created on first use), else the general path through that engine's pinned staging.
 
-    def __init__(self, encoder: RowEncoder, engine: ForestEngine, has_outlier: bool = False, numeric_features=()):
+    ``lock`` is held around every call on the handle, whoever makes it (calls on one handle must not overlap:
+    ``include/b2f.h``).  It is reentrant because ``B200Model.explain`` holds it across the engine call and ``score``."""
+
+    def __init__(self, encoder: RowEncoder, engine: ForestEngine, has_outlier: bool = False, numeric_features=(), host_threads: int = 0):
         self.encoder, self.engine, self.has_outlier, self.numeric_features = encoder, engine, has_outlier, list(numeric_features)
+        self.host_threads = host_threads
+        self.lock = threading.RLock()
         self._scorer, self._scorer_failed = None, os.environ.get("B200_SCORER", "1") == "0"
-
-    def _scorer_for(self):
-        if self._scorer is None and not self._scorer_failed:
-            try:
-                self._scorer = self.engine.scorer(self.encoder, int(os.environ.get("B200_HOST_THREADS", "0")))
-            except Exception:
-                self._scorer_failed = True
-        return self._scorer
+        self.last_timing = None  # seconds spent in the stages of the last request-pipeline job: columns / first chunk / chunks
 
     def score(self, df: pd.DataFrame, want_outliers: bool = True):
         """-> (proba1 float64 (n,), is_outlier int32 (n,) or None).  ``want_outliers=False``: the classifier alone (no
         outlier forest, so NaN numerics are accepted), on the same row format and kernels as the full pass."""
         n = len(df)
         full = self.has_outlier and want_outliers
-        sc = self._scorer_for() if n else None
-        cols = self.encoder.frame_columns(df) if sc is not None else None
-        if cols is not None:
-            # the columnar request pipeline (csrc/scorer.h): column buffers -> encode threads -> H2D -> kernel(s) -> D2H
+        chunks = self._chunks(df, full)
+        next(chunks)
+        proba, flags = np.empty(n, dtype=np.float64), (np.empty(n, dtype=np.int32) if full else None)
+        for lo, p, f in chunks:
+            proba[lo:lo + len(p)] = p
+            if full:
+                flags[lo:lo + len(f)] = f
+        return proba, flags
+
+    def _chunks(self, df: pd.DataFrame, full: bool):
+        """Score ``df`` on this GPU, holding ``lock`` until the generator is exhausted or closed.  Yields None once the job is
+        in flight (what the caller makes meanwhile overlaps the first chunk), then ``(lo, proba1, is_outlier or None)`` for
+        rows [lo, lo + len(proba1)) as they land; ``full``: the outlier forest too.  The parts are views over pinned buffers
+        that the next job reuses."""
+        t0 = time.perf_counter()
+        with self.lock:
+            n = len(df)
+            if self._scorer is None and not self._scorer_failed and n:
+                try:
+                    self._scorer = self.engine.scorer(self.encoder, self.host_threads)
+                except Exception:
+                    self._scorer_failed = True
+            cols = self.encoder.frame_columns(df) if self._scorer is not None and n else None
+            if cols is None:
+                yield None
+                proba, _, flags = self._staged(df, full)
+                yield 0, proba, flags
+                return
+            # the columnar request pipeline: column buffers -> encode threads -> H2D -> kernel(s) -> D2H, chunk by chunk
             if full:
                 _reject_nan(df, self.numeric_features)
-            n_chunks = sc.start(n, cols, out_mode=OUT_FULL if full else OUT_F64,
-                                fmt=(1 if self.encoder.packed_ok else 0) if self.has_outlier else None)
+            t1 = time.perf_counter()
+            sc = self._scorer
+            # classifier only: the scorer's own choice of rows (64-byte float32 rows: cheapest to encode; ranked rows with
+            # B200_SCORER_ROWS=ranked); with an outlier forest attached float32 rows, even for the classifier alone (ranks are
+            # relative to ONE forest's split values)
+            fmt = (ROWS_PACKED64 if self.encoder.packed_ok else ROWS_WORDS24) if self.has_outlier else None
+            n_chunks = sc.start(n, cols, out_mode=OUT_FULL if full else OUT_F64, fmt=fmt)
+            out, bounds, t_first = sc.results(), sc.bounds, None
+            yield None
             for c in range(n_chunks):  # chunks ride different streams: each has its own completion event
                 sc.wait(c)
-            out = sc.results()
-            if full:
-                return np.array(out["proba1"], dtype=np.float64), np.array(out["is_outlier"])
-            return np.array(out, dtype=np.float64), None
+                t_first = t_first or time.perf_counter()
+                part = out[bounds[c]:bounds[c + 1]]
+                yield (bounds[c], part["proba1"], part["is_outlier"]) if full else (bounds[c], part, None)
+            t2 = time.perf_counter()
+            self.last_timing = {"columns_s": t1 - t0, "first_chunk_s": (t_first or t2) - t1, "chunks_and_lists_s": t2 - t1,
+                                "chunks": n_chunks, "threads": sc.threads, "row_format": sc.last_fmt}
+
+    def _staged(self, df: pd.DataFrame, full: bool, target=None):
+        """The general path: encode into this engine's pinned staging and score with ONE call of ``target`` (this engine, or the
+        group that slices the rows over every GPU) -> views (proba1, label, is_outlier or None) over that staging.  The caller
+        holds the lock of every handle ``target`` drives."""
+        n = len(df)
+        # large requests travel as 64-byte packed rows (one third fewer PCIe bytes), encoded natively in one pass
         packed = self.encoder.packed_ok and n > self.encoder.SMALL_BATCH
-        rows, proba, _ = self.engine.staging(n, packed=packed)
+        rows, proba, label = self.engine.staging(n, packed=packed)
         if packed:
             self.encoder.encode_frame_packed(df, out=rows)
         else:
             self.encoder.encode_frame(df, out=rows)
+        target = self.engine if target is None else target
         if full:
             _reject_nan(df, self.numeric_features)
-            rec = self.engine.predict_full(rows, out=self.engine.staging_full(n))
-            return np.array(rec["proba1"], dtype=np.float64), np.array(rec["is_outlier"])
-        self.engine.predict_rows(rows, proba_dtype=np.float64, want_label=False, out_proba=proba)
-        return np.array(proba, dtype=np.float64), None
-
-    def predict_proba1(self, df: pd.DataFrame) -> np.ndarray:
-        return self.score(df)[0]
+            rec = target.predict_full(rows, out=self.engine.staging_full(n))
+            return rec["proba1"], rec["label"], rec["is_outlier"]
+        target.predict_rows(rows, out_proba=proba, out_label=label)
+        return proba, label, None
 
 
 # ---------------------------------------------------------------------- loading

@@ -66,7 +66,8 @@ class _Pending:
 
 
 class MicroBatcher:
-    """Cross-request batching in front of a replica's ``score`` (one worker thread per model).
+    """Cross-request batching in front of a replica's ``score`` (one worker thread per model; ``score`` takes the replica's
+    lock, so other callers of the same GPU's handle take turns with the worker).
 
     ``models`` is a list (one per GPU); consecutive batches go round-robin over it."""
 
@@ -78,9 +79,6 @@ class MicroBatcher:
         self.batches = 0
         self.rows = 0
         self._stop = False
-        # replica i's engine handle is driven by worker i only, under locks[i]: another caller of that handle (the /explain
-        # handler on the first GPU) takes the same lock, so calls on one handle never overlap (include/b2f.h)
-        self.locks = [threading.Lock() for _ in self.models]
         self._threads = [threading.Thread(target=self._run, args=(i,), daemon=True, name=f"b200-batcher-{i}")
                          for i in range(len(self.models))]
         for t in self._threads:
@@ -139,8 +137,7 @@ class MicroBatcher:
             items = self._collect()
             if items is None:
                 return
-            with self.locks[idx]:
-                self._serve(model, items)
+            self._serve(model, items)
 
     def _serve(self, model, items) -> None:
         try:
@@ -323,28 +320,32 @@ def create_app(model=None, loader=None) -> FastAPI:
 
     app = FastAPI(title=_service_name(), docs_url="/", lifespan=lifespan)
 
-    async def explained(request: Request, method: str, key: str, attached: str = "explainer_attached", missing: str = "explainer",
-                        extra: tuple = ()) -> Response:
-        """The body and error rules of the /explain routes: parse like /predict, 501 unless ``model.<attached>`` (the model has
-        a ``missing``), run ``model.<method>`` under the first batcher worker's lock and answer its ``key`` array as nested lists,
-        plus its ``extra`` keys."""
+    async def answered(request: Request, call) -> Response:
+        """What the /explain routes share: parse the body like /predict (an empty list is a 500, as there), then run
+        ``call(model, frame)`` on the executor.  It returns the answer: a Response, or a dict sent as compact JSON."""
         input_df = parser.frame(await request.body())
         if len(input_df) == 0:
             raise KeyError(f"None of {ALL_FEATURES} are in the [columns]")
-        m = ml_models["credit_default"]
-        if not getattr(m, attached, False):
-            return Response(content=json.dumps({"detail": f"this model has no {missing}"}), status_code=501, media_type="application/json")
-        batcher = ml_models["_batcher"]
+        out = await asyncio.get_running_loop().run_in_executor(None, call, ml_models["credit_default"], input_df)
+        if isinstance(out, Response):
+            return out
+        return Response(content=json.dumps(out, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
 
-        def run():
-            with batcher.locks[0]:  # the explainer sits on the first GPU, whose handle batcher worker 0 drives
-                return getattr(m, method)(input_df)
+    async def explained(request: Request, method: str, key: str, attached: str = "explainer_attached", missing: str = "explainer",
+                        extra: tuple = ()) -> Response:
+        """The TreeSHAP routes: 501 unless ``model.<attached>`` (the model has a ``missing``), else ``model.<method>``'s ``key``
+        array as nested lists, plus its ``extra`` keys."""
 
-        out = await asyncio.get_running_loop().run_in_executor(None, run)
-        body = {"feature_names": list(out["feature_names"]), "output": out["output"], "base_value": float(out["base_value"]),
-                "predictions": list(out["predictions"]), key: np.asarray(out[key], dtype=np.float64).tolist()}
-        body.update({k: out[k] for k in extra})
-        return Response(content=json.dumps(body, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
+        def call(m, input_df):
+            if not getattr(m, attached, False):
+                return Response(content=json.dumps({"detail": f"this model has no {missing}"}), status_code=501, media_type="application/json")
+            out = getattr(m, method)(input_df)
+            body = {"feature_names": list(out["feature_names"]), "output": out["output"], "base_value": float(out["base_value"]),
+                    "predictions": list(out["predictions"]), key: np.asarray(out[key], dtype=np.float64).tolist()}
+            body.update({k: out[k] for k in extra})
+            return body
+
+        return await answered(request, call)
 
     @app.post("/explain", openapi_extra={"requestBody": _REQUEST_SCHEMA})
     async def explain(request: Request):
@@ -385,34 +386,28 @@ def create_app(model=None, loader=None) -> FastAPI:
         problem = _dependence_problem(features, values, kind, grid_resolution)
         if problem:
             return _unprocessable(problem)
-        input_df = parser.frame(await request.body())
-        if len(input_df) == 0:
-            raise KeyError(f"None of {ALL_FEATURES} are in the [columns]")
-        m = ml_models["credit_default"]
-        kw = {"kind": kind, "grid_resolution": grid_resolution}
-        if values:
-            name = features[0]
-            try:
-                kw["custom_values"] = {name: [_query_value(v, name in m.categorical_features) for v in values]}
-            except ValueError:
-                return _unprocessable(f"value parameters of numeric field {name!r} must be numbers")
-        elif getattr(m, "background_attached", False):
-            grids = m.dependence_grids if grid_resolution == dependence.DEFAULT_RESOLUTION else {}
-            kw["custom_values"] = {f: grids[f] for f in features if f in grids}
-            kw["grid_frame"] = m.background
-        batcher = ml_models["_batcher"]
 
-        def run():
-            with batcher.locks[0]:  # the first GPU's handle, which batcher worker 0 drives
-                return m.partial_dependence(input_df, features, **kw)
+        def call(m, input_df):
+            kw = {"kind": kind, "grid_resolution": grid_resolution}
+            if values:
+                name = features[0]
+                try:
+                    kw["custom_values"] = {name: [_query_value(v, name in m.categorical_features) for v in values]}
+                except ValueError:
+                    return _unprocessable(f"value parameters of numeric field {name!r} must be numbers")
+            elif getattr(m, "background_attached", False):
+                grids = m.dependence_grids if grid_resolution == dependence.DEFAULT_RESOLUTION else {}
+                kw["custom_values"] = {f: grids[f] for f in features if f in grids}
+                kw["grid_frame"] = m.background
+            out = m.partial_dependence(input_df, features, **kw)
+            body = {"feature_names": out["feature_names"], "output": out["output"],
+                    "grid_values": [[_json_value(v) for v in g] for g in out["grid_values"]]}
+            for key in ("average", "individual"):
+                if key in out:
+                    body[key] = [np.asarray(a, dtype=np.float64).tolist() for a in out[key]]
+            return body
 
-        out = await asyncio.get_running_loop().run_in_executor(None, run)
-        body = {"feature_names": out["feature_names"], "output": out["output"],
-                "grid_values": [[_json_value(v) for v in g] for g in out["grid_values"]]}
-        for key in ("average", "individual"):
-            if key in out:
-                body[key] = [np.asarray(a, dtype=np.float64).tolist() for a in out[key]]
-        return Response(content=json.dumps(body, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
+        return await answered(request, call)
 
     @app.post("/explain/counterfactual", openapi_extra={"requestBody": _REQUEST_SCHEMA, "parameters": _COUNTERFACTUAL_PARAMETERS})
     async def explain_counterfactual(request: Request):
@@ -427,21 +422,14 @@ def create_app(model=None, loader=None) -> FastAPI:
         problem = _counterfactual_problem(features, cutoff)
         if problem:
             return _unprocessable(problem)
-        input_df = parser.frame(await request.body())
-        if len(input_df) == 0:
-            raise KeyError(f"None of {ALL_FEATURES} are in the [columns]")
-        m = ml_models["credit_default"]
-        batcher = ml_models["_batcher"]
 
-        def run():
-            with batcher.locks[0]:  # the first GPU's handle, which batcher worker 0 drives
-                return m.counterfactuals(input_df, features or None, cutoff=float(cutoff))
+        def call(m, input_df):
+            out = m.counterfactuals(input_df, features or None, cutoff=float(cutoff))
+            return {"feature_names": list(out["feature_names"]), "output": out["output"], "cutoff": out["cutoff"],
+                    "predictions": np.asarray(out["predictions"], dtype=np.float64).tolist(), "decisions": np.asarray(out["decisions"]).tolist(),
+                    "counterfactuals": [_counterfactual_json(f, cf) for f, cf in zip(out["feature_names"], out["counterfactuals"])]}
 
-        out = await asyncio.get_running_loop().run_in_executor(None, run)
-        body = {"feature_names": list(out["feature_names"]), "output": out["output"], "cutoff": out["cutoff"],
-                "predictions": np.asarray(out["predictions"], dtype=np.float64).tolist(), "decisions": np.asarray(out["decisions"]).tolist(),
-                "counterfactuals": [_counterfactual_json(f, cf) for f, cf in zip(out["feature_names"], out["counterfactuals"])]}
-        return Response(content=json.dumps(body, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
+        return await answered(request, call)
 
     @app.post("/predict", response_model=ModelOutput, openapi_extra={"requestBody": _REQUEST_SCHEMA})
     async def predict(request: Request):

@@ -4,6 +4,7 @@
 import json
 import os
 import struct
+import threading
 
 import numpy as np
 import pandas as pd
@@ -268,9 +269,10 @@ def test_http_explain_stub():
 class _Replica:
     def __init__(self, idx, log):
         self.idx, self.log = idx, log
+        self.lock = threading.RLock()
 
     def score(self, df, want_outliers=True):
-        self.log.append((self.idx, want_outliers))
+        self.log.append((self.idx, want_outliers, self.lock._is_owned()))
         if self.idx:
             raise AssertionError("explain() must not touch another GPU's replica")
         return (df["credit_limit"].to_numpy(dtype=np.float64) % 1000) / 1000.0, None
@@ -281,10 +283,11 @@ class _Untouchable:
         raise AssertionError(f"explain() must not use the multi-GPU group ({name})")
 
 
-def test_explain_uses_the_first_gpu_only():
+def test_explain_uses_the_first_gpu_only_under_its_lock():
     """On a multi-GPU model explain() runs entirely on the first GPU's handle -- contributions from its engine, predictions
     from its scoring replica (classifier only) -- and never enters the group call that drives every GPU's handle, whose
-    replicas the HTTP batcher's other workers are using at the same time."""
+    replicas the HTTP batcher's other workers are using at the same time.  The first replica's lock is held across both
+    calls, so the batcher's first worker cannot score on that handle in between."""
     from databricks_kubernetes_mlops_poc_b200.model import B200Model
     from databricks_kubernetes_mlops_poc_b200.schema import ALL_FEATURES, sample_request
 
@@ -307,5 +310,5 @@ def test_explain_uses_the_first_gpu_only():
     df = pd.DataFrame(sample_request() * 3)
     df["credit_limit"] = [1250.0, 2500.0, 100.0]
     out = m.explain(df)
-    assert log == [(0, False)]
+    assert log == [(0, False, True)] and not m.replicas[0].lock._is_owned()
     assert out["predictions"] == [0.25, 0.5, 0.1] and out["base_value"] == 0.25 and out["output"] == "probability"

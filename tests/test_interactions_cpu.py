@@ -204,9 +204,10 @@ def test_http_explain_interactions_stub():
     assert "/explain/interactions" in paths
 
 
-def test_explain_interactions_uses_the_first_gpu_only():
+def test_explain_interactions_uses_the_first_gpu_only_under_its_lock():
     """On a multi-GPU model explain_interactions() runs on the first GPU's handle only: interaction values from its engine,
-    predictions from its scoring replica with the classifier alone, never the group call that drives every GPU."""
+    predictions from its scoring replica with the classifier alone, never the group call that drives every GPU.  The first
+    replica's lock is held across both calls."""
     import pandas as pd
 
     from databricks_kubernetes_mlops_poc_b200.model import B200Model
@@ -232,7 +233,7 @@ def test_explain_interactions_uses_the_first_gpu_only():
     df = pd.DataFrame(sample_request() * 3)
     df["credit_limit"] = [1250.0, 2500.0, 100.0]
     out = m.explain_interactions(df)
-    assert log == [(0, False)]
+    assert log == [(0, False, True)] and not m.replicas[0].lock._is_owned()
     assert out["predictions"] == [0.25, 0.5, 0.1] and out["base_value"] == 0.25 and out["interactions"].shape == (3, 23, 23)
     m.explain_blob = None
     with pytest.raises(RuntimeError, match="no explainer"):

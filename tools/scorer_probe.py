@@ -59,16 +59,13 @@ for th in (1, 8, 16, 32, 48):
     gap()
     res[f"scorer_t{th}_chunk8192_after_3ms_idle_us"] = 1e6 * float(np.median([gap() for _ in range(20)]))
     sc.close()
-# plugin call by request size, pipeline vs general path
-for minrows in ("1", "1000000"):
-    os.environ["B200_PIPELINE_MIN_ROWS"] = minrows
-    import importlib
-    from databricks_kubernetes_mlops_poc_b200 import model as mm
-    mm.B200Model.PIPELINE_MIN_ROWS = int(minrows)
+# plugin call by request size, pipeline vs general path (B200_SCORER=0)
+for scorer in ("1", "0"):
+    os.environ["B200_SCORER"] = scorer
     m = B200Model(flat, devices=[0])
     for n in (1, 16, 128, 256, 1024, 4096, 65536):
         sub = df.iloc[:n]
-        res[f"predict_n{n}_minrows{minrows}_us"] = med(lambda: m.predict(sub), 30)
+        res[f"predict_n{n}_scorer{scorer}_us"] = med(lambda: m.predict(sub), 30)
     m.close()
 print(json.dumps(res, indent=1))
 os.makedirs(OUT, exist_ok=True)

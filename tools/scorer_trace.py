@@ -19,7 +19,7 @@ df = training.arrays_to_frame(pv, pc, pn)[ALL_FEATURES]
 model = B200Model(flat, devices=[0], host_threads=int(os.environ.get("TRACE_THREADS", "0")))
 for _ in range(20):
     model.predict(df)
-sc = model._scorer
+sc = model.replicas[0]._scorer
 lib = _cabi.load_library()
 K = int(os.environ.get("TRACE_STEPS", "200"))
 chunk_rows = int(os.environ.get("TRACE_CHUNK_ROWS", "0"))
