@@ -36,6 +36,10 @@ PD_PROBE_DTYPE = np.dtype([("word", np.int32), ("grid_offset", np.int32), ("coun
 COUNTERFACTUAL_DTYPE = np.dtype(  # struct b2f_counterfactual, 32 bytes
     [("lower_p1", np.float64), ("upper_p1", np.float64), ("lower", np.float32), ("upper", np.float32), ("value", np.float32), ("reserved", np.int32)]
 )
+PERM_SCORE_DTYPE = np.dtype(  # struct b2f_perm_score, 64 bytes
+    [("tp", np.int64), ("fp", np.int64), ("tn", np.int64), ("fn", np.int64), ("log_loss_sum", np.float64), ("brier_sum", np.float64),
+     ("auc_u2", np.uint64), ("reserved", np.uint64)]
+)
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG_DIR, "lib", "libb200forest.so")
@@ -187,6 +191,11 @@ SIGNATURES = {
     "b2f_counterfactual_device": (
         C.c_int,
         [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_void_p],
+    ),
+    "b2f_permutation_scores": (
+        C.c_int,
+        [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+         C.POINTER(C.c_float)],
     ),
     "b2f_predict_async_ex": (
         C.c_int,

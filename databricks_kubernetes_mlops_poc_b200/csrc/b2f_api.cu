@@ -34,6 +34,7 @@
 #include "forest_rank.h"
 #include "partial_dependence.cuh"
 #include "counterfactual.cuh"
+#include "permutation_importance.cuh"
 #include "tree_shap.cuh"
 #include "tree_shap_interactions.cuh"
 #include "tree_shap_interventional.cuh"
@@ -175,6 +176,18 @@ struct Counterfactual {
     DevBuf dev;                  /* the table on the device */
 };
 
+/* permutation importance (b2f_permutation_scores; permutation_importance.cuh): a call's rows, labels and permutations and
+ * its groups' scratch, on the compute stream; grown on demand and kept for the model's life */
+struct Importance {
+    DevBuf rows, labels, perm;
+    DevBuf keys;    /* two [point][row] key arrays of a group: the kernel's and the sort's other buffer */
+    DevBuf flags;   /* the same for the flags bytes */
+    DevBuf temp;    /* the segmented sort's temporary storage */
+    DevBuf offsets; /* point p of a group starts at p * n */
+    DevBuf segs;    /* the group's PiSeg table */
+    DevBuf scores;  /* the group's records */
+};
+
 struct TicketRec {
     uint64_t id = 0;
     cudaEvent_t ev[B2F_STREAMS] = {nullptr, nullptr, nullptr, nullptr};
@@ -220,6 +233,7 @@ struct b2f_model {
     Explainer *ex = nullptr; /* attached TreeSHAP path table (b2f_model_attach_explainer) */
     Dependence pd;
     Counterfactual cf;
+    Importance pi;
     b2f_model *outlier = nullptr; /* attached isolation forest (b2f_model_attach_outlier_forest): a child handle on the
                                      same device whose kernels are launched on this handle's streams and rows */
     Slot slots[B2F_STREAMS];
@@ -865,6 +879,7 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
         if (sl.stream) cudaStreamDestroy(sl.stream);
     }
     for (DevBuf *b : {&m->scratch, &m->pd.host_spec, &m->pd.device_spec, &m->cf.dev, &m->mom_rows, &m->gather, &m->flush}) b->release();
+    for (DevBuf *b : {&m->pi.rows, &m->pi.labels, &m->pi.perm, &m->pi.keys, &m->pi.flags, &m->pi.temp, &m->pi.offsets, &m->pi.segs, &m->pi.scores}) b->release();
     for (auto &t : m->tickets)
         for (auto &e : t.ev)
             if (e) cudaEventDestroy(e);
@@ -1724,3 +1739,6 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
 
 /* ------------------------------------------------------------------ counterfactuals (K7) */
 #include "counterfactual_api.cuh"
+
+/* ------------------------------------------------------------------ permutation importance (K8) */
+#include "importance_api.cuh"

@@ -103,8 +103,10 @@ __device__ __forceinline__ void pd_stage_row(const PdParams &p, const uint32_t *
 }
 
 /* The mask walk: acc[k] += every leaf payload that point k of a segment reaches, tree by tree in tree order.  One walk per
- * (row, tree) forks only at splits on row word `word`, with gv[k] (shared) the word point k puts there and `full` the mask
- * of the segment's points; xw = the warp's staged rows; stk = the block's walk stacks, column threadIdx.x this thread's. */
+ * (row, tree) forks only at splits on row word `word`, with gv[k * PSTRIDE] (shared) the word point k puts there and `full`
+ * the mask of the segment's points; xw = the warp's staged rows; stk = the block's walk stacks, column threadIdx.x this
+ * thread's.  PSTRIDE = 1: one point table for the block (K6, K7); K8 passes its thread's column of a per-thread table. */
+template <int PSTRIDE = 1>
 __device__ __forceinline__ void pd_mask_walk(const PdParams &p, uint32_t word, uint32_t full, const uint32_t *gv, const uint32_t (*xw)[32],
                                              int lane, unsigned long long (*stk)[B2F_PD_WARPS * 32], double (&acc)[B2F_PD_SEG]) {
     for (int g = 0; g < p.n_groups; ++g) {
@@ -133,7 +135,7 @@ __device__ __forceinline__ void pd_mask_walk(const PdParams &p, uint32_t word, u
                 if (feat == word) {
                     uint32_t sec = 0;
 #pragma unroll
-                    for (int k = 0; k < B2F_PD_SEG; ++k) sec |= (take_second(gv[k], tm.x, tm.y) ? 1u : 0u) << k;
+                    for (int k = 0; k < B2F_PD_SEG; ++k) sec |= (take_second(gv[k * PSTRIDE], tm.x, tm.y) ? 1u : 0u) << k;
                     const uint32_t m2 = mask & sec, m1 = mask & ~sec;
                     if (m1 && m2) { /* fork: the second child waits on the stack */
                         stk[sp++][threadIdx.x] = ((unsigned long long)m2 << 32) | (first + 1u);

@@ -282,6 +282,26 @@ class ForestEngine:
         check(self._lib.b2f_counterfactual_device(self._h, rows_dev, n, fmt, ptr(w), len(w), float(cutoff), proba_dev, out_dev),
               "b2f_counterfactual_device")
 
+    # ------------------------------------------------------------------ permutation importance (csrc/permutation_importance.cuh)
+    def permutation_scores(self, rows: np.ndarray, labels, perm: np.ndarray, words, device_ms: bool = False):
+        """Encoded rows (N, 24) or packed (N, 16), 0/1 labels (N,), permutations (R, N) of row indices and probed row words
+        -> (records (len(words), R) of ``PERM_SCORE_DTYPE``, baseline record[, device ms]): the metric sums of the rows
+        scored with each word taken from row ``perm[r, i]``, and of the rows as they are (``importance.py`` turns them into
+        scores)."""
+        rows = np.ascontiguousarray(rows)
+        y = np.ascontiguousarray(labels, dtype=np.int32)
+        p = np.ascontiguousarray(perm, dtype=np.int32)
+        w = np.ascontiguousarray(words, dtype=np.int32)
+        n_repeats = p.shape[0] if p.ndim == 2 else 0
+        if y.shape != (rows.shape[0],) or p.ndim != 2 or p.shape[1] != rows.shape[0]:
+            raise ValueError(f"labels {y.shape} and perm {p.shape} must be ({rows.shape[0]},) and (n_repeats, {rows.shape[0]})")
+        out = np.zeros((len(w), max(n_repeats, 1)), dtype=_cabi.PERM_SCORE_DTYPE)
+        base = np.zeros(1, dtype=_cabi.PERM_SCORE_DTYPE)
+        ms = C.c_float(0.0)
+        check(self._lib.b2f_permutation_scores(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(y), ptr(p), n_repeats, ptr(w), len(w),
+                                               ptr(out), ptr(base), C.byref(ms)), "b2f_permutation_scores")
+        return (out, base[0], ms.value) if device_ms else (out, base[0])
+
     # ------------------------------------------------------------------ device-resident interface
     def device_alloc(self, nbytes: int) -> int:
         p = self._lib.b2f_device_alloc(self._h, nbytes)

@@ -28,7 +28,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pandas as pd
 
-from . import dependence
+from . import dependence, importance
 from ._cabi import OUT_F64, OUT_FULL, ROWS_PACKED64, ROWS_WORDS24
 from ._pylists import ListBuilder
 from .encode import RowEncoder
@@ -375,6 +375,35 @@ class B200Model:
                             "upper": r["upper"].astype(np.float64), "upper_prediction": r["upper_p1"].copy()})
         return {"feature_names": features, "output": "probability", "cutoff": cutoff, "predictions": proba, "decisions": decisions,
                 "counterfactuals": out}
+
+    def permutation_importance(self, df, y, *, scoring=None, n_repeats: int = 5, random_state=None) -> dict:
+        """How much the model relies on each request field: scikit-learn's ``permutation_importance(pipeline, df, y,
+        scoring=scoring, n_repeats=n_repeats, random_state=random_state)`` of the fitted pipeline, computed on the GPU.
+
+        Every request field is probed, in the model's field order (the frame's column order does not matter: sklearn uses
+        one permutation for every column).  ``scoring``: None (accuracy, as ``estimator.score``), one name of
+        ``importance.SCORERS`` or a list of them; with a list the answer is a dict keyed by scorer, as sklearn's.  Each
+        answer holds ``importances`` float64 (n_fields, n_repeats) (baseline minus permuted score), ``importances_mean``,
+        ``importances_std`` (ddof 0), ``baseline_score``, ``feature_names``, ``n_repeats`` and ``rows``.  ``y``: one 0/1
+        label per row.  Rows are scored by the classifier alone, as ``explain`` scores them, so NaN numerics are accepted
+        even with an outlier forest attached.  ``roc_auc`` is NaN with one class in ``y``; ``neg_log_loss`` raises
+        ValueError there, as sklearn does.  It runs on the first GPU's handle only, under ``replicas[0].lock``."""
+        names, multi = importance.check_scoring(scoring)
+        n_repeats = importance.check_n_repeats(n_repeats)
+        df = df if isinstance(df, pd.DataFrame) else pd.DataFrame(df)
+        if len(df.columns) == 0:
+            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        labels = importance.check_labels(y, len(df))
+        if len(df) == 0:
+            raise ValueError("permutation importance needs at least one row")
+        importance.check_single_class(names, labels)
+        perm = importance.permutations(len(df), n_repeats, random_state)
+        rows = self.encoder.encode_frame(df)
+        words = [dependence.word_of(self.encoder, f) for f in self.all_features]
+        with self.replicas[0].lock:
+            rec, base = self.engine.permutation_scores(rows, labels, perm, words)
+        out = {s: importance.result(s, rec, base, self.all_features, n_repeats, len(df)) for s in names}
+        return out if multi else out[names[0]]
 
     def explain_interventional(self, model_input) -> dict:
         """Exact interventional TreeSHAP contributions of every request field against the attached background set (what

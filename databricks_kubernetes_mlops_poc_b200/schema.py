@@ -12,9 +12,9 @@ batching loop here builds its columns directly and does not need that).
 
 from __future__ import annotations
 
-from typing import TypedDict
+from typing import Annotated, Required, TypedDict
 
-from pydantic import BaseModel, TypeAdapter, create_model
+from pydantic import BaseModel, Field, TypeAdapter, create_model
 
 # (name, default) in the order the model was trained on: categorical block, then numeric block
 # (reference 01-train-model.ipynb:126-158; defaults from app/model.py:12-34 -- including the
@@ -54,6 +54,19 @@ LoanApplicantRow = TypedDict(
     total=False,
 )
 REQUEST_ROWS = TypeAdapter(list[LoanApplicantRow])  # validate_json: JSON parsing + validation in one pass of pydantic-core
+
+# A labelled applicant (``POST /explain/importance``): the same fields plus the reference's target column, required and 0/1
+# (reference 01-train-model.ipynb: ``default_payment_next_month``).
+TARGET = "default_payment_next_month"
+_Label = Annotated[int, Field(ge=0, le=1)]
+LabelledApplicant = create_model("LabelledApplicant", __base__=LoanApplicant, **{TARGET: (_Label, ...)})
+LabelledApplicant.__doc__ = "One applicant with its observed outcome: LoanApplicant's fields plus the 0/1 target."
+LabelledApplicantRow = TypedDict(
+    "LabelledApplicantRow",
+    {**{n: str for n in CATEGORICAL_FEATURES}, **{n: float for n in NUMERIC_FEATURES}, TARGET: Required[_Label]},
+    total=False,
+)
+LABELLED_ROWS = TypeAdapter(list[LabelledApplicantRow])
 
 FeatureBatchDrift = create_model("FeatureBatchDrift", **{n: (float, ...) for n in ALL_FEATURES})
 FeatureBatchDrift.__doc__ = "Per-feature drift score of the request batch (1 - p-value)."

@@ -40,9 +40,12 @@ import numpy as np
 import pandas as pd
 from fastapi import FastAPI, Request, Response
 
-from . import dependence
+from fastapi.exceptions import RequestValidationError
+from pydantic import ValidationError
+
+from . import dependence, importance
 from .ingest import NativeRequestParser, parse_rows, rows_to_frame  # noqa: F401  (rows_to_frame re-exported)
-from .schema import ALL_FEATURES, LoanApplicant, ModelOutput
+from .schema import ALL_FEATURES, LABELLED_ROWS, TARGET, LabelledApplicant, LoanApplicant, ModelOutput
 
 ml_models: dict = {}
 
@@ -249,6 +252,46 @@ def _counterfactual_json(name: str, cf: dict) -> dict:
                                 for k in ("value", "lower", "lower_prediction", "upper", "upper_prediction")}}
 
 
+_LABELLED_SCHEMA = {"required": True, "content": {"application/json": {"schema": {
+    "title": "Data", "type": "array", "items": LabelledApplicant.model_json_schema()}}}}
+
+_IMPORTANCE_PARAMETERS = [
+    {"name": "scoring", "in": "query", "required": False, "description": "scorer; repeat for several; none = accuracy",
+     "schema": {"type": "array", "items": {"type": "string", "enum": list(importance.SCORERS)}}, "style": "form", "explode": True},
+    {"name": "n_repeats", "in": "query", "required": False,
+     "schema": {"type": "integer", "minimum": 1, "maximum": importance.MAX_REPEATS, "default": 5}},
+    {"name": "random_state", "in": "query", "required": False, "description": "seed of the permutations (numpy RandomState)",
+     "schema": {"type": "integer", "minimum": 0, "maximum": 2**32 - 1, "default": 0}},
+]
+
+
+def _importance_problem(scoring, n_repeats: str, random_state: str) -> str | None:
+    """Why a /explain/importance query is unprocessable, or None."""
+    try:
+        importance.check_scoring(scoring or None)
+    except ValueError as e:
+        return str(e)
+    try:
+        importance.check_n_repeats(int(n_repeats))
+    except ValueError:
+        return f"n_repeats must be an integer in 1..{importance.MAX_REPEATS}"
+    try:
+        seed = int(random_state)
+    except ValueError:
+        seed = -1
+    if not 0 <= seed < 2**32:
+        return "random_state must be an integer in [0, 2**32 - 1]"
+    return None
+
+
+def parse_labelled(raw: bytes) -> list:
+    """A /explain/importance body -> validated dict rows (pydantic-core, FastAPI's 422 on a bad field or label)."""
+    try:
+        return LABELLED_ROWS.validate_json(raw)
+    except ValidationError as e:
+        raise RequestValidationError([{**err, "loc": ("body", *err["loc"])} for err in e.errors(include_url=False, include_context=False)])
+
+
 def _dependence_problem(features, values, kind, grid_resolution) -> str | None:
     """Why a /explain/dependence query is unprocessable, or None."""
     if not features:
@@ -430,6 +473,45 @@ def create_app(model=None, loader=None) -> FastAPI:
                     "counterfactuals": [_counterfactual_json(f, cf) for f, cf in zip(out["feature_names"], out["counterfactuals"])]}
 
         return await answered(request, call)
+
+    @app.post("/explain/importance", openapi_extra={"requestBody": _LABELLED_SCHEMA, "parameters": _IMPORTANCE_PARAMETERS})
+    async def explain_importance(request: Request):
+        """Which fields the model relies on: permutation importance against labelled applicants (each applicant's fields
+        plus its observed `default_payment_next_month`), scikit-learn's `permutation_importance` of the fitted pipeline.
+        Every field is shuffled across the applicants `n_repeats` times and the drop of each scorer below its baseline is
+        reported per field (`importances_mean`, `importances_std`, and every repeat in `importances`); null where a score is
+        undefined (roc_auc with one class).  422 for an unknown scorer, a bad n_repeats or random_state, a missing or
+        non-0/1 label, and labels of one class with neg_log_loss."""
+        q = request.query_params
+        scoring, n_repeats, random_state = q.getlist("scoring"), q.get("n_repeats", "5"), q.get("random_state", "0")
+        problem = _importance_problem(scoring, n_repeats, random_state)
+        if problem:
+            return _unprocessable(problem)
+        rows = parse_labelled(await request.body())
+        if len(rows) == 0:
+            raise KeyError(f"None of {ALL_FEATURES} are in the [columns]")
+        labels = np.array([r[TARGET] for r in rows], dtype=np.int32)
+        names = scoring or [importance.DEFAULT_SCORER]
+        try:
+            importance.check_single_class(names, labels)
+        except ValueError as e:
+            return _unprocessable(str(e))
+        frame = rows_to_frame(rows)
+
+        def call():
+            out = ml_models["credit_default"].permutation_importance(frame, labels, scoring=names, n_repeats=int(n_repeats),
+                                                                    random_state=int(random_state))
+            first = out[names[0]]
+            return {"feature_names": list(first["feature_names"]), "rows": int(first["rows"]), "n_repeats": int(first["n_repeats"]),
+                    "random_state": int(random_state),
+                    "scores": {s: {"baseline": importance.json_number(r["baseline_score"]),
+                                   "importances_mean": [importance.json_number(v) for v in r["importances_mean"]],
+                                   "importances_std": [importance.json_number(v) for v in r["importances_std"]],
+                                   "importances": [[importance.json_number(v) for v in row] for row in r["importances"]]}
+                               for s, r in out.items()}}
+
+        out = await asyncio.get_running_loop().run_in_executor(None, call)
+        return Response(content=json.dumps(out, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
 
     @app.post("/predict", response_model=ModelOutput, openapi_extra={"requestBody": _REQUEST_SCHEMA})
     async def predict(request: Request):

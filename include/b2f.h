@@ -414,6 +414,38 @@ int b2f_counterfactual(b2f_model *m, const void *rows, int64_t n, int row_format
 int b2f_counterfactual_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const int32_t *words, int n_words,
                               double cutoff, double *proba_dev, struct b2f_counterfactual *out_dev);
 
+/* ---- permutation importance (csrc/permutation_importance.cuh) ----
+ * sklearn's permutation_importance against labelled rows, as the records its scorers are computed from.  For each probed
+ * row word words[f] and repeat r, every row i is scored with that word taken from row perm[r * n + i] (the other words its
+ * own), by the classifier alone, exactly as b2f_partial_dependence scores a substituted row (tile order, bit for bit).
+ * out[f * n_repeats + r] gets the metrics of those n scores against labels; baseline gets those of the rows as they are:
+ *     tp, fp, tn, fn   confusion counts of the predicted label (b2f_predict's) against the label (positive = 1)
+ *     log_loss_sum     sum over rows of -log(clip(y ? p1 : 1 - p1, eps, 1 - eps)), eps = float64 epsilon
+ *     brier_sum        sum over rows of (y - p1)^2
+ *     auc_u2           twice the Mann-Whitney statistic of the ranking key with ties counted 1/2 (ROC AUC = auc_u2 / (2 P N));
+ *                      the key is P(class 1) for a RandomForest and the raw margin for a GBDT (sklearn's decision_function)
+ * Integer fields do not depend on order and the sums are in a fixed order, so results are bit-identical from run to run and
+ * do not depend on how the points are grouped.  rows: B2F_ROWS_WORDS24 or B2F_ROWS_PACKED64 in host memory; labels: n int32
+ * (0 or 1); perm: n_repeats x n int32 row indices; words: 1..n_cat + n_num row words (repeats allowed).  The rows, labels and
+ * permutations go to the device once per call, on the compute stream, into buffers the model keeps; the (point, row) keys,
+ * flags and sort buffers of a group of points stay under B2F_PERM_SCRATCH_BYTES (at least one point per group).  Errors:
+ * B2F_EINVAL for ranked rows, n outside 1 .. 2^31 - 1, a label that is not 0 or 1, n_repeats outside 1..B2F_PERM_MAX_REPEATS,
+ * a word outside the fields, a perm entry that is not a row index, a NULL pointer or a forest deeper than 32 levels;
+ * B2F_ENOMEM (with the byte count) when a device buffer cannot be allocated.  device_ms (may be NULL): from the first
+ * upload to the last record's copy back, CUDA events on the compute stream. */
+#define B2F_PERM_MAX_REPEATS 256
+#define B2F_PERM_SCRATCH_BYTES (256ll << 20)
+struct b2f_perm_score {
+    int64_t tp, fp, tn, fn;
+    double log_loss_sum;
+    double brier_sum;
+    uint64_t auc_u2;
+    uint64_t reserved;
+};
+int b2f_permutation_scores(b2f_model *m, const void *rows, int64_t n, int row_format, const int32_t *labels, const int32_t *perm, int n_repeats,
+                           const int32_t *words, int n_words, struct b2f_perm_score *out /* [n_words][n_repeats] */,
+                           struct b2f_perm_score *baseline, float *device_ms);
+
 /* asynchronous form for the request-batching ring: buffers must be pinned and stay valid until
  * b2f_wait(ticket) returns.  proba_is_f64 selects double (1) or float (0) outputs. */
 int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned,
