@@ -197,6 +197,14 @@ SIGNATURES = {
         [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
          C.POINTER(C.c_float)],
     ),
+    "b2f_model_attach_mmd_reference": (
+        C.c_int,
+        [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_float)],
+    ),
+    "b2f_mmd_drift": (
+        C.c_int,
+        [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_double), C.c_void_p, C.POINTER(C.c_float)],
+    ),
     "b2f_predict_async_ex": (
         C.c_int,
         [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_uint64)],

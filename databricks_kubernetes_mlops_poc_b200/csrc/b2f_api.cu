@@ -35,6 +35,7 @@
 #include "partial_dependence.cuh"
 #include "counterfactual.cuh"
 #include "permutation_importance.cuh"
+#include "mmd_drift.cuh"
 #include "tree_shap.cuh"
 #include "tree_shap_interactions.cuh"
 #include "tree_shap_interventional.cuh"
@@ -188,6 +189,17 @@ struct Importance {
     DevBuf scores;  /* the group's records */
 };
 
+/* the MMD drift test (b2f_model_attach_mmd_reference / b2f_mmd_drift; mmd_drift.cuh): the reference's embedding and
+ * kernel row sums, kept between calls, and a call's buffers; all on the compute stream, grown on demand */
+struct Mmd {
+    MmdParams mp;
+    int64_t n_ref = 0; /* 0: no reference */
+    double sigma = 0.0, coef = 0.0;
+    DevBuf ref_z, ref_c, r_ref; /* the reference: embedding and sum_{j != i} k(i, j) over the reference */
+    DevBuf rows, z, c;          /* a call's rows and the batch's embedding */
+    DevBuf r, partial, sub, pairs, out, hist;
+};
+
 struct TicketRec {
     uint64_t id = 0;
     cudaEvent_t ev[B2F_STREAMS] = {nullptr, nullptr, nullptr, nullptr};
@@ -234,6 +246,7 @@ struct b2f_model {
     Dependence pd;
     Counterfactual cf;
     Importance pi;
+    Mmd mmd;
     b2f_model *outlier = nullptr; /* attached isolation forest (b2f_model_attach_outlier_forest): a child handle on the
                                      same device whose kernels are launched on this handle's streams and rows */
     Slot slots[B2F_STREAMS];
@@ -880,6 +893,9 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
     }
     for (DevBuf *b : {&m->scratch, &m->pd.host_spec, &m->pd.device_spec, &m->cf.dev, &m->mom_rows, &m->gather, &m->flush}) b->release();
     for (DevBuf *b : {&m->pi.rows, &m->pi.labels, &m->pi.perm, &m->pi.keys, &m->pi.flags, &m->pi.temp, &m->pi.offsets, &m->pi.segs, &m->pi.scores}) b->release();
+    for (DevBuf *b : {&m->mmd.ref_z, &m->mmd.ref_c, &m->mmd.r_ref, &m->mmd.rows, &m->mmd.z, &m->mmd.c, &m->mmd.r, &m->mmd.partial, &m->mmd.sub,
+                      &m->mmd.pairs, &m->mmd.out, &m->mmd.hist})
+        b->release();
     for (auto &t : m->tickets)
         for (auto &e : t.ev)
             if (e) cudaEventDestroy(e);
@@ -1742,3 +1758,6 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
 
 /* ------------------------------------------------------------------ permutation importance (K8) */
 #include "importance_api.cuh"
+
+/* ------------------------------------------------------------------ MMD drift test (K9) */
+#include "mmd_api.cuh"

@@ -52,6 +52,7 @@ class ForestEngine:
         self._pinned: dict[str, PinnedBuffer] = {}
         self.explainer_attached = False
         self.background_rows = 0
+        self.mmd_reference_rows = 0
         inf = self.info()
         self.rank_words = inf["rank_row_bytes"] // 4 if inf["rank_ok"] else 0  # width of a ranked row, 0 = not available
 
@@ -301,6 +302,37 @@ class ForestEngine:
         check(self._lib.b2f_permutation_scores(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(y), ptr(p), n_repeats, ptr(w), len(w),
                                                ptr(out), ptr(base), C.byref(ms)), "b2f_permutation_scores")
         return (out, base[0], ms.value) if device_ms else (out, base[0])
+
+    # ------------------------------------------------------------------ MMD drift test (csrc/mmd_drift.cuh)
+    def attach_mmd_reference(self, rows: np.ndarray, num_mean, num_scale, sigma: float | None = None, device_ms: bool = False):
+        """Encoded reference rows (N, 24) or packed (N, 16), 2 <= N <= 131 072, and the per-numeric mean and scale of the
+        embedding -> sigma[, device ms]; ``sigma=None``: alibi's median heuristic on the reference.  Replaces an earlier
+        reference."""
+        rows = np.ascontiguousarray(rows)
+        mean = np.ascontiguousarray(num_mean, dtype=np.float64)
+        scale = np.ascontiguousarray(num_scale, dtype=np.float64)
+        out, ms = C.c_double(0.0), C.c_float(0.0)
+        self.mmd_reference_rows = 0  # a failed attach leaves no reference
+        check(self._lib.b2f_model_attach_mmd_reference(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(mean), ptr(scale),
+                                                       float("nan") if sigma is None else float(sigma), C.byref(out), C.byref(ms)),
+              "b2f_model_attach_mmd_reference")
+        self.mmd_reference_rows = rows.shape[0]
+        return (out.value, ms.value) if device_ms else out.value
+
+    def mmd_statistics(self, rows: np.ndarray, subsets: np.ndarray, device_ms: bool = False):
+        """Encoded batch rows (M, 24) or packed (M, 16), M >= 2, and (B, min(M, N_ref)) sorted pool indices -> (observed
+        mmd^2, float64 (B,) permuted mmd^2[, device ms]) against the attached reference (``mmd.py`` draws the subsets)."""
+        rows = np.ascontiguousarray(rows)
+        sub = np.ascontiguousarray(subsets, dtype=np.int32)
+        if sub.ndim != 2:
+            raise ValueError(f"subsets must be (n_permutations, subset size), not {sub.shape}")
+        if self.mmd_reference_rows and sub.shape[1] != min(rows.shape[0], self.mmd_reference_rows):
+            raise ValueError(f"subsets hold {sub.shape[1]} indices each; this batch needs min({rows.shape[0]}, {self.mmd_reference_rows})")
+        perm = np.empty(sub.shape[0], dtype=np.float64)
+        obs, ms = C.c_double(0.0), C.c_float(0.0)
+        check(self._lib.b2f_mmd_drift(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(sub), sub.shape[0], C.byref(obs), ptr(perm),
+                                      C.byref(ms)), "b2f_mmd_drift")
+        return (obs.value, perm, ms.value) if device_ms else (obs.value, perm)
 
     # ------------------------------------------------------------------ device-resident interface
     def device_alloc(self, nbytes: int) -> int:

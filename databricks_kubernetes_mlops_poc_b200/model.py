@@ -20,6 +20,7 @@ when a reference table is supplied; without one every score is 0.0.
 from __future__ import annotations
 
 import contextlib
+import math
 import os
 import threading
 import time
@@ -28,25 +29,27 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pandas as pd
 
-from . import dependence, importance
-from ._cabi import OUT_F64, OUT_FULL, ROWS_PACKED64, ROWS_WORDS24
+from . import dependence, importance, mmd
+from ._cabi import OUT_F64, OUT_FULL, ROWS_PACKED64, ROWS_WORDS24, B2FError
 from ._pylists import ListBuilder
 from .encode import RowEncoder
 from .engine import EngineGroup, ForestEngine
-from .flatten import AGG_RF_MEAN, FlatForest, flatten_explainer, flatten_isolation_forest, flatten_pipeline
+from .flatten import AGG_RF_MEAN, FlatForest, flatten_explainer, flatten_isolation_forest, flatten_pipeline, parse_header
 
 BLOB_FILE = "forest.b2f.npz"
 OUTLIER_BLOB_FILE = "outlier.b2f"
 DRIFT_FILE = "drift_reference.npz"
 EXPLAIN_FILE = "explain.b2f"  # TreeSHAP path table (flatten_explainer); optional
 BACKGROUND_FILE = "explain_background.npz"  # background rows of interventional explanations (raw columns); optional
+MMD_FILE = "mmd_reference.npz"  # reference rows of the MMD drift test (raw columns, and its sigma); optional
 OUTLIER_PICKLE = os.path.join("artifacts", "outlier.pkl")  # joblib.dump(outlier, ".../outlier.pkl"), 02-register-model.ipynb:264,326-328
 SKLEARN_PICKLE = os.path.join("artifacts", "classifier", "model", "model.pkl")  # MLflow layout, 02-register-model.ipynb:317-321
 
 
 class B200Model:
     def __init__(self, flat: FlatForest, devices=None, drift=None, outlier_blob: bytes | None = None, host_threads: int = 0,
-                 explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None):
+                 explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None,
+                 mmd_reference: pd.DataFrame | None = None, mmd_sigma: float | None = None):
         self.flat = flat
         self.all_features = flat.all_features
         self.categorical_features = list(flat.cat_features)
@@ -80,6 +83,10 @@ class B200Model:
         self.dependence_grids = None  # field -> default partial-dependence grid of the background (attach_background)
         if explain_background is not None:
             self.attach_background(explain_background)
+        self.mmd_reference_rows = 0
+        self.mmd_sigma = None  # the attached MMD reference's kernel width
+        if mmd_reference is not None:
+            self.attach_mmd_reference(mmd_reference, sigma=mmd_sigma)
 
     # ------------------------------------------------------------------ construction
     @classmethod
@@ -90,7 +97,8 @@ class B200Model:
         ``outlier``: the reference's fitted outlier detector (an alibi-detect ``IForest`` or a bare sklearn
         ``IsolationForest`` plus ``outlier_threshold=``), flattened into a second forest over the same rows.
         ``explain``: also build the TreeSHAP path table, so that ``explain()`` works.  ``background``: a frame of raw rows
-        (e.g. the training table) to attach for ``explain_interventional()``; it needs ``explain``."""
+        (e.g. the training table) to attach for ``explain_interventional()``; it needs ``explain``.  ``mmd_reference=frame``
+        (and ``mmd_sigma=``): the reference table of ``mmd_drift()``."""
         if background is not None and not explain:
             raise ValueError("a background is for interventional explanations: pass explain=True with it")
         flat = flatten_pipeline(pipeline)
@@ -405,6 +413,55 @@ class B200Model:
         out = {s: importance.result(s, rec, base, self.all_features, n_repeats, len(df)) for s in names}
         return out if multi else out[names[0]]
 
+    @property
+    def mmd_reference_attached(self) -> bool:
+        return self.mmd_reference_rows > 0
+
+    def attach_mmd_reference(self, frame: pd.DataFrame, *, sigma: float | None = None) -> float:
+        """Attach the reference table of ``mmd_drift``: 2..131 072 raw rows, encoded as requests are, embedded once on the
+        first GPU with the z-score constants of their numerics; replaces an earlier reference.  ``sigma``: the Gaussian
+        kernel's width; None: alibi-detect's median heuristic on the reference (ValueError when the median pair distance is 0).
+        -> sigma."""
+        sigma = mmd.check_sigma(sigma)
+        frame = frame if isinstance(frame, pd.DataFrame) else pd.DataFrame(frame)
+        mmd.check_reference(len(frame))
+        rows = self.encoder.encode_frame(frame)
+        n_cat, n_num = len(self.categorical_features), len(self.numeric_features)
+        impute = parse_header(self.flat.blob)["impute"][n_cat:n_cat + n_num]
+        mean, scale = mmd.standardization(mmd.numerics(rows, n_cat, n_num, impute))
+        self.mmd_reference_rows, self.mmd_sigma = 0, None
+        with self.replicas[0].lock:
+            try:
+                got = self.engine.attach_mmd_reference(rows, mean, scale, sigma)
+            except B2FError as e:
+                if "median pair distance is 0" in str(e):
+                    raise ValueError(f"{e}: attach this reference with an explicit sigma") from e
+                raise
+        self.mmd_reference_rows, self.mmd_sigma = len(frame), got
+        return got
+
+    def mmd_drift(self, model_input, *, n_permutations: int = 100, p_val: float = 0.05, random_state: int = 0) -> dict:
+        """Has the joint distribution of the request fields moved?  alibi-detect's ``MMDDrift(x_ref, p_val=p_val,
+        n_permutations=n_permutations).predict(x)["data"]`` on the classifier's input vectors (``mmd.py``), with the kernel
+        sums on the GPU: the unbiased MMD^2 of the batch against the attached reference and a p-value from permutations of
+        the pooled rows.  -> ``{"is_drift": 0/1, "distance": mmd^2, "p_val", "threshold": p_val, "distance_threshold": the
+        permuted statistic at the p_val quantile, "sigma", "n_permutations", "reference_rows", "rows"}``.  It runs on the
+        first GPU's handle only, under ``replicas[0].lock``.  RuntimeError without a reference; ValueError for fewer than 2
+        rows, a bad argument or more kernel pairs than ``mmd.PAIR_BUDGET``."""
+        if not self.mmd_reference_attached:
+            raise RuntimeError("this model has no MMD reference: attach_mmd_reference(frame), from_pipeline(..., mmd_reference=frame) "
+                               f"or a model directory that holds {MMD_FILE} (save_model_dir(..., mmd_reference=frame))")
+        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
+        if len(df.columns) == 0:
+            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        n_ref = self.mmd_reference_rows
+        n_permutations, p_val, random_state = mmd.check_request(len(df), n_ref, n_permutations, p_val, random_state)
+        rows = self.encoder.encode_frame(df)
+        subsets = mmd.draw_subsets(n_ref, len(df), n_permutations, random_state)
+        with self.replicas[0].lock:
+            obs, perm = self.engine.mmd_statistics(rows, subsets)
+        return mmd.result(obs, perm, p_val, self.mmd_sigma, n_ref, len(df))
+
     def explain_interventional(self, model_input) -> dict:
         """Exact interventional TreeSHAP contributions of every request field against the attached background set (what
         shap's ``TreeExplainer(model, data)`` computes): the mean, over background rows z, of each field's Shapley value in
@@ -537,10 +594,12 @@ class _Replica:
 
 # ---------------------------------------------------------------------- loading
 def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | None = None, outlier_blob: bytes | None = None,
-                   explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None) -> None:
+                   explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None,
+                   mmd_reference: pd.DataFrame | None = None, mmd_sigma: float | None = None) -> None:
     """Write the GPU-side artefact next to (or instead of) the MLflow pickles.  ``explain_blob``: the TreeSHAP path table
     (``flatten_explainer``), written as ``explain.b2f`` so that ``load_model`` attaches it.  ``explain_background``: raw
-    rows written as ``explain_background.npz``, attached by ``load_model`` with the explainer."""
+    rows written as ``explain_background.npz``, attached by ``load_model`` with the explainer.  ``mmd_reference``: raw rows
+    written as ``mmd_reference.npz`` with ``mmd_sigma`` (None: the median heuristic at load), attached by ``load_model``."""
     os.makedirs(path, exist_ok=True)
     flat.save(os.path.join(path, BLOB_FILE))
     if explain_blob is not None:
@@ -548,6 +607,9 @@ def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | 
             f.write(explain_blob)
     if explain_background is not None:
         _save_background(os.path.join(path, BACKGROUND_FILE), flat, explain_background)
+    if mmd_reference is not None:
+        sigma = mmd.check_sigma(mmd_sigma)
+        _save_background(os.path.join(path, MMD_FILE), flat, mmd_reference, mmd_sigma=np.float64(np.nan if sigma is None else sigma))
     if outlier_blob is not None:
         with open(os.path.join(path, OUTLIER_BLOB_FILE), "wb") as f:
             f.write(outlier_blob)
@@ -557,10 +619,10 @@ def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | 
         TabularDrift(reference_frame[flat.all_features], flat.cat_features, device=None).save(os.path.join(path, DRIFT_FILE))
 
 
-def _save_background(path: str, flat: FlatForest, frame: pd.DataFrame) -> None:
+def _save_background(path: str, flat: FlatForest, frame: pd.DataFrame, **extra) -> None:
     """The raw columns of ``flat.all_features``: numerics as float64, categories as ``U`` strings with ``null__<name>`` telling
-    a string (0) from None (1) and NaN (2), which the encoder maps differently."""
-    arrays = {}
+    a string (0) from None (1) and NaN (2), which the encoder maps differently; ``extra`` arrays beside them."""
+    arrays = dict(extra)
     for name in flat.all_features:
         if name in flat.num_features:
             arrays[name] = frame[name].to_numpy(dtype=np.float64)
@@ -658,4 +720,10 @@ def load_model(path: str, devices=None, **kw) -> B200Model:
         background_path = os.path.join(path, BACKGROUND_FILE)
         if "explain_background" not in kw and os.path.exists(background_path):
             kw["explain_background"] = _load_background(background_path, flat)
+    mmd_path = os.path.join(path, MMD_FILE)
+    if "mmd_reference" not in kw and os.path.exists(mmd_path) and os.environ.get("B200_MMD", "gpu") != "off":
+        kw["mmd_reference"] = _load_background(mmd_path, flat)
+        with np.load(mmd_path, allow_pickle=False) as z:
+            sigma = float(z["mmd_sigma"])
+        kw["mmd_sigma"] = None if math.isnan(sigma) else sigma
     return B200Model(flat, devices=devices, drift=drift, outlier_blob=outlier_blob, **kw)

@@ -43,7 +43,7 @@ from fastapi import FastAPI, Request, Response
 from fastapi.exceptions import RequestValidationError
 from pydantic import ValidationError
 
-from . import dependence, importance
+from . import dependence, importance, mmd
 from .ingest import NativeRequestParser, parse_rows, rows_to_frame  # noqa: F401  (rows_to_frame re-exported)
 from .schema import ALL_FEATURES, LABELLED_ROWS, TARGET, LabelledApplicant, LoanApplicant, ModelOutput
 
@@ -312,6 +312,16 @@ def _dependence_problem(features, values, kind, grid_resolution) -> str | None:
     return None
 
 
+_MMD_PARAMETERS = [
+    {"name": "n_permutations", "in": "query", "required": False,
+     "schema": {"type": "integer", "minimum": 1, "maximum": mmd.MAX_PERMUTATIONS, "default": 100}},
+    {"name": "p_val", "in": "query", "required": False, "description": "drift when the permutation p-value is below it",
+     "schema": {"type": "number", "exclusiveMinimum": 0, "maximum": 1, "default": 0.05}},
+    {"name": "random_state", "in": "query", "required": False, "description": "seed of the permutations (numpy default_rng)",
+     "schema": {"type": "integer", "minimum": 0, "default": 0}},
+]
+
+
 def _unprocessable(detail: str) -> Response:
     return Response(content=json.dumps({"detail": detail}), status_code=422, media_type="application/json")
 
@@ -511,6 +521,31 @@ def create_app(model=None, loader=None) -> FastAPI:
                                for s, r in out.items()}}
 
         out = await asyncio.get_running_loop().run_in_executor(None, call)
+        return Response(content=json.dumps(out, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
+
+    @app.post("/drift/mmd", openapi_extra={"requestBody": _REQUEST_SCHEMA, "parameters": _MMD_PARAMETERS})
+    async def drift_mmd(request: Request):
+        """Has the joint distribution of the applicants moved?  The kernel two-sample (MMD) test of the batch against the
+        model's reference table, alibi-detect's MMDDrift on the classifier's input vectors: `distance` is the unbiased MMD^2,
+        `p_val` its permutation p-value, `is_drift` = p_val < `threshold`, and `distance_threshold` the permuted statistic
+        at that quantile.  Per-field tests (/predict's feature_drift_batch) cannot see a change in how fields move together;
+        this can.  501 when the model has no reference; 422 for fewer than 2 applicants, a bad parameter, or a request whose
+        permutations need more than 2^36 kernel pairs."""
+        q = request.query_params
+        try:
+            n_permutations, p_val, random_state = int(q.get("n_permutations", "100")), float(q.get("p_val", "0.05")), int(q.get("random_state", "0"))
+        except ValueError:
+            return _unprocessable("n_permutations and random_state must be integers and p_val a number")
+        m = ml_models["credit_default"]
+        if not getattr(m, "mmd_reference_attached", False):
+            return Response(content=json.dumps({"detail": "this model has no MMD reference"}), status_code=501, media_type="application/json")
+        input_df = parser.frame(await request.body())
+        try:
+            mmd.check_request(len(input_df), m.mmd_reference_rows, n_permutations, p_val, random_state)
+        except ValueError as e:
+            return _unprocessable(str(e))
+        out = await asyncio.get_running_loop().run_in_executor(
+            None, lambda: m.mmd_drift(input_df, n_permutations=n_permutations, p_val=p_val, random_state=random_state))
         return Response(content=json.dumps(out, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
 
     @app.post("/predict", response_model=ModelOutput, openapi_extra={"requestBody": _REQUEST_SCHEMA})

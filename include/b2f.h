@@ -446,6 +446,39 @@ int b2f_permutation_scores(b2f_model *m, const void *rows, int64_t n, int row_fo
                            const int32_t *words, int n_words, struct b2f_perm_score *out /* [n_words][n_repeats] */,
                            struct b2f_perm_score *baseline, float *device_ms);
 
+/* ---- MMD drift test (csrc/mmd_drift.cuh) ----
+ * alibi-detect's MMDDrift (kernel two-sample test, permutation p-value) of a batch against a reference table.  A row is
+ * embedded as the classifier's input vector: its category codes (one-hot; -1 = the all-zero block) and its numerics as
+ * scored (float32, NaN = the blob's training median) z-scored in float64, z = (v - num_mean[k]) / num_scale[k].  The squared
+ * distance is sum_num (z_a - z_b)^2 + per categorical 2 (both known, different), 1 (one unknown) or 0; the kernel is
+ * k = exp(-d / (2 sigma^2)).
+ *
+ * b2f_model_attach_mmd_reference embeds n_ref rows (B2F_ROWS_WORDS24 or B2F_ROWS_PACKED64, host memory), sets sigma
+ * (NaN: alibi's median heuristic, sigma^2 = v / 2 with v the floor((P - 1) / 2)-th smallest, 0-based, of the P = n_ref
+ * (n_ref - 1) / 2 pair distances, found by an exact radix select) into *sigma_out, and keeps the embedding and the
+ * reference's kernel row sums on the device; it replaces an earlier reference (none is left when it fails).
+ * num_mean / num_scale: n_num doubles, finite, scale > 0.
+ *
+ * b2f_mmd_drift scores a batch of m rows against it.  The pool is [reference; batch], N = n_ref + m indices, s = min(m, n_ref).
+ * subsets: n_perm x s pool indices, each subset strictly increasing: the batch-sized side of a split when m <= n_ref, else
+ * the reference-sized side.  *mmd2_obs gets the unbiased statistic (zero diagonal) of the split [reference | batch] and
+ * mmd2_perm[b] that of subset b's split:  mmd^2 = S_XX / (n (n - 1)) + S_YY / (m (m - 1)) - 2 S_XY / (n m), the S over distinct
+ * pairs.  The observed split is computed as one more subset, so a subset equal to it gives the same bits.  Float64
+ * throughout, no float atomics: results are bit-identical from run to run and across the two row formats.
+ *
+ * Limits and errors: 2 <= n_ref <= B2F_MMD_MAX_REF, m >= 2 (n_ref + m < 2^31), 1 <= n_perm <= B2F_MMD_MAX_PERM.  B2F_EINVAL for
+ * ranked rows, a row count out of range, a subset index outside the pool, an unsorted or repeated subset, a non-finite mean
+ * or scale, a scale <= 0, a sigma that is not NaN, finite and positive, a median distance of 0 (pass sigma), or a NULL pointer;
+ * B2F_ESTATE (b2f_mmd_drift) without a reference; B2F_ENOMEM with the byte count when a device buffer cannot be allocated
+ * (the subset tile sums take (n_perm + 1) * ceil(s / 128)^2 doubles).  device_ms (may be NULL): from the first upload to the
+ * last copy back, CUDA events on the compute stream. */
+#define B2F_MMD_MAX_REF 131072
+#define B2F_MMD_MAX_PERM 10000
+int b2f_model_attach_mmd_reference(b2f_model *m, const void *rows, int64_t n, int row_format, const double *num_mean, const double *num_scale,
+                                   double sigma, double *sigma_out, float *device_ms);
+int b2f_mmd_drift(b2f_model *m, const void *rows, int64_t n, int row_format, const int32_t *subsets, int n_perm, double *mmd2_obs,
+                  double *mmd2_perm, float *device_ms);
+
 /* asynchronous form for the request-batching ring: buffers must be pinned and stay valid until
  * b2f_wait(ticket) returns.  proba_is_f64 selects double (1) or float (0) outputs. */
 int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned,
