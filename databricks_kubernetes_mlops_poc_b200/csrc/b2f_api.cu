@@ -35,6 +35,7 @@
 #include "partial_dependence.cuh"
 #include "counterfactual.cuh"
 #include "permutation_importance.cuh"
+#include "pair_dependence.cuh"
 #include "mmd_drift.cuh"
 #include "tree_shap.cuh"
 #include "tree_shap_interactions.cuh"
@@ -168,6 +169,17 @@ struct Dependence {
     DevBuf device_spec;         /* the device form's: a host call never overwrites a spec an enqueued device-form launch reads */
 };
 
+/* two-way partial dependence (b2f_pair_dependence; pair_dependence.cuh): the current call's spec (PpSeg table, then two
+ * words per point); the mean form's rows, partial sums and means, on the compute stream, grown on demand and kept */
+struct PairDependence {
+    int n_segs = 0;
+    int64_t points = 0;
+    std::vector<uint32_t> spec;
+    DevBuf host_spec; /* a curve call's spec, read by its host job's chunks */
+    DevBuf spec_dev;  /* the spec of the mean form and of the device form, written on the compute stream */
+    DevBuf rows, partial, out;
+};
+
 /* nearest single-field counterfactuals (b2f_counterfactual; counterfactual.cuh).  The split-value table is built on the
  * first call; the forest fields of cp are set at model creation, the probe fields are the current call's. */
 struct Counterfactual {
@@ -244,6 +256,7 @@ struct b2f_model {
     int64_t forest_bytes = 0;
     Explainer *ex = nullptr; /* attached TreeSHAP path table (b2f_model_attach_explainer) */
     Dependence pd;
+    PairDependence pair;
     Counterfactual cf;
     Importance pi;
     Mmd mmd;
@@ -892,6 +905,7 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
         if (sl.stream) cudaStreamDestroy(sl.stream);
     }
     for (DevBuf *b : {&m->scratch, &m->pd.host_spec, &m->pd.device_spec, &m->cf.dev, &m->mom_rows, &m->gather, &m->flush}) b->release();
+    for (DevBuf *b : {&m->pair.host_spec, &m->pair.spec_dev, &m->pair.rows, &m->pair.partial, &m->pair.out}) b->release();
     for (DevBuf *b : {&m->pi.rows, &m->pi.labels, &m->pi.perm, &m->pi.keys, &m->pi.flags, &m->pi.temp, &m->pi.offsets, &m->pi.segs, &m->pi.scores}) b->release();
     for (DevBuf *b : {&m->mmd.ref_z, &m->mmd.ref_c, &m->mmd.r_ref, &m->mmd.rows, &m->mmd.z, &m->mmd.c, &m->mmd.r, &m->mmd.partial, &m->mmd.sub,
                       &m->mmd.pairs, &m->mmd.out, &m->mmd.hist})
@@ -1752,6 +1766,9 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
 
 /* ------------------------------------------------------------------ partial dependence (K6) */
 #include "dependence_api.cuh"
+
+/* ------------------------------------------------------------------ two-way partial dependence (K10) */
+#include "pair_dependence_api.cuh"
 
 /* ------------------------------------------------------------------ counterfactuals (K7) */
 #include "counterfactual_api.cuh"

@@ -261,6 +261,32 @@ class ForestEngine:
         check(self._lib.b2f_partial_dependence_device(self._h, rows_dev, n, fmt, ptr(pr), len(pr), ptr(grid), out_dev),
               "b2f_partial_dependence_device")
 
+    # ------------------------------------------------------------------ two-way partial dependence (csrc/pair_dependence.cuh)
+    def pair_dependence_rows(self, rows: np.ndarray, probes, point_words: np.ndarray, mean: bool = False, device_ms: bool = False):
+        """Encoded rows (N, 24) or packed (N, 16), probes [(word a, word b or -1, point offset, count)] and the points' row
+        words (P', 2) -> float64 (N, sum of counts), or with ``mean`` (sum of counts,) [, device ms]: each point's score of
+        every row with word a set to the point's first word and word b to its second (a probe's points concatenated in
+        probe order), or its mean over the rows, taken on the device."""
+        rows = np.ascontiguousarray(rows)
+        pr = _pair_probe_table(probes)
+        words = np.ascontiguousarray(point_words, dtype=np.uint32).reshape(-1, 2)
+        P = int(pr["count"].sum())
+        out = np.empty(P if mean else (rows.shape[0], P), dtype=np.float64)
+        ms = C.c_float(0.0)
+        check(self._lib.b2f_pair_dependence(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(pr), len(pr), ptr(words), int(bool(mean)),
+                                            ptr(out), C.byref(ms)), "b2f_pair_dependence")
+        return (out, ms.value) if device_ms else out
+
+    def pair_dependence_device(self, rows_dev: int, n: int, probes, point_words: np.ndarray, out_dev: int, mean: bool = False,
+                               fmt: int = ROWS_WORDS24) -> None:
+        """Enqueue the two-way curves (n x sum of counts doubles) or, with ``mean``, their means (sum of counts doubles) of
+        device-resident rows into device out; probes and point words are host arrays, as for ``pair_dependence_rows``;
+        ``sync`` waits."""
+        pr = _pair_probe_table(probes)
+        words = np.ascontiguousarray(point_words, dtype=np.uint32).reshape(-1, 2)
+        check(self._lib.b2f_pair_dependence_device(self._h, rows_dev, n, fmt, ptr(pr), len(pr), ptr(words), int(bool(mean)), out_dev),
+              "b2f_pair_dependence_device")
+
     # ------------------------------------------------------------------ counterfactuals (csrc/counterfactual.cuh)
     def counterfactual_rows(self, rows: np.ndarray, words, cutoff: float = 0.5, device_ms: bool = False):
         """Encoded rows (N, 24) or packed (N, 16) and numeric row words -> (proba float64 (N,), records (N, len(words)) of
@@ -539,6 +565,11 @@ def blob_split_values(blob: bytes, word: int) -> np.ndarray:
 def _probe_table(probes) -> np.ndarray:
     """[(row word, grid offset, count)] -> b2f_pd_probe records."""
     return np.array([tuple(int(v) for v in p) for p in probes], dtype=_cabi.PD_PROBE_DTYPE)
+
+
+def _pair_probe_table(probes) -> np.ndarray:
+    """[(word a, word b or -1, point offset, count)] -> b2f_pair_probe records."""
+    return np.array([tuple(int(v) for v in p) for p in probes], dtype=_cabi.PAIR_PROBE_DTYPE)
 
 
 def moments_merge(parts: np.ndarray) -> np.ndarray:

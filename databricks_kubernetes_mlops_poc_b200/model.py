@@ -29,7 +29,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pandas as pd
 
-from . import dependence, importance, mmd
+from . import dependence, importance, interaction, mmd
 from ._cabi import OUT_F64, OUT_FULL, ROWS_PACKED64, ROWS_WORDS24, B2FError
 from ._pylists import ListBuilder
 from .encode import RowEncoder
@@ -307,6 +307,103 @@ class B200Model:
             out = self.engine.partial_dependence_rows(rows, probes, np.concatenate(words))
         res = {"feature_names": features, "output": "probability", "grid_values": grids}
         res.update(dependence.split_output(out, [len(g) for g in grids], kind))
+        return res
+
+    def pair_grids(self, model_input, pairs, *, grid_resolution: int = 100, percentiles=(0.05, 0.95), custom_values: dict | None = None,
+                   grid_frame: pd.DataFrame | None = None) -> list:
+        """The two grids of each pair ``pair_dependence`` probes: ``custom_values[f]`` when given, else the default rule of
+        ``dependence.grid_from_column`` over ``grid_frame``'s column, or ``model_input``'s.  ValueError for an unknown field,
+        a pair of one field, or an axis outside 1..256 points."""
+        pairs = interaction.check_pairs(pairs, self.all_features)
+        custom_values = dict(custom_values or {})
+        unknown = [f for f in custom_values if f not in self.all_features]
+        if unknown:
+            raise ValueError(f"custom_values for unknown feature(s) {unknown}")
+        source = model_input if grid_frame is None else grid_frame
+        source = source if isinstance(source, pd.DataFrame) else pd.DataFrame(source)
+        cache, out = {}, []
+        for pair in pairs:
+            for name in pair:
+                if name in cache:
+                    continue
+                if name in custom_values:
+                    grid = list(custom_values[name])
+                else:
+                    grid = dependence.grid_from_column(source[name], name in self.categorical_features, grid_resolution, percentiles).tolist()
+                if not 1 <= len(grid) <= interaction.MAX_AXIS_POINTS:
+                    raise ValueError(f"feature {name!r}: {len(grid)} grid points, expected 1..{interaction.MAX_AXIS_POINTS}")
+                cache[name] = grid
+            out.append([cache[pair[0]], cache[pair[1]]])
+        return out
+
+    def pair_dependence(self, model_input, pairs, *, kind: str = "average", grid_resolution: int = 100, percentiles=(0.05, 0.95),
+                        custom_values: dict | None = None, grid_frame: pd.DataFrame | None = None) -> dict:
+        """Two-way partial dependence of pairs of request fields: per pair ``(a, b)``, what scikit-learn's
+        ``partial_dependence(pipeline, model_input, [a, b], kind=..., method="brute", categorical_features=...)`` returns.
+
+        -> ``{"feature_names": pairs, "output": "probability", "grid_values": [[grid a, grid b] per pair], "average": [float64
+        (G_a, G_b)], "individual": [float64 (n, G_a, G_b)]}``: ``individual[p][i, u, v]`` is P(class 1) for row i with field
+        a set to ``grid_values[p][0][u]`` and b to ``grid_values[p][1][v]``, bit for bit the tile kernel's score of that
+        row; ``average`` (kind "average" or "both") is its mean over the rows, taken on the device in a fixed order (never
+        copying the curves), ``individual`` is there for "individual" and "both".  Grids follow ``pair_grids``: at most 256
+        points per axis.  ``pairs``: one pair or a list of them.  Every model has it; rows with NaN numerics are accepted
+        (the classifier alone is scored).  It runs on the first GPU's handle only, under ``replicas[0].lock``."""
+        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
+        if len(df.columns) == 0:
+            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        if kind not in dependence.KINDS:
+            raise ValueError(f"kind={kind!r}: expected one of {dependence.KINDS}")
+        pairs = interaction.check_pairs(pairs, self.all_features)
+        grids = self.pair_grids(df, pairs, grid_resolution=grid_resolution, percentiles=percentiles, custom_values=custom_values,
+                                grid_frame=grid_frame)
+        if len(df) == 0:
+            raise ValueError("pair dependence needs at least one row")
+        probes, points, off = [], [], 0
+        for (a, b), (ga, gb) in zip(pairs, grids):
+            pts = interaction.cartesian(dependence.encode_grid(self.encoder, a, ga), dependence.encode_grid(self.encoder, b, gb))
+            probes.append((dependence.word_of(self.encoder, a), dependence.word_of(self.encoder, b), off, len(pts)))
+            points.append(pts)
+            off += len(pts)
+        rows = self.encoder.encode_frame(df)
+        res = {"feature_names": pairs, "output": "probability", "grid_values": grids}
+        shapes = [(len(ga), len(gb)) for ga, gb in grids]
+        with self.replicas[0].lock:
+            if kind in ("average", "both"):
+                means = self.engine.pair_dependence_rows(rows, probes, np.concatenate(points), mean=True)
+                res["average"] = [means[p[2]:p[2] + p[3]].reshape(s) for p, s in zip(probes, shapes)]
+            if kind in ("individual", "both"):  # one call per pair: a call's curves hold at most 65 536 points per row
+                res["individual"] = [self.engine.pair_dependence_rows(rows, [(p[0], p[1], 0, p[3])], pts).reshape((len(df),) + s)
+                                     for p, pts, s in zip(probes, points, shapes)]
+        return res
+
+    def interaction_strength(self, model_input, features=None, *, sample: int = interaction.DEFAULT_SAMPLE, random_state: int = 0) -> dict:
+        """Which pairs of request fields interact, across the applicants: Friedman's H-statistic H^2 of every pair of
+        ``features`` (default: every field, in field order) over a sample S of the rows (every row when there are at most
+        ``sample``, else ``RandomState(random_state).choice(n, sample, replace=False)``); the formula is in
+        ``interaction.py``, with f = P(class 1) as ``partial_dependence`` scores it.
+
+        -> ``{"pairs": [(a, b)] in itertools.combinations order, "h_squared", "numerator", "denominator": float64 (pairs,),
+        "matrix": float64 (F, F) symmetric with a NaN diagonal, "feature_names", "rows": |S|}``; H^2 is NaN where the
+        denominator is 0, and unstable where F_jk is nearly flat (hence the numerator and denominator).  One device call
+        scores the distinct (x_j, x_k) of S per pair and the distinct x_j per field, each as a mean over S; centring and
+        sums are float64 numpy in a fixed order.  ValueError for an unknown or repeated field, fewer than two fields, a
+        sample outside 2..10 000, a bad seed or fewer than two rows.  It runs on the first GPU's handle only, under
+        ``replicas[0].lock``."""
+        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
+        if len(df.columns) == 0:
+            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        features = interaction.check_features(features, self.all_features)
+        sample, random_state = interaction.check_sample(sample, random_state)
+        S = interaction.sample_rows(len(df), sample, random_state)
+        rows = self.encoder.encode_frame(df.iloc[S].reset_index(drop=True))
+        n_cat, n_num = len(self.categorical_features), len(self.numeric_features)
+        words = interaction.impute(rows, n_cat, n_num, parse_header(self.flat.blob)["impute"])
+        fields = [dependence.word_of(self.encoder, f) for f in features]
+        probes, points, maps = interaction.strength_plan(words, fields, [f in self.categorical_features for f in features])
+        with self.replicas[0].lock:
+            means = self.engine.pair_dependence_rows(rows, probes, points, mean=True)
+        res = interaction.strength_result(means, maps, features)
+        res["rows"] = len(S)
         return res
 
     def counterfactuals(self, model_input, features=None, *, cutoff: float = 0.5) -> dict:

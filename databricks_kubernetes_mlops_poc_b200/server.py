@@ -43,7 +43,7 @@ from fastapi import FastAPI, Request, Response
 from fastapi.exceptions import RequestValidationError
 from pydantic import ValidationError
 
-from . import dependence, importance, mmd
+from . import dependence, importance, interaction, mmd
 from .ingest import NativeRequestParser, parse_rows, rows_to_frame  # noqa: F401  (rows_to_frame re-exported)
 from .schema import ALL_FEATURES, LABELLED_ROWS, TARGET, LabelledApplicant, LoanApplicant, ModelOutput
 
@@ -217,6 +217,60 @@ _DEPENDENCE_PARAMETERS = [
      "description": "explicit grid point of the one probed field; repeat for several; empty = missing",
      "schema": {"type": "array", "items": {"type": "string"}}, "style": "form", "explode": True},
 ]
+
+
+_PAIR_PARAMETERS = [
+    {"name": "feature", "in": "query", "required": True, "description": "the two request fields of the pair, in order: exactly two, distinct",
+     "schema": {"type": "array", "items": {"type": "string"}, "minItems": 2, "maxItems": 2}, "style": "form", "explode": True},
+    {"name": "kind", "in": "query", "required": False, "schema": {"type": "string", "enum": list(dependence.KINDS), "default": "average"}},
+    {"name": "grid_resolution", "in": "query", "required": False,
+     "schema": {"type": "integer", "minimum": 2, "maximum": interaction.MAX_AXIS_POINTS, "default": dependence.DEFAULT_RESOLUTION}},
+]
+
+_STRENGTH_PARAMETERS = [
+    {"name": "feature", "in": "query", "required": False, "description": "request field; repeat for several (at least 2), each at most once; none = every field",
+     "schema": {"type": "array", "items": {"type": "string"}}, "style": "form", "explode": True},
+    {"name": "sample", "in": "query", "required": False, "description": "rows of the sample the statistic is taken over",
+     "schema": {"type": "integer", "minimum": 2, "maximum": interaction.MAX_SAMPLE, "default": interaction.DEFAULT_SAMPLE}},
+    {"name": "random_state", "in": "query", "required": False, "description": "seed of the sample (numpy RandomState)",
+     "schema": {"type": "integer", "minimum": 0, "maximum": 2**32 - 1, "default": 0}},
+]
+
+
+def _pair_problem(features, kind, grid_resolution) -> str | None:
+    """Why a /explain/dependence/pair query is unprocessable, or None."""
+    if len(features) != 2:
+        return "exactly two feature parameters are needed"
+    unknown = [f for f in features if f not in ALL_FEATURES]
+    if unknown:
+        return f"unknown feature(s) {unknown}"
+    if features[0] == features[1]:
+        return "the two features must differ"
+    if kind not in dependence.KINDS:
+        return f"kind must be one of {list(dependence.KINDS)}"
+    if grid_resolution < 2:
+        return "grid_resolution must be at least 2"
+    if grid_resolution > interaction.MAX_AXIS_POINTS:
+        return f"at most {interaction.MAX_AXIS_POINTS} grid points per feature"
+    return None
+
+
+def _strength_problem(features, sample: str, random_state: str) -> str | None:
+    """Why a /explain/interaction_strength query is unprocessable, or None."""
+    try:
+        interaction.check_features(features or None, ALL_FEATURES)
+    except ValueError as e:
+        return str(e)
+    try:
+        interaction.check_sample(int(sample), int(random_state))
+    except ValueError:
+        return f"sample must be an integer in 2..{interaction.MAX_SAMPLE} and random_state an integer in [0, 2**32 - 1]"
+    return None
+
+
+def _nullable(a) -> list:
+    """A float array for JSON: NaN -> null."""
+    return [None if v != v else v for v in np.asarray(a, dtype=np.float64).tolist()]
 
 
 _COUNTERFACTUAL_PARAMETERS = [
@@ -459,6 +513,72 @@ def create_app(model=None, loader=None) -> FastAPI:
                 if key in out:
                     body[key] = [np.asarray(a, dtype=np.float64).tolist() for a in out[key]]
             return body
+
+        return await answered(request, call)
+
+    @app.post("/explain/dependence/pair", openapi_extra={"requestBody": _REQUEST_SCHEMA, "parameters": _PAIR_PARAMETERS})
+    async def explain_dependence_pair(request: Request):
+        """How the score moves when two fields change together: two-way partial dependence.  For each point (u, v) of the
+        two fields' grids (their Cartesian product, the first field slowest), each applicant's default probability with
+        the first field set to u and the second to v (`individual`, applicants x u x v) and their mean over the applicants
+        (`average`, u x v).  Grids as /explain/dependence: the model's background set when it has one, else the request
+        rows.  422 for other than two distinct known fields, a bad kind, grid_resolution < 2, an axis of more than 256
+        points, or an `individual` of more than 2^24 values."""
+        q = request.query_params
+        features, kind = q.getlist("feature"), q.get("kind", "average")
+        try:
+            grid_resolution = int(q.get("grid_resolution", dependence.DEFAULT_RESOLUTION))
+        except ValueError:
+            return _unprocessable("grid_resolution must be an integer")
+        problem = _pair_problem(features, kind, grid_resolution)
+        if problem:
+            return _unprocessable(problem)
+        pair = (features[0], features[1])
+
+        def call(m, input_df):
+            kw = {"grid_resolution": grid_resolution}
+            if getattr(m, "background_attached", False):
+                grids = m.dependence_grids if grid_resolution == dependence.DEFAULT_RESOLUTION else {}
+                kw["custom_values"] = {f: grids[f] for f in pair if f in grids}
+                kw["grid_frame"] = m.background
+            try:
+                (ga, gb), = m.pair_grids(input_df, [pair], **kw)
+            except ValueError as e:
+                return _unprocessable(str(e))
+            if kind != "average" and len(input_df) * len(ga) * len(gb) > interaction.MAX_INDIVIDUAL_VALUES:
+                return _unprocessable(f"individual would hold {len(input_df) * len(ga) * len(gb)} values, more than 2^24")
+            out = m.pair_dependence(input_df, [pair], kind=kind, custom_values={pair[0]: ga, pair[1]: gb})
+            body = {"feature_names": list(pair), "output": out["output"],
+                    "grid_values": [[_json_value(v) for v in g] for g in out["grid_values"][0]]}
+            for key in ("average", "individual"):
+                if key in out:
+                    body[key] = np.asarray(out[key][0], dtype=np.float64).tolist()
+            return body
+
+        return await answered(request, call)
+
+    @app.post("/explain/interaction_strength", openapi_extra={"requestBody": _REQUEST_SCHEMA, "parameters": _STRENGTH_PARAMETERS})
+    async def explain_interaction_strength(request: Request):
+        """Which pairs of fields interact across the applicants: Friedman's H-statistic H^2 of every pair of the `feature`
+        fields (every field without one), over a sample of at most `sample` applicants (numpy RandomState(random_state)
+        when there are more).  H^2 is the share of the pair's two-way partial dependence that the two one-way ones do not
+        explain: 0 for fields that act additively.  The answer lists the pairs, `h_squared` with its `numerator` and
+        `denominator` (H^2 is unstable where the denominator is small), the symmetric `matrix` and the sample size `rows`;
+        null where the denominator is 0.  422 for an unknown or repeated field, fewer than 2 fields, a bad sample or
+        random_state, or fewer than 2 applicants."""
+        q = request.query_params
+        features, sample, random_state = q.getlist("feature"), q.get("sample", str(interaction.DEFAULT_SAMPLE)), q.get("random_state", "0")
+        problem = _strength_problem(features, sample, random_state)
+        if problem:
+            return _unprocessable(problem)
+
+        def call(m, input_df):
+            if len(input_df) < 2:
+                return _unprocessable(f"interaction strength needs at least 2 rows, got {len(input_df)}")
+            out = m.interaction_strength(input_df, features or None, sample=int(sample), random_state=int(random_state))
+            return {"feature_names": list(out["feature_names"]), "rows": int(out["rows"]), "pairs": [list(p) for p in out["pairs"]],
+                    "h_squared": _nullable(out["h_squared"]), "numerator": _nullable(out["numerator"]),
+                    "denominator": _nullable(out["denominator"]), "matrix": [_nullable(r) for r in out["matrix"]]}
 
         return await answered(request, call)
 

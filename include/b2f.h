@@ -383,6 +383,40 @@ int b2f_partial_dependence(b2f_model *m, const void *rows, int64_t n, int row_fo
 int b2f_partial_dependence_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const b2f_pd_probe *probes, int n_probes,
                                   const uint32_t *grid_words, double *out_dev);
 
+/* ---- two-way partial dependence (csrc/pair_dependence.cuh) ----
+ * sklearn's two-way partial_dependence(method="brute"): for row i and each point (u, v) of a probe, the model's output
+ * (b2f_predict_f64's proba1) for row i with row word word_a replaced by u and row word word_b by v.  A probe with word_b =
+ * -1 is one-way (its points' second words are ignored).  point_words holds two words per point (a's, then b's), with
+ * b2f_partial_dependence's grid-word semantics (category code, -1 = unknown; float32 bits, NaN = missing, imputed with the
+ * training median); a probe reads points point_offset .. point_offset + count - 1, i.e. point_words[2 * point_offset ..).
+ * The call's P points are its probes' points, concatenated in probe order.
+ *   mean = 0: out gets n x P doubles, row-major; each point equals, bit for bit, the tile kernel's score of the substituted
+ *             row.  Pipelined over the model's streams like b2f_partial_dependence, in chunks of at most 64 MB of output.
+ *   mean = 1: out gets P doubles, each point's mean over the n rows: per 128-row CTA a fixed-order sum of those scores,
+ *             then the CTA sums in order, divided by n.  The rows go to the device once per call, on the compute stream,
+ *             into buffers the model keeps; the per-CTA sums of a group of points stay under B2F_PERM_SCRATCH_BYTES.
+ * No atomics: results are bit-identical from run to run, and a point's value does not depend on the other points of the
+ * call.  Errors: B2F_EINVAL for ranked rows, n < 0 (mean = 1: n < 1), a NULL pointer, mean not 0 or 1, more than
+ * B2F_PAIR_MAX_PROBES probes, a word outside the fields, word_a == word_b, a count outside 1..B2F_PAIR_MAX_POINTS, a point
+ * range past B2F_PAIR_MAX_PROBES * B2F_PAIR_MAX_POINTS points, mean = 0 with P > B2F_PAIR_MAX_CURVE_POINTS, a category code
+ * outside [-1, vocabulary) or a forest deeper than 32 levels; B2F_ERANGE for an infinite numeric point word; B2F_ENOMEM
+ * (with the byte count) when a buffer of the mean form cannot be allocated.  device_ms (may be NULL): as b2f_explain
+ * (mean = 0), or from the first upload to the copy back, CUDA events on the compute stream (mean = 1). */
+#define B2F_PAIR_MAX_POINTS 65536
+#define B2F_PAIR_MAX_PROBES 276 /* 253 pairs and 23 single fields of the credit schema */
+#define B2F_PAIR_MAX_CURVE_POINTS 65536
+typedef struct b2f_pair_probe {
+    int32_t word_a, word_b;  /* row words; word_b = -1: one-way */
+    int32_t point_offset;    /* first point in point_words (2 words per point) */
+    int32_t count;           /* points: 1 .. B2F_PAIR_MAX_POINTS */
+} b2f_pair_probe;
+int b2f_pair_dependence(b2f_model *m, const void *rows, int64_t n, int row_format, const b2f_pair_probe *probes, int n_probes,
+                        const uint32_t *point_words, int mean, double *out, float *device_ms);
+/* device-resident form: rows_dev and out_dev in device memory, probes and point_words in host memory; enqueued on the
+ * compute stream (asynchronous, like b2f_partial_dependence_device; b2f_sync waits) */
+int b2f_pair_dependence_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const b2f_pair_probe *probes, int n_probes,
+                               const uint32_t *point_words, int mean, double *out_dev);
+
 /* ---- nearest single-field counterfactuals (csrc/counterfactual.cuh) ----
  * "What is the smallest change to this one field that changes the decision?"  For row i and probed numeric row word w with
  * the forest's split values t'_0 < ... < t'_{m-1} (b2f_blob_split_values), every float32 value of a piece [t'_{k-1}, t'_k)
