@@ -37,6 +37,7 @@
 #include "permutation_importance.cuh"
 #include "pair_dependence.cuh"
 #include "mmd_drift.cuh"
+#include "knn.cuh"
 #include "tree_shap.cuh"
 #include "tree_shap_interactions.cuh"
 #include "tree_shap_interventional.cuh"
@@ -212,6 +213,17 @@ struct Mmd {
     DevBuf r, partial, sub, pairs, out, hist;
 };
 
+/* the k-nearest reference search of trust scores (b2f_model_attach_knn_reference / b2f_knn; knn.cuh): the class-sorted
+ * reference's embedding and row map, kept between calls, and a call's buffers; all on the compute stream, grown on demand */
+struct Knn {
+    MmdParams mp;
+    int64_t n_ref = 0; /* 0: no reference */
+    int64_t n_cls[2] = {0, 0};
+    DevBuf ref_z, ref_c, orig; /* the reference: embedding (class 0 rows, then class 1) and position -> original row */
+    DevBuf rows, z, c;         /* a piece's rows and the queries' embedding */
+    DevBuf cand_d, cand_i, dist, index;
+};
+
 struct TicketRec {
     uint64_t id = 0;
     cudaEvent_t ev[B2F_STREAMS] = {nullptr, nullptr, nullptr, nullptr};
@@ -260,6 +272,7 @@ struct b2f_model {
     Counterfactual cf;
     Importance pi;
     Mmd mmd;
+    Knn knn;
     b2f_model *outlier = nullptr; /* attached isolation forest (b2f_model_attach_outlier_forest): a child handle on the
                                      same device whose kernels are launched on this handle's streams and rows */
     Slot slots[B2F_STREAMS];
@@ -909,6 +922,9 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
     for (DevBuf *b : {&m->pi.rows, &m->pi.labels, &m->pi.perm, &m->pi.keys, &m->pi.flags, &m->pi.temp, &m->pi.offsets, &m->pi.segs, &m->pi.scores}) b->release();
     for (DevBuf *b : {&m->mmd.ref_z, &m->mmd.ref_c, &m->mmd.r_ref, &m->mmd.rows, &m->mmd.z, &m->mmd.c, &m->mmd.r, &m->mmd.partial, &m->mmd.sub,
                       &m->mmd.pairs, &m->mmd.out, &m->mmd.hist})
+        b->release();
+    for (DevBuf *b : {&m->knn.ref_z, &m->knn.ref_c, &m->knn.orig, &m->knn.rows, &m->knn.z, &m->knn.c, &m->knn.cand_d, &m->knn.cand_i,
+                      &m->knn.dist, &m->knn.index})
         b->release();
     for (auto &t : m->tickets)
         for (auto &e : t.ev)
@@ -1778,3 +1794,6 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
 
 /* ------------------------------------------------------------------ MMD drift test (K9) */
 #include "mmd_api.cuh"
+
+/* ------------------------------------------------------------------ k-nearest reference rows of trust scores (K11) */
+#include "knn_api.cuh"

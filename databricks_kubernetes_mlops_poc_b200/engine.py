@@ -53,6 +53,7 @@ class ForestEngine:
         self.explainer_attached = False
         self.background_rows = 0
         self.mmd_reference_rows = 0
+        self.knn_class_rows = (0, 0)  # rows of each class in the attached trust reference
         inf = self.info()
         self.rank_words = inf["rank_row_bytes"] // 4 if inf["rank_ok"] else 0  # width of a ranked row, 0 = not available
 
@@ -359,6 +360,32 @@ class ForestEngine:
         check(self._lib.b2f_mmd_drift(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(sub), sub.shape[0], C.byref(obs), ptr(perm),
                                       C.byref(ms)), "b2f_mmd_drift")
         return (obs.value, perm, ms.value) if device_ms else (obs.value, perm)
+
+    # ------------------------------------------------------------------ k-nearest reference rows of trust scores (csrc/knn.cuh)
+    def attach_knn_reference(self, rows: np.ndarray, classes, num_mean, num_scale) -> None:
+        """Encoded reference rows (N, 24) or packed (N, 16), 2 <= N <= 131 072, their classes (0 / 1, each present) and the
+        per-numeric mean and scale of the embedding.  Replaces an earlier reference; a failed attach leaves none."""
+        rows = np.ascontiguousarray(rows)
+        cls = np.ascontiguousarray(classes, dtype=np.int32)
+        if cls.shape != (rows.shape[0],):
+            raise ValueError(f"classes must be ({rows.shape[0]},), not {cls.shape}")
+        mean = np.ascontiguousarray(num_mean, dtype=np.float64)
+        scale = np.ascontiguousarray(num_scale, dtype=np.float64)
+        self.knn_class_rows = (0, 0)
+        check(self._lib.b2f_model_attach_knn_reference(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(cls), ptr(mean), ptr(scale)),
+              "b2f_model_attach_knn_reference")
+        self.knn_class_rows = (int((cls == 0).sum()), int((cls == 1).sum()))
+
+    def knn(self, rows: np.ndarray, k: int, device_ms: bool = False):
+        """Encoded query rows (M, 24) or packed (M, 16), M >= 1 -> (float64 (M, 2, k) distances, int32 (M, 2, k) reference row
+        indices[, device ms]): per class the k nearest reference rows, ordered by (distance, index)."""
+        rows = np.ascontiguousarray(rows)
+        n = rows.shape[0]
+        dist = np.empty((n, 2, max(int(k), 0)), dtype=np.float64)
+        index = np.empty((n, 2, max(int(k), 0)), dtype=np.int32)
+        ms = C.c_float(0.0)
+        check(self._lib.b2f_knn(self._h, ptr(rows), n, self._fmt(rows), int(k), ptr(dist), ptr(index), C.byref(ms)), "b2f_knn")
+        return (dist, index, ms.value) if device_ms else (dist, index)
 
     # ------------------------------------------------------------------ device-resident interface
     def device_alloc(self, nbytes: int) -> int:

@@ -29,7 +29,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pandas as pd
 
-from . import dependence, importance, interaction, mmd
+from . import dependence, importance, interaction, mmd, trust
 from ._cabi import OUT_F64, OUT_FULL, ROWS_PACKED64, ROWS_WORDS24, B2FError
 from ._pylists import ListBuilder
 from .encode import RowEncoder
@@ -42,6 +42,8 @@ DRIFT_FILE = "drift_reference.npz"
 EXPLAIN_FILE = "explain.b2f"  # TreeSHAP path table (flatten_explainer); optional
 BACKGROUND_FILE = "explain_background.npz"  # background rows of interventional explanations (raw columns); optional
 MMD_FILE = "mmd_reference.npz"  # reference rows of the MMD drift test (raw columns, and its sigma); optional
+TRUST_FILE = "trust_reference.npz"  # labelled reference rows of trust scores (raw columns, labels, fit options); optional
+TRUST_TARGET = "default_payment_next_month"  # the label column a trust reference frame carries by default
 OUTLIER_PICKLE = os.path.join("artifacts", "outlier.pkl")  # joblib.dump(outlier, ".../outlier.pkl"), 02-register-model.ipynb:264,326-328
 SKLEARN_PICKLE = os.path.join("artifacts", "classifier", "model", "model.pkl")  # MLflow layout, 02-register-model.ipynb:317-321
 
@@ -49,7 +51,8 @@ SKLEARN_PICKLE = os.path.join("artifacts", "classifier", "model", "model.pkl")  
 class B200Model:
     def __init__(self, flat: FlatForest, devices=None, drift=None, outlier_blob: bytes | None = None, host_threads: int = 0,
                  explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None,
-                 mmd_reference: pd.DataFrame | None = None, mmd_sigma: float | None = None):
+                 mmd_reference: pd.DataFrame | None = None, mmd_sigma: float | None = None,
+                 trust_reference: pd.DataFrame | None = None, trust_options: dict | None = None):
         self.flat = flat
         self.all_features = flat.all_features
         self.categorical_features = list(flat.cat_features)
@@ -87,6 +90,10 @@ class B200Model:
         self.mmd_sigma = None  # the attached MMD reference's kernel width
         if mmd_reference is not None:
             self.attach_mmd_reference(mmd_reference, sigma=mmd_sigma)
+        self.trust_reference_rows = None  # rows kept per class of the attached trust reference
+        self._trust_positions = None  # attached reference row -> its position in the fitted frame
+        if trust_reference is not None:
+            self.attach_trust_reference(trust_reference, **(trust_options or {}))
 
     # ------------------------------------------------------------------ construction
     @classmethod
@@ -98,7 +105,8 @@ class B200Model:
         ``IsolationForest`` plus ``outlier_threshold=``), flattened into a second forest over the same rows.
         ``explain``: also build the TreeSHAP path table, so that ``explain()`` works.  ``background``: a frame of raw rows
         (e.g. the training table) to attach for ``explain_interventional()``; it needs ``explain``.  ``mmd_reference=frame``
-        (and ``mmd_sigma=``): the reference table of ``mmd_drift()``."""
+        (and ``mmd_sigma=``): the reference table of ``mmd_drift()``.  ``trust_reference=frame`` (and ``trust_options=``, the
+        keywords of ``attach_trust_reference``): the labelled reference of ``trust_score()``."""
         if background is not None and not explain:
             raise ValueError("a background is for interventional explanations: pass explain=True with it")
         flat = flatten_pipeline(pipeline)
@@ -559,6 +567,77 @@ class B200Model:
             obs, perm = self.engine.mmd_statistics(rows, subsets)
         return mmd.result(obs, perm, p_val, self.mmd_sigma, n_ref, len(df))
 
+    @property
+    def trust_reference_attached(self) -> bool:
+        return self.trust_reference_rows is not None
+
+    def attach_trust_reference(self, frame: pd.DataFrame, labels=None, *, k_filter: int = 10, alpha: float = 0.0, filter_type=None,
+                               dist_filter_type: str = "point") -> list:
+        """Fit alibi's ``TrustScore(k_filter, alpha, filter_type, dist_filter_type).fit(X, Y)`` on a labelled reference
+        (``trust.py``): 2..131 072 raw rows, encoded as requests are and embedded on the first GPU with the z-score constants of
+        their numerics, taken over the whole frame.  ``labels``: the model's classes per row (default: the frame's
+        ``default_payment_next_month`` column).  ``filter_type="distance_knn"`` drops, per class, the rows whose distance to
+        their ``k_filter``-th nearest same-class row ("point") or mean distance to the ``k_filter`` nearest ("mean") lies above
+        the ``(1 - alpha)`` percentile; its neighbours come from the same GPU search as the scores.  Replaces an earlier
+        reference.  -> the rows kept per class.  ValueError for a bad argument, a label outside the model's classes, or a class
+        with too few rows."""
+        frame = frame if isinstance(frame, pd.DataFrame) else pd.DataFrame(frame)
+        k_filter, alpha, filter_type, dist_filter_type = trust.check_fit(len(frame), k_filter, alpha, filter_type, dist_filter_type)
+        if labels is None:
+            if TRUST_TARGET not in frame.columns:
+                raise ValueError(f"pass labels, or a frame with a {TRUST_TARGET!r} column")
+            labels = frame[TRUST_TARGET].to_numpy()
+        if len(labels) != len(frame):
+            raise ValueError(f"{len(labels)} labels for {len(frame)} reference rows")
+        cls = trust.class_indices(labels, self.classes)
+        trust.check_class_rows(cls, filter_type, k_filter)
+        rows = self.encoder.encode_frame(frame)
+        n_cat, n_num = len(self.categorical_features), len(self.numeric_features)
+        impute = parse_header(self.flat.blob)["impute"][n_cat:n_cat + n_num]
+        mean, scale = mmd.standardization(mmd.numerics(rows, n_cat, n_num, impute))
+        positions = np.arange(len(frame))
+        self.trust_reference_rows, self._trust_positions = None, None
+        with self.replicas[0].lock:
+            self.engine.attach_knn_reference(rows, cls, mean, scale)
+            if filter_type == "distance_knn":
+                dist, _ = self.engine.knn(rows, k_filter + 1)
+                keep = np.zeros(len(frame), dtype=bool)
+                for c in (0, 1):
+                    own = cls == c
+                    keep[own] = trust.filter_keep(trust.filter_radius(dist[own, c, :], dist_filter_type), alpha)
+                positions = np.nonzero(keep)[0]
+                self.engine.attach_knn_reference(rows[positions], cls[positions], mean, scale)
+        kept = [int((cls[positions] == c).sum()) for c in (0, 1)]
+        self.trust_reference_rows, self._trust_positions = kept, positions
+        return kept
+
+    def trust_score(self, model_input, *, k: int = 2, dist_type: str = "point") -> dict:
+        """Can this decision be trusted?  alibi's ``TrustScore.score(X, Y, k, dist_type)`` with Y the classifier's own
+        predictions: per row, D_c is the k-th nearest distance ("point") or the mean of the k nearest distances ("mean") to
+        the attached reference rows of class c, and ``trust_score = D_other / (D_pred + 1e-12)``: below 1 the other class's
+        reference rows are nearer than the predicted class's.  -> ``{"trust_score", "closest_not_pred", "predictions": P(class
+        1), "labels": the predicted class, "distance_to_pred", "distance_to_other", "k", "dist_type", "reference_rows": rows
+        kept per class, "neighbours": per class {"class", "index": (n, k) positions in the fitted frame, "distance": (n, k)}}``,
+        neighbours ordered by (distance, position).  The classifier alone is scored, so NaN numerics are accepted.  It runs on
+        the first GPU's handle only, under ``replicas[0].lock``.  RuntimeError without a reference; ValueError for a bad k or
+        dist_type or no rows."""
+        if not self.trust_reference_attached:
+            raise RuntimeError("this model has no trust reference: attach_trust_reference(frame), from_pipeline(..., trust_reference=frame) "
+                               f"or a model directory that holds {TRUST_FILE} (save_model_dir(..., trust_reference=frame))")
+        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
+        if len(df.columns) == 0:
+            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        k, dist_type = trust.check_score(k, dist_type, self.trust_reference_rows)
+        if len(df) == 0:
+            raise ValueError("trust scores need at least one row")
+        rows = self.encoder.encode_frame(df)
+        with self.replicas[0].lock:
+            dist, index = self.engine.knn(rows, k)
+            proba, _ = self.replicas[0].score(df, want_outliers=False)
+            _, label = self.engine.predict_rows(rows)
+        return trust.result(dist, index, proba, label.astype(np.int64), self.classes, self._trust_positions, k, dist_type,
+                            self.trust_reference_rows)
+
     def explain_interventional(self, model_input) -> dict:
         """Exact interventional TreeSHAP contributions of every request field against the attached background set (what
         shap's ``TreeExplainer(model, data)`` computes): the mean, over background rows z, of each field's Shapley value in
@@ -692,11 +771,14 @@ class _Replica:
 # ---------------------------------------------------------------------- loading
 def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | None = None, outlier_blob: bytes | None = None,
                    explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None,
-                   mmd_reference: pd.DataFrame | None = None, mmd_sigma: float | None = None) -> None:
+                   mmd_reference: pd.DataFrame | None = None, mmd_sigma: float | None = None,
+                   trust_reference: pd.DataFrame | None = None, trust_options: dict | None = None) -> None:
     """Write the GPU-side artefact next to (or instead of) the MLflow pickles.  ``explain_blob``: the TreeSHAP path table
     (``flatten_explainer``), written as ``explain.b2f`` so that ``load_model`` attaches it.  ``explain_background``: raw
     rows written as ``explain_background.npz``, attached by ``load_model`` with the explainer.  ``mmd_reference``: raw rows
-    written as ``mmd_reference.npz`` with ``mmd_sigma`` (None: the median heuristic at load), attached by ``load_model``."""
+    written as ``mmd_reference.npz`` with ``mmd_sigma`` (None: the median heuristic at load), attached by ``load_model``.
+    ``trust_reference``: raw rows written as ``trust_reference.npz`` with their labels (``trust_options["labels"]``, else the
+    frame's ``default_payment_next_month``) and the other ``attach_trust_reference`` options, fitted by ``load_model``."""
     os.makedirs(path, exist_ok=True)
     flat.save(os.path.join(path, BLOB_FILE))
     if explain_blob is not None:
@@ -707,6 +789,19 @@ def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | 
     if mmd_reference is not None:
         sigma = mmd.check_sigma(mmd_sigma)
         _save_background(os.path.join(path, MMD_FILE), flat, mmd_reference, mmd_sigma=np.float64(np.nan if sigma is None else sigma))
+    if trust_reference is not None:
+        opts = dict(trust_options or {})
+        labels = opts.pop("labels", None)
+        unknown = set(opts) - {"k_filter", "alpha", "filter_type", "dist_filter_type"}
+        if unknown:
+            raise ValueError(f"unknown trust option(s) {sorted(unknown)}")
+        k_filter, alpha, filter_type, dist_filter_type = trust.check_fit(len(trust_reference), opts.get("k_filter", 10), opts.get("alpha", 0.0),
+                                                                         opts.get("filter_type"), opts.get("dist_filter_type", "point"))
+        labels = np.asarray(trust_reference[TRUST_TARGET] if labels is None else labels)
+        trust.class_indices(labels, flat.classes)
+        _save_background(os.path.join(path, TRUST_FILE), flat, trust_reference, trust_labels=labels, trust_k_filter=np.int64(k_filter),
+                         trust_alpha=np.float64(alpha), trust_filter_type=np.str_(filter_type or ""),
+                         trust_dist_filter_type=np.str_(dist_filter_type))
     if outlier_blob is not None:
         with open(os.path.join(path, OUTLIER_BLOB_FILE), "wb") as f:
             f.write(outlier_blob)
@@ -823,4 +918,10 @@ def load_model(path: str, devices=None, **kw) -> B200Model:
         with np.load(mmd_path, allow_pickle=False) as z:
             sigma = float(z["mmd_sigma"])
         kw["mmd_sigma"] = None if math.isnan(sigma) else sigma
+    trust_path = os.path.join(path, TRUST_FILE)
+    if "trust_reference" not in kw and os.path.exists(trust_path) and os.environ.get("B200_TRUST", "gpu") != "off":
+        kw["trust_reference"] = _load_background(trust_path, flat)
+        with np.load(trust_path, allow_pickle=False) as z:
+            kw["trust_options"] = {"labels": z["trust_labels"], "k_filter": int(z["trust_k_filter"]), "alpha": float(z["trust_alpha"]),
+                                   "filter_type": str(z["trust_filter_type"]) or None, "dist_filter_type": str(z["trust_dist_filter_type"])}
     return B200Model(flat, devices=devices, drift=drift, outlier_blob=outlier_blob, **kw)

@@ -43,7 +43,7 @@ from fastapi import FastAPI, Request, Response
 from fastapi.exceptions import RequestValidationError
 from pydantic import ValidationError
 
-from . import dependence, importance, interaction, mmd
+from . import dependence, importance, interaction, mmd, trust
 from .ingest import NativeRequestParser, parse_rows, rows_to_frame  # noqa: F401  (rows_to_frame re-exported)
 from .schema import ALL_FEATURES, LABELLED_ROWS, TARGET, LabelledApplicant, LoanApplicant, ModelOutput
 
@@ -376,6 +376,39 @@ _MMD_PARAMETERS = [
 ]
 
 
+_TRUST_PARAMETERS = [
+    {"name": "k", "in": "query", "required": False, "description": "neighbours per class: at most the rows the reference keeps in either class",
+     "schema": {"type": "integer", "minimum": 1, "maximum": trust.MAX_K, "default": 2}},
+    {"name": "dist_type", "in": "query", "required": False, "description": "D_c: the k-th nearest distance (point) or the mean of the k nearest",
+     "schema": {"type": "string", "enum": list(trust.DIST_TYPES), "default": "point"}},
+    {"name": "neighbours", "in": "query", "required": False, "description": "also answer each applicant's neighbours per class",
+     "schema": {"type": "boolean", "default": False}},
+]
+
+
+def _trust_problem(k: str, dist_type: str, neighbours: str) -> str | None:
+    """Why a /explain/trust query is unprocessable, or None (the k bound against the reference is the model's)."""
+    try:
+        k_ = int(k)
+    except ValueError:
+        return f"k must be an integer in 1..{trust.MAX_K}"
+    if not 1 <= k_ <= trust.MAX_K:
+        return f"k must be an integer in 1..{trust.MAX_K}"
+    if dist_type not in trust.DIST_TYPES:
+        return f"dist_type must be one of {list(trust.DIST_TYPES)}"
+    if neighbours not in ("true", "false"):
+        return "neighbours must be true or false"
+    return None
+
+
+def _finite_or_null(a) -> list:
+    """A float array for JSON: every value that is not a finite number (NaN, or a distance past float64's range) -> null."""
+    a = np.asarray(a, dtype=np.float64)
+    out = a.astype(object)
+    out[~np.isfinite(a)] = None
+    return out.tolist()
+
+
 def _unprocessable(detail: str) -> Response:
     return Response(content=json.dumps({"detail": detail}), status_code=422, media_type="application/json")
 
@@ -642,6 +675,41 @@ def create_app(model=None, loader=None) -> FastAPI:
 
         out = await asyncio.get_running_loop().run_in_executor(None, call)
         return Response(content=json.dumps(out, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
+
+    @app.post("/explain/trust", openapi_extra={"requestBody": _REQUEST_SCHEMA, "parameters": _TRUST_PARAMETERS})
+    async def explain_trust(request: Request):
+        """Can each decision be trusted?  alibi's trust score against the model's labelled reference: the distance from the
+        applicant to its k-th nearest reference applicant of the other class (`distance_to_other`) over the distance to its
+        k-th nearest of the predicted class (`distance_to_pred`), on the classifier's input vectors (one-hot categoricals,
+        z-scored numerics).  Below 1, applicants like this one mostly turned out the other way.  `labels` is the predicted
+        class, `closest_not_pred` the other one, `predictions` P(class 1).  With `neighbours=true`, per class the reference
+        rows found (positions in the reference frame) and their distances, nearest first.  null stands for a value that is
+        not a finite number.  501 when the model has no trust reference; 422 for a bad k, dist_type or neighbours."""
+        q = request.query_params
+        k, dist_type, neighbours = q.get("k", "2"), q.get("dist_type", "point"), q.get("neighbours", "false")
+        problem = _trust_problem(k, dist_type, neighbours)
+        if problem:
+            return _unprocessable(problem)
+        m = ml_models["credit_default"]
+        if not getattr(m, "trust_reference_attached", False):
+            return Response(content=json.dumps({"detail": "this model has no trust reference"}), status_code=501, media_type="application/json")
+        try:
+            trust.check_score(int(k), dist_type, m.trust_reference_rows)
+        except ValueError as e:
+            return _unprocessable(str(e))
+
+        def call(m, input_df):
+            out = m.trust_score(input_df, k=int(k), dist_type=dist_type)
+            body = {"trust_score": _finite_or_null(out["trust_score"]), "closest_not_pred": np.asarray(out["closest_not_pred"]).tolist(),
+                    "predictions": np.asarray(out["predictions"], dtype=np.float64).tolist(), "labels": np.asarray(out["labels"]).tolist(),
+                    "distance_to_pred": _finite_or_null(out["distance_to_pred"]), "distance_to_other": _finite_or_null(out["distance_to_other"]),
+                    "k": out["k"], "dist_type": out["dist_type"], "reference_rows": list(out["reference_rows"])}
+            if neighbours == "true":
+                body["neighbours"] = [{"class": nb["class"], "index": np.asarray(nb["index"]).tolist(), "distance": _finite_or_null(nb["distance"])}
+                                      for nb in out["neighbours"]]
+            return body
+
+        return await answered(request, call)
 
     @app.post("/drift/mmd", openapi_extra={"requestBody": _REQUEST_SCHEMA, "parameters": _MMD_PARAMETERS})
     async def drift_mmd(request: Request):

@@ -513,6 +513,32 @@ int b2f_model_attach_mmd_reference(b2f_model *m, const void *rows, int64_t n, in
 int b2f_mmd_drift(b2f_model *m, const void *rows, int64_t n, int row_format, const int32_t *subsets, int n_perm, double *mmd2_obs,
                   double *mmd2_perm, float *device_ms);
 
+/* ---- k-nearest reference rows of trust scores (csrc/knn.cuh) ----
+ * The exact k nearest rows of each class of a labelled reference, the half of alibi's TrustScore that needs the GPU.  The
+ * space is the MMD test's: a row is embedded as its category codes (one-hot; -1 = the all-zero block) and its numerics as
+ * scored (float32, NaN = the blob's training median) z-scored in float64, z = (v - num_mean[k]) / num_scale[k]; the squared
+ * distance d is sum_num (z_a - z_b)^2 in field order (separate multiplies and adds) plus per categorical 2 (both known,
+ * different), 1 (one unknown) or 0, and a NaN d (only infinite inputs make one) counts as +inf.
+ *
+ * b2f_model_attach_knn_reference embeds n rows (B2F_ROWS_WORDS24 or B2F_ROWS_PACKED64, host memory) with their classes
+ * cls[i] in {0, 1} and keeps them on the device; it replaces an earlier reference (none is left when it fails).
+ * num_mean / num_scale: n_num doubles, finite, scale > 0.
+ *
+ * b2f_knn finds, for each of n query rows and each class c, the k reference rows of class c nearest to it, ordered by
+ * (d, reference row index): ties go to the lower index.  dist[(i * 2 + c) * k + j] = sqrt(d) (correctly rounded) of the j-th,
+ * index[...] its row index in the reference as attached.  No float atomics: two calls give the same bytes, whatever the row
+ * format.  The queries are taken in pieces of at most 65 536 rows whose candidate scratch stays under 256 MiB.
+ *
+ * Limits and errors: 2 <= n_ref <= B2F_MMD_MAX_REF with at least one row per class, n >= 1, 1 <= k <= B2F_KNN_MAX_K and k at
+ * most the rows of either class.  B2F_EINVAL for ranked rows, a row count or k out of range, a class value other than 0 / 1,
+ * a class without rows, a non-finite mean or scale, a scale <= 0 or a NULL pointer; B2F_ESTATE (b2f_knn) without a reference;
+ * B2F_ENOMEM with the byte count when a device buffer cannot be allocated.  device_ms (may be NULL): from the first upload to
+ * the last copy back, CUDA events on the compute stream. */
+#define B2F_KNN_MAX_K 64
+int b2f_model_attach_knn_reference(b2f_model *m, const void *rows, int64_t n, int row_format, const int32_t *cls, const double *num_mean,
+                                   const double *num_scale);
+int b2f_knn(b2f_model *m, const void *rows, int64_t n, int row_format, int k, double *dist, int32_t *index, float *device_ms);
+
 /* asynchronous form for the request-batching ring: buffers must be pinned and stay valid until
  * b2f_wait(ticket) returns.  proba_is_f64 selects double (1) or float (0) outputs. */
 int b2f_predict_async(b2f_model *m, const void *rows_pinned, int64_t n, void *proba1_pinned,
