@@ -20,6 +20,8 @@
 
 #include <algorithm>
 #include <cmath>
+#include <limits>
+#include <mutex>
 #include <string>
 #include <thread>
 #include <new>
@@ -245,6 +247,7 @@ struct b2f_model {
     bool tile_ok = false;
     TParams tp;
     void *d_tile_layout = nullptr;
+    KParams *d_kp = nullptr; /* device copy of kp: the tile kernel re-decides rows inside the rounding band on it */
     TPiece *d_tile_pieces = nullptr;
     int tile_smem_bytes = 0;
     int tile_cwarps = B2F_TILE_WARPS_MIN;
@@ -457,13 +460,27 @@ static RankKernel<OutT> rank_kernel(const b2f_model *m) {
         return nullptr;
     } else {
         if (m->rp.depth != D) return rank_kernel<OutT, D + 1>(m);
-        if (m->rank_stream) return k_forest_predict_rank<D, 4, true, OutT>;
-        return m->rank_u == 8 ? k_forest_predict_rank<D, 8, false, OutT> : k_forest_predict_rank<D, 4, false, OutT>;
+        /* a GBDT has no exact re-decision (forest_decide.cuh): its instances carry none of that code */
+        if (m->hdr.agg_mode == B2F_AGG_GBDT_LOGISTIC) {
+            if (m->rank_stream) return k_forest_predict_rank<D, 4, true, false, OutT>;
+            return m->rank_u == 8 ? k_forest_predict_rank<D, 8, false, false, OutT> : k_forest_predict_rank<D, 4, false, false, OutT>;
+        }
+        if (m->rank_stream) return k_forest_predict_rank<D, 4, true, true, OutT>;
+        return m->rank_u == 8 ? k_forest_predict_rank<D, 8, false, true, OutT> : k_forest_predict_rank<D, 4, false, true, OutT>;
     }
 }
+/* The dynamic shared-memory limit belongs to the kernel function on the current device, not to a model: every model of the
+ * process that launches `kernel` shares it.  So it only ever rises -- a later model with a smaller forest (an attached
+ * outlier forest, a second engine) must not lower it under an earlier model's launches, which would then fail. */
 template <typename K>
 static cudaError_t set_smem_limit(K kernel, int bytes) {
-    return kernel ? cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) : cudaErrorInvalidValue;
+    if (!kernel) return cudaErrorInvalidValue;
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lock(mu);
+    cudaFuncAttributes a;
+    const cudaError_t e = cudaFuncGetAttributes(&a, kernel);
+    if (e != cudaSuccess || a.maxDynamicSharedSizeBytes >= bytes) return e;
+    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }
 
 /* ------------------------------------------------------------------ environment hooks read at model creation (INTEGRATION.md) */
@@ -645,6 +662,31 @@ static bool build_tile_layout(const uint8_t *blob, const b2f_blob_header &h, uin
     return true;
 }
 
+/* What the kernels' aggregate() compares with: an isolation forest flags `s <= bound` on its path-length sum s (forest_predict.cuh).
+ * The blob carries the bound flatten.py derived with numpy, the library's own arithmetic; for a blob written without one the same
+ * search runs here with libm's pow.  Other modes: the header's threshold, unused. */
+static double decision_threshold(const b2f_blob_header &h) {
+    if (h.agg_mode != B2F_AGG_IFOREST) return h.threshold;
+    if (h.flags & B2F_BLOB_HAS_PATH_BOUND) return h.path_bound;
+    auto flagged = [&](int64_t bits) {
+        double s;
+        memcpy(&s, &bits, sizeof(s));
+        return std::pow(2.0, -(s / h.denom)) + h.init_raw > h.threshold;
+    };
+    const double inf = std::numeric_limits<double>::infinity();
+    int64_t lo = 0, hi;
+    memcpy(&hi, &inf, sizeof(hi));
+    if (!flagged(lo)) return -inf;
+    if (flagged(hi)) return inf;
+    while (hi - lo > 1) {
+        const int64_t mid = lo + (hi - lo) / 2;
+        (flagged(mid) ? lo : hi) = mid;
+    }
+    double s;
+    memcpy(&s, &lo, sizeof(s));
+    return s;
+}
+
 /* rank kernel: 4-byte integer nodes, complete trees, rows as ranks (forest_rank.h) */
 static int rank_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
     m->rank_ok = false;
@@ -701,7 +743,7 @@ static int rank_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
     rp.n_pieces = m->rk.n_trees_padded / 8;
     rp.init_raw = m->hdr.init_raw;
     rp.denom = m->hdr.denom;
-    rp.threshold = m->hdr.threshold;
+    rp.threshold = decision_threshold(m->hdr);
     rp.mul_two = 2u;
     rp.mul_64k = 65536u;
     rp.add_64k = 65535u;
@@ -737,7 +779,7 @@ static int warp_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
     kp.n_num = (int)m->hdr.n_num;
     kp.init_raw = m->hdr.init_raw;
     kp.denom = m->hdr.denom;
-    kp.threshold = m->hdr.threshold;
+    kp.threshold = decision_threshold(m->hdr);
     memcpy(kp.impute, m->hdr.impute, sizeof(kp.impute));
     const b2f_blob_group *gt = reinterpret_cast<const b2f_blob_group *>(blob + m->hdr.groups_off);
     for (uint32_t g = 0; g < m->hdr.n_groups; ++g) {
@@ -822,6 +864,8 @@ static int tile_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
     const KParams &kp = m->kp;
     TParams &tp = m->tp;
     memset(&tp, 0, sizeof(tp));
+    CUDA_TRY(cudaMalloc((void **)&m->d_kp, sizeof(KParams)));
+    CUDA_TRY(cudaMemcpy(m->d_kp, &m->kp, sizeof(KParams), cudaMemcpyHostToDevice));
     tp.layout = static_cast<const uint8_t *>(m->d_tile_layout);
     tp.pieces = m->d_tile_pieces;
     tp.n_pieces = (int)pieces.size();
@@ -833,6 +877,7 @@ static int tile_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
     tp.init_raw = kp.init_raw;
     tp.denom = kp.denom;
     tp.threshold = kp.threshold;
+    tp.blob = m->d_kp;
     memcpy(tp.impute, kp.impute, sizeof(tp.impute));
     m->tile_cwarps = cwarps;
     m->tile_smem_bytes = 4096 + cwarps * B2F_TILE_XS_BYTES + n_slots * (int)slot_bytes;
@@ -932,6 +977,7 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
     if (m->compute) cudaStreamDestroy(m->compute);
     if (m->d_blob) cudaFree(m->d_blob);
     if (m->d_tile_layout) cudaFree(m->d_tile_layout);
+    if (m->d_kp) cudaFree(m->d_kp);
     if (m->d_tile_pieces) cudaFree(m->d_tile_pieces);
     if (m->d_rank_layout) cudaFree(m->d_rank_layout);
     if (m->d_mom_partials) cudaFree(m->d_mom_partials);

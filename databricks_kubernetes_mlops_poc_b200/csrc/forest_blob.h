@@ -47,6 +47,7 @@
 #define B2F_META_FEAT_SHIFT 27u
 #define B2F_NODE_STRIDE 256u /* bytes between consecutive slots of one tree (32 lanes x 8 B) */
 #define B2F_META_CAT 0x04000000u
+#define B2F_BLOB_HAS_PATH_BOUND 1u
 
 typedef struct b2f_blob_header {
     char magic[8];
@@ -59,7 +60,7 @@ typedef struct b2f_blob_header {
     uint32_t n_cat;
     uint32_t n_num;
     uint32_t max_depth;
-    uint32_t reserved0;
+    uint32_t flags;  /* B2F_BLOB_HAS_PATH_BOUND */
     double init_raw; /* GBDT: raw prediction of the init estimator; RF: 0; isolation forest: offset_ */
     double denom;    /* RF: n_trees (proba = sum / denom); GBDT: 1; isolation forest: n_trees * c(max_samples) */
     uint64_t groups_off;
@@ -69,7 +70,9 @@ typedef struct b2f_blob_header {
     float impute[24];  /* per row word: replacement for NaN (numeric words), float32(median) */
     int32_t vocab[24]; /* per row word: vocabulary size (categorical words), else 0 */
     double threshold;  /* isolation forest: is_outlier = score > threshold; other modes: 0 */
-    uint8_t pad[B2F_BLOB_HEADER_BYTES - 96 - 192 - 8];
+    double path_bound; /* isolation forest with B2F_BLOB_HAS_PATH_BOUND: the largest path-length sum whose score numpy puts
+                          above `threshold` (flatten.py iforest_path_bound); the kernels flag s <= path_bound */
+    uint8_t pad[B2F_BLOB_HEADER_BYTES - 96 - 192 - 16];
 } b2f_blob_header;
 
 typedef struct b2f_blob_group {

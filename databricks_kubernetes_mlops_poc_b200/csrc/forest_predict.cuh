@@ -169,9 +169,11 @@ __device__ __forceinline__ double warp_sum(double v) {
  *   GBDT     : p1 = expit(init + s), label = raw >= 0   (sklearn >= 1.4 `_gb.py` predict: `raw_predictions >= 0`, the
  *              library the oracle runs; the reference's pin 1.1.1 takes argmax([1-p, p]) and differs only on the exact
  *              tie raw == 0, where it picks class 0.  The reference itself serves a RandomForest, never a GBDT.)
- *   IFOREST  : score = 2^(-s / (n_trees * c(max_samples))) + offset_, flag = score > threshold
+ *   IFOREST  : score = 2^(-s / (n_trees * c(max_samples))) + offset_, flag = score > user threshold, decided as
+ *              s <= `threshold`, the largest path-length sum whose score numpy puts above the user threshold (flatten.py)
  *              (sklearn IsolationForest: -decision_function; alibi-detect IForest.predict,
- *              reference databricks/src/02-register-model.ipynb:232-233,339,344) */
+ *              reference databricks/src/02-register-model.ipynb:232-233,339,344)
+ * Labels and flags of rows inside the rounding band of the decision are re-decided by forest_decide.cuh. */
 __device__ __forceinline__ void aggregate(int agg_mode, double init_raw, double denom, double threshold, double s, double &p1, int &lab) {
     if (agg_mode == B2F_AGG_RF_MEAN) {
         p1 = s / denom;
@@ -182,7 +184,7 @@ __device__ __forceinline__ void aggregate(int agg_mode, double init_raw, double 
         lab = raw >= 0.0;
     } else {
         p1 = exp2(-(s / denom)) + init_raw;
-        lab = p1 > threshold;
+        lab = s <= threshold; /* threshold: the host's path-length bound, score > user threshold <=> s <= bound */
     }
 }
 
@@ -193,14 +195,17 @@ __device__ __forceinline__ void aggregate(int agg_mode, double init_raw, double 
 __device__ __forceinline__ int ostride_p(int o) { return o & 0xffff; }
 __device__ __forceinline__ int ostride_l(int o) { return (o >> 16) ? (o >> 16) : (o & 0xffff); }
 
+#include "forest_decide.cuh"
+
 /* aggregate -> (probability, label) for one row per lane; rows < 0 are empty slots */
-template <typename OutT>
-__device__ __forceinline__ void finalize_store(const KParams &p, double s, long long row, OutT *__restrict__ proba,
-                                               int32_t *__restrict__ label, int ostride) {
+template <bool PACKED, typename OutT>
+__device__ __forceinline__ void finalize_store(const KParams &p, double s, long long row, const uint32_t *__restrict__ rows,
+                                               OutT *__restrict__ proba, int32_t *__restrict__ label, int ostride) {
     if (row < 0) return;
     double p1;
     int lab;
     aggregate(p.agg_mode, p.init_raw, p.denom, p.threshold, s, p1, lab);
+    if (label && decide_exactly(p.agg_mode, s, p.denom, p.threshold)) lab = decide_row_blob<PACKED>(p, rows, row);
     if (proba) proba[row * ostride_p(ostride)] = (OutT)p1;
     if (label) label[row * ostride_l(ostride)] = lab;
 }
@@ -376,13 +381,13 @@ __global__ void __launch_bounds__(B2F_PREDICT_THREADS, 1)
                 pend_row = row < n ? row : -1;
             }
             if (++pend_n == 32) {
-                finalize_store(p, pend_sum, pend_row, proba, label, ostride);
+                finalize_store<PACKED>(p, pend_sum, pend_row, rows, proba, label, ostride);
                 pend_n = 0;
                 pend_row = -1;
             }
         }
     }
-    if (pend_n > 0) finalize_store(p, pend_sum, pend_row, proba, label, ostride);
+    if (pend_n > 0) finalize_store<PACKED>(p, pend_sum, pend_row, rows, proba, label, ostride);
 
     if constexpr (SMEM) {
         /* never retire a CTA while a bulk copy into its shared memory is still in flight */
@@ -448,6 +453,6 @@ __global__ void __launch_bounds__(1024, 1)
         double s = 0.0;
         for (int k = 0; k < p.n_groups; ++k) s += part[k][r]; /* group order: deterministic */
         const long long row = b * R + r;
-        finalize_store(p, s, row < n ? row : -1, proba, label, ostride);
+        finalize_store<PACKED>(p, s, row < n ? row : -1, rows, proba, label, ostride);
     }
 }

@@ -129,6 +129,41 @@ __device__ __forceinline__ uint32_t lds_u16(uint32_t a) {
     return v;
 }
 
+/* the decision of one ranked row inside the rounding band (forest_decide.cuh): one thread walks the rank layout in global
+ * memory tree by tree, reading value[f] straight from the row as the staging of phase 1 would have placed it */
+__device__ __noinline__ int decide_row_rank(const RParams &p, const uint8_t *rows, long long row) {
+    const uint8_t *r = rows + (size_t)row * p.row_bytes;
+    unsigned long long cw = __ldg(reinterpret_cast<const uint32_t *>(r));
+    if (p.cat_bytes == 8) cw |= (unsigned long long)__ldg(reinterpret_cast<const uint32_t *>(r) + 1) << 32;
+    const uint32_t num_slots = (uint32_t)((p.n_num + 1) >> 1) * 2u;
+    auto value = [&](uint32_t f) -> uint32_t {
+        if (f < num_slots) return (int)f < p.n_num ? (uint32_t)__ldg(reinterpret_cast<const unsigned short *>(r + p.cat_bytes) + f) : 0u;
+        const uint32_t slot = f - num_slots; /* one-hot pseudo-feature: (categorical feature, category) pair `slot` */
+        for (int j = 0; j < p.n_cat; ++j) {
+            const uint32_t code1 = (uint32_t)(cw >> p.cat_shift[j]) & ((1u << p.cat_bits[j]) - 1u);
+            const unsigned long long m = p.cat_mask[j];
+            if (code1 != 0u && code1 <= 64u && ((m >> (code1 - 1u)) & 1ull) &&
+                (uint32_t)p.cat_start[j] + (uint32_t)__popcll(m & ((1ull << (code1 - 1u)) - 1ull)) == slot)
+                return 1u;
+        }
+        return 0u;
+    };
+    return decide_from_payloads(p.agg_mode, p.denom, p.threshold, [&](auto add) {
+        const uint32_t n_leaf = 1u << p.depth;
+        for (int t = 0; t < p.n_trees_padded; ++t) {
+            const uint8_t *tree = p.layout + (size_t)t * p.tree_stride;
+            uint32_t i = 0;
+            for (int d = 0; d < p.depth; ++d) {
+                const uint32_t nw = __ldg(reinterpret_cast<const uint32_t *>(tree) + i);
+                const uint32_t off = nw & 0x1F82u; /* (f >> 1) * 128 + (f & 1) * 2 */
+                const uint32_t x = value(((off >> 7) << 1) | ((off >> 1) & 1u)) * 65536u + 65535u;
+                i = 2u * i + (x >= nw ? 2u : 1u);
+            }
+            add(__ldg(reinterpret_cast<const double *>(tree + n_leaf * 4u) + (i - (n_leaf - 1u))));
+        }
+    });
+}
+
 /* walk U consecutive trees (first tree at shared address t0) for this lane's row; payloads are added in tree order.
  * A chain keeps the ABSOLUTE shared address a = B + 4i of its node (B = the tree's base): the child 2i+1 (+1) sits at
  * 2a - B + 4 (+4), i.e. one SEL between the two per-tree constants (4 - B, 8 - B) and one multiply-add (FMA pipe).
@@ -172,7 +207,8 @@ __device__ __forceinline__ void rank_walk_group(const RParams &p, int tree0, uin
     for (int u = 0; u < U; ++u) acc += lds_f64(at[u] + at[u] + k4[u] + 4u - (4u << D));
 }
 
-template <int D, int U, bool STREAM, typename OutT>
+/* DECIDE: rows inside the rounding band are re-decided exactly (RF, isolation forest); false for a GBDT */
+template <int D, int U, bool STREAM, bool DECIDE, typename OutT>
 __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
     k_forest_predict_rank(const __grid_constant__ RParams p, const uint8_t *__restrict__ rows, long long n, OutT *__restrict__ proba,
                           int32_t *__restrict__ label, int ostride) {
@@ -318,6 +354,9 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
                 int lab;
                 aggregate(p.agg_mode, p.agg_mode == B2F_AGG_GBDT_LOGISTIC ? 0.0 : p.init_raw, p.denom, p.threshold, s, p1, lab);
                 const long long row = row0 + r;
+                if constexpr (DECIDE)
+                    if constexpr (DECIDE)
+                if (label && decide_exactly(p.agg_mode, s, p.denom, p.threshold)) lab = decide_row_rank(p, rows, row);
                 if (proba) proba[row * ostride_p(ostride)] = (OutT)p1;
                 if (label) label[row * ostride_l(ostride)] = lab;
             }
@@ -360,6 +399,8 @@ __global__ void __launch_bounds__(B2F_RANK_THREADS, 1)
             int lab;
             aggregate(p.agg_mode, p.agg_mode == B2F_AGG_GBDT_LOGISTIC ? 0.0 : p.init_raw, p.denom, p.threshold, s, p1, lab);
             const long long row = row0 + r;
+            if constexpr (DECIDE)
+                if (label && decide_exactly(p.agg_mode, s, p.denom, p.threshold)) lab = decide_row_rank(p, rows, row);
             if (proba) proba[row * ostride_p(ostride)] = (OutT)p1;
             if (label) label[row * ostride_l(ostride)] = lab;
         }

@@ -79,6 +79,7 @@ struct TParams {
     double denom;
     double threshold;
     float impute[24];
+    const KParams *blob;    /* device copy of the blob parameters: rows inside the rounding band are re-decided on it */
 };
 
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
@@ -300,6 +301,7 @@ __global__ void __launch_bounds__(B2F_TILE_THREADS_MAX, 1)
             int lab;
             /* the GBDT init value is already in acc (added first, as sklearn does) */
             aggregate(p.agg_mode, p.agg_mode == B2F_AGG_GBDT_LOGISTIC ? 0.0 : p.init_raw, p.denom, p.threshold, acc, p1, lab);
+            if (label && decide_exactly(p.agg_mode, acc, p.denom, p.threshold)) lab = decide_row_blob<PACKED>(*p.blob, rows, row);
             if (proba) proba[row * ostride_p(ostride)] = (OutT)p1;
             if (label) label[row * ostride_l(ostride)] = lab;
         }

@@ -45,7 +45,8 @@ AGG_GBDT_LOGISTIC = 1
 AGG_IFOREST = 2
 BLOB_VERSION = 2
 
-_HEADER_FMT = "<8s" + "I" * 10 + "dd" + "Q" * 4 + "24f" + "24i" + "d"  # 296 bytes, padded to 512
+_HEADER_FMT = "<8s" + "I" * 10 + "dd" + "Q" * 4 + "24f" + "24i" + "dd"  # 304 bytes, padded to 512
+HEADER_HAS_PATH_BOUND = 1  # header flags bit: ``path_bound`` holds the isolation forest's decision bound
 _GROUP_FMT = "<8I"
 
 
@@ -180,7 +181,7 @@ def _flatten_tree(tree, col_word, col_cat_code, col_is_cat, leaf_value):
     return T, M, LV, depth
 
 
-def _assemble_blob(flat, agg, init_raw, denom, n_cat, n_num, impute, vocab, threshold=0.0):
+def _assemble_blob(flat, agg, init_raw, denom, n_cat, n_num, impute, vocab, threshold=0.0, path_bound=None):
     """Flattened trees ``[(T, M, LV, depth), ...]`` -> (blob bytes, max depth): groups of 32 interleaved trees."""
     n_trees = len(flat)
     if not (1 <= n_trees <= MAX_TREES):
@@ -223,7 +224,7 @@ def _assemble_blob(flat, agg, init_raw, denom, n_cat, n_num, impute, vocab, thre
         n_cat,
         n_num,
         max_depth,
-        0,
+        0 if path_bound is None else HEADER_HAS_PATH_BOUND,
         init_raw,
         denom,
         groups_off,
@@ -233,6 +234,7 @@ def _assemble_blob(flat, agg, init_raw, denom, n_cat, n_num, impute, vocab, thre
         *np.asarray(impute, dtype=np.float32).tolist(),
         *np.asarray(vocab, dtype=np.int32).tolist(),
         float(threshold),
+        0.0 if path_bound is None else float(path_bound),
     )
     header = header + b"\0" * (HEADER_BYTES - len(header))
     table = b"".join(struct.pack(_GROUP_FMT, *g) for g in groups)
@@ -253,6 +255,29 @@ def _average_path_length(n):
     return out
 
 
+def iforest_path_bound(offset: float, denom: float, threshold: float) -> float:
+    """The largest path-length sum ``s >= 0`` that sklearn flags: ``-decision_function = -((-(2 ** (-s / denom))) - offset)
+    > threshold``, evaluated with numpy exactly as ``IsolationForest`` does.  The score falls as ``s`` grows, so the kernels
+    decide ``s <= bound`` on the path-length sum instead of comparing a score rounded by other arithmetic (CUDA's exp2)
+    with the threshold.  -inf: no sum is flagged; +inf: every sum is."""
+
+    def flagged(bits: int) -> bool:
+        s = np.array([bits], dtype=np.int64).view(np.float64)
+        scores = 2 ** (-np.divide(s, denom))
+        return bool(-(-scores - offset)[0] > threshold)
+
+    inf_bits = int(np.array([np.inf]).view(np.int64)[0])
+    if not flagged(0):
+        return -np.inf
+    if flagged(inf_bits):
+        return np.inf
+    lo, hi = 0, inf_bits  # flagged(lo), not flagged(hi): non-negative doubles are ordered as their bit patterns
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        lo, hi = (mid, hi) if flagged(mid) else (lo, mid)
+    return float(np.array([lo], dtype=np.int64).view(np.float64)[0])
+
+
 def flatten_isolation_forest(detector, n_cat: int, n_num: int, vocab=None, threshold: float | None = None) -> bytes:
     """Fitted outlier detector -> forest blob with ``agg_mode = AGG_IFOREST`` over the classifier's encoded rows.
 
@@ -263,8 +288,10 @@ def flatten_isolation_forest(detector, n_cat: int, n_num: int, vocab=None, thres
     feature k of the request, i.e. row word ``n_cat + k``.  What the GPU reproduces:
 
     * ``score = -decision_function(X) = 2 ** (-sum_t h_t(x) / (n_trees * c(max_samples))) + offset_`` with
-      ``h_t(x) = depth(leaf) + c(n_node_samples[leaf])`` (``_iforest.py`` ``_compute_score_samples``);
-    * ``is_outlier = score > threshold``.
+      ``h_t(x) = (depth(leaf) + 1) + c(n_node_samples[leaf]) - 1.0``, sklearn's per-tree term to the last bit
+      (``_iforest.py`` ``_compute_score_samples``);
+    * ``is_outlier = score > threshold``, decided as ``sum_t h_t(x) <= iforest_path_bound(...)``; a row near the bound is
+      summed again in tree order, as sklearn sums it (``csrc/forest_decide.cuh``), so the flag is sklearn's.
 
     Splits compare float32 inputs with float64 thresholds exactly as the classifier's trees do.  NaN inputs are
     outside the contract: the reference's pinned scikit-learn 1.1.1 (``app/requirements.txt:14``) rejects them in
@@ -295,7 +322,7 @@ def flatten_isolation_forest(detector, n_cat: int, n_num: int, vocab=None, thres
         for i in range(tree.node_count):  # sklearn stores parents before children
             if left[i] != -1:
                 depth[left[i]] = depth[right[i]] = depth[i] + 1.0
-        payload = depth + _average_path_length(tree.n_node_samples)
+        payload = (depth.astype(np.int64) + 1) + _average_path_length(tree.n_node_samples) - 1.0
         flat.append(_flatten_tree(tree, col_word, np.zeros_like(col_word), none, payload))
     denom = float(len(flat)) * float(_average_path_length(np.array([iso._max_samples]))[0])
     if not denom > 0.0:
@@ -305,7 +332,9 @@ def flatten_isolation_forest(detector, n_cat: int, n_num: int, vocab=None, thres
     v = np.zeros(ROW_WORDS, dtype=np.int32)
     if vocab is not None:
         v[:n_cat] = np.asarray(vocab, dtype=np.int32)[:n_cat]
-    blob, _ = _assemble_blob(flat, AGG_IFOREST, float(iso.offset_), denom, n_cat, n_num, impute, v, threshold=float(threshold))
+    bound = iforest_path_bound(float(iso.offset_), denom, float(threshold))
+    blob, _ = _assemble_blob(flat, AGG_IFOREST, float(iso.offset_), denom, n_cat, n_num, impute, v, threshold=float(threshold),
+                             path_bound=bound)
     return blob
 
 
@@ -430,11 +459,12 @@ def parse_header(blob: bytes) -> dict:
     """Decode the fixed header + group table (host-side mirror of ``forest_blob.h``)."""
     f = struct.unpack_from(_HEADER_FMT, blob, 0)
     keys = ["magic", "version", "header_bytes", "agg_mode", "n_trees", "n_groups", "row_words", "n_cat", "n_num",
-            "max_depth", "reserved0", "init_raw", "denom", "groups_off", "chunks_off", "chunks_bytes", "total_bytes"]
+            "max_depth", "flags", "init_raw", "denom", "groups_off", "chunks_off", "chunks_bytes", "total_bytes"]
     h = dict(zip(keys, f[:17]))
     h["impute"] = np.array(f[17:41], dtype=np.float32)
     h["vocab"] = np.array(f[41:65], dtype=np.int32)
     h["threshold"] = f[65]
+    h["path_bound"] = f[66]
     gk = ["chunk_off", "chunk_bytes", "n_slots", "n_leaf_slots", "depth", "n_trees"]
     h["groups"] = [
         dict(zip(gk, struct.unpack_from(_GROUP_FMT, blob, h["groups_off"] + 32 * g)[:6])) for g in range(h["n_groups"])
