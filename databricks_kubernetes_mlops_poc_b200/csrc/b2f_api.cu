@@ -204,25 +204,30 @@ struct Importance {
     DevBuf scores;  /* the group's records */
 };
 
-/* the MMD drift test (b2f_model_attach_mmd_reference / b2f_mmd_drift; mmd_drift.cuh): the reference's embedding and
- * kernel row sums, kept between calls, and a call's buffers; all on the compute stream, grown on demand */
-struct Mmd {
+/* a reference table in K9's embedding (k_mmd_embed; mmd_drift.cuh), which MMD drift and trust scores share: its constants and
+ * embedding, kept between calls, and a call's rows and their embedding; all on the compute stream, grown on demand */
+struct EmbeddedRef {
     MmdParams mp;
-    int64_t n_ref = 0; /* 0: no reference */
+    int64_t n_ref = 0;   /* 0: no reference */
+    DevBuf ref_z, ref_c; /* the reference's embedding */
+    DevBuf rows, z, c;   /* a call's rows and their embedding */
+};
+
+/* the MMD drift test (b2f_model_attach_mmd_reference / b2f_mmd_drift; mmd_drift.cuh): the reference and its kernel row
+ * sums, kept between calls, and a call's buffers; all on the compute stream, grown on demand */
+struct Mmd {
+    EmbeddedRef ref;
     double sigma = 0.0, coef = 0.0;
-    DevBuf ref_z, ref_c, r_ref; /* the reference: embedding and sum_{j != i} k(i, j) over the reference */
-    DevBuf rows, z, c;          /* a call's rows and the batch's embedding */
+    DevBuf r_ref; /* sum_{j != i} k(i, j) over the reference */
     DevBuf r, partial, sub, pairs, out, hist;
 };
 
 /* the k-nearest reference search of trust scores (b2f_model_attach_knn_reference / b2f_knn; knn.cuh): the class-sorted
- * reference's embedding and row map, kept between calls, and a call's buffers; all on the compute stream, grown on demand */
+ * reference and its row map, kept between calls, and a call's buffers; all on the compute stream, grown on demand */
 struct Knn {
-    MmdParams mp;
-    int64_t n_ref = 0; /* 0: no reference */
+    EmbeddedRef ref; /* class 0 rows, then class 1; a call embeds a piece of its queries */
     int64_t n_cls[2] = {0, 0};
-    DevBuf ref_z, ref_c, orig; /* the reference: embedding (class 0 rows, then class 1) and position -> original row */
-    DevBuf rows, z, c;         /* a piece's rows and the queries' embedding */
+    DevBuf orig; /* reference position -> original row */
     DevBuf cand_d, cand_i, dist, index;
 };
 
@@ -965,12 +970,10 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
     for (DevBuf *b : {&m->scratch, &m->pd.host_spec, &m->pd.device_spec, &m->cf.dev, &m->mom_rows, &m->gather, &m->flush}) b->release();
     for (DevBuf *b : {&m->pair.host_spec, &m->pair.spec_dev, &m->pair.rows, &m->pair.partial, &m->pair.out}) b->release();
     for (DevBuf *b : {&m->pi.rows, &m->pi.labels, &m->pi.perm, &m->pi.keys, &m->pi.flags, &m->pi.temp, &m->pi.offsets, &m->pi.segs, &m->pi.scores}) b->release();
-    for (DevBuf *b : {&m->mmd.ref_z, &m->mmd.ref_c, &m->mmd.r_ref, &m->mmd.rows, &m->mmd.z, &m->mmd.c, &m->mmd.r, &m->mmd.partial, &m->mmd.sub,
-                      &m->mmd.pairs, &m->mmd.out, &m->mmd.hist})
-        b->release();
-    for (DevBuf *b : {&m->knn.ref_z, &m->knn.ref_c, &m->knn.orig, &m->knn.rows, &m->knn.z, &m->knn.c, &m->knn.cand_d, &m->knn.cand_i,
-                      &m->knn.dist, &m->knn.index})
-        b->release();
+    for (EmbeddedRef *e : {&m->mmd.ref, &m->knn.ref})
+        for (DevBuf *b : {&e->ref_z, &e->ref_c, &e->rows, &e->z, &e->c}) b->release();
+    for (DevBuf *b : {&m->mmd.r_ref, &m->mmd.r, &m->mmd.partial, &m->mmd.sub, &m->mmd.pairs, &m->mmd.out, &m->mmd.hist}) b->release();
+    for (DevBuf *b : {&m->knn.orig, &m->knn.cand_d, &m->knn.cand_i, &m->knn.dist, &m->knn.index}) b->release();
     for (auto &t : m->tickets)
         for (auto &e : t.ev)
             if (e) cudaEventDestroy(e);
@@ -1375,6 +1378,64 @@ struct Events {
     }
 };
 
+/* ------------------------------------------------------------------ helpers of the entry points beside scoring (moments, *_api.cuh) */
+
+/* reserve bytes of b on the compute stream, a failure reported as B2F_ENOMEM and its byte count */
+static int compute_reserve(b2f_model *m, DevBuf &b, size_t bytes, const char *who, const char *what) {
+    if (b.reserve(m->compute, bytes, bytes) == B2F_OK) return B2F_OK;
+    (void)cudaGetLastError(); /* the failed cudaMalloc's error: not left for the next launch check to report */
+    return set_err(B2F_ENOMEM, "%s: cannot allocate %zu device bytes for %s", who, bytes, what);
+}
+
+/* after a <<< >>> launch (or cudaLaunchKernel): its error, or one more launch counted */
+static int launched(b2f_model *m, const char *name) {
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_err(B2F_ECUDA, "%s launch failed: %s", name, cudaGetErrorString(e));
+    m->launches++;
+    return B2F_OK;
+}
+
+/* device_ms (may be NULL) of a region of the compute stream: start() records its start; finish() records its end, waits for
+ * the stream (also without device_ms) and writes the elapsed time */
+struct TimedRegion {
+    b2f_model *m;
+    float *device_ms;
+    Events evs;
+    int start() {
+        if (!device_ms) return B2F_OK;
+        const int rc = evs.create(2);
+        if (rc) return rc;
+        CUDA_TRY(cudaEventRecord(evs.e[0], m->compute));
+        return B2F_OK;
+    }
+    int finish() {
+        const cudaStream_t st = m->compute;
+        if (device_ms) CUDA_TRY(cudaEventRecord(evs.e[1], st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (device_ms) CUDA_TRY(cudaEventElapsedTime(device_ms, evs.e[0], evs.e[1]));
+        return B2F_OK;
+    }
+};
+
+/* every analysis reads row values, which ranked rows do not carry; subject: the caller with its verb ("explanations take") */
+static int check_value_rows(int fmt, const char *subject) {
+    if (fmt == B2F_ROWS_RANKED)
+        return set_err(B2F_EINVAL, "%s float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values", subject);
+    return B2F_OK;
+}
+
+/* a call's spec into buf: synchronously, before a host job's chunks (each host call synchronises, so no earlier call still
+ * reads it), or on the compute stream (async), ordered with the launches that read it.  who: the prefix of a failed
+ * allocation's B2F_ENOMEM; NULL: DevBuf::reserve's B2F_ECUDA */
+static int upload_spec(b2f_model *m, DevBuf &buf, const std::vector<uint32_t> &spec, bool async, const char *who) {
+    const size_t bytes = spec.size() * sizeof(uint32_t);
+    const int rc = who ? compute_reserve(m, buf, bytes, who, "the point table") : buf.reserve(m->compute, bytes, bytes);
+    if (rc) return rc;
+    if (async) CUDA_TRY(cudaMemcpyAsync(buf.p, spec.data(), bytes, cudaMemcpyHostToDevice, m->compute));
+    else CUDA_TRY(cudaMemcpy(buf.p, spec.data(), bytes, cudaMemcpyHostToDevice));
+    return B2F_OK;
+}
+
 /* a synchronous host batch of n >= 0 rows of a checked job; device_ms (may be NULL): from the first H2D to the end of the last
  * chunk */
 static int timed_host_batch(b2f_model *m, const HostJob &job, const void *rows, int64_t n, int row_format, double *out, float *device_ms) {
@@ -1644,10 +1705,7 @@ static int launch_moments(b2f_model *m, const void *rows_dev, int64_t n) {
     if (blocks < 1) blocks = 1;
     k_feature_moments<<<(unsigned)blocks, B2F_MOM_THREADS, B2F_MOM_SMEM, m->compute>>>(static_cast<const uint4 *>(rows_dev), (long long)n,
                                                                                      (int)m->hdr.n_cat, m->d_mom_partials, m->d_mom_ticket, m->d_mom_out);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_feature_moments launch failed: %s", cudaGetErrorString(e));
-    m->launches++;
-    return B2F_OK;
+    return launched(m, "k_feature_moments");
 }
 
 extern "C" int b2f_moments_device(b2f_model *m, const void *rows_dev, int64_t n, double *out) {

@@ -65,8 +65,8 @@ static int cf_build_table(b2f_model *m) {
 /* check a call's arguments, then set the probe fields of m->cf.cp (builds the table on the first call) */
 static int cf_prepare(b2f_model *m, int64_t n, int fmt, const int32_t *words, int n_words, double cutoff, bool have_out) {
     const b2f_blob_header &h = m->hdr;
-    if (fmt == B2F_ROWS_RANKED)
-        return set_err(B2F_EINVAL, "counterfactuals take float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
+    int rc = check_value_rows(fmt, "counterfactuals take");
+    if (rc) return rc;
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
     if (!have_out) return set_err(B2F_EINVAL, "out is NULL");
     if (!words) return set_err(B2F_EINVAL, "words is NULL");
@@ -79,8 +79,7 @@ static int cf_prepare(b2f_model *m, int64_t n, int fmt, const int32_t *words, in
                            i, words[i], h.n_cat, h.n_cat + h.n_num - 1);
     if (!std::isfinite(cutoff) || cutoff < 0.0 || cutoff > 1.0) return set_err(B2F_EINVAL, "cutoff %g: expected a number in [0, 1]", cutoff);
     if (h.max_depth > B2F_PD_STACK) return set_err(B2F_EINVAL, "counterfactuals walk trees of depth <= %d; this forest has depth %u", B2F_PD_STACK, h.max_depth);
-    int rc = cf_build_table(m);
-    if (rc) return rc;
+    if ((rc = cf_build_table(m))) return rc;
     CfParams &cp = m->cf.cp;
     cp.cutoff = cutoff;
     cp.n_words = n_words;
@@ -115,19 +114,14 @@ static int launch_counterfactual(b2f_model *m, cudaStream_t st, const void *rows
             k_counterfactual<true><<<grid, B2F_PD_WARPS * 32, 0, st>>>(cp, rows, (long long)n, cand);
         else
             k_counterfactual<false><<<grid, B2F_PD_WARPS * 32, 0, st>>>(cp, rows, (long long)n, cand);
-        const cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_counterfactual launch failed: %s", cudaGetErrorString(e));
-        m->launches++;
+        if ((rc = launched(m, "k_counterfactual"))) return rc;
     }
     const dim3 fgrid((unsigned)((n + 127) / 128), (unsigned)cp.n_words);
     if (pk)
         k_counterfactual_finish<true><<<fgrid, 128, 0, st>>>(cp, rows, (long long)n, cand, out, out_stride, proba, proba_stride);
     else
         k_counterfactual_finish<false><<<fgrid, 128, 0, st>>>(cp, rows, (long long)n, cand, out, out_stride, proba, proba_stride);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_counterfactual_finish launch failed: %s", cudaGetErrorString(e));
-    m->launches++;
-    return B2F_OK;
+    return launched(m, "k_counterfactual_finish");
 }
 
 /* A host chunk's output row is the row's n_words records, then its p1: one D2H copy per chunk into a staging array, split

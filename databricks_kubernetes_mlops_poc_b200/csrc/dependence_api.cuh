@@ -17,10 +17,9 @@ static int64_t pd_chunk_rows(const b2f_model *m) {
  * A call's probes and grid become one spec: a PdSeg per run of up to B2F_PD_SEG points of a probe, then every point's
  * word in output order (a row's output is its probes' points, concatenated), numerics imputed as the kernels impute rows.
  * The spec is checked and built on the host, uploaded once per call, and read by every chunk's launch. */
-static int pd_check(const b2f_model *m, int fmt, bool have_out) {
-    (void)m;
-    if (fmt == B2F_ROWS_RANKED)
-        return set_err(B2F_EINVAL, "partial dependence takes float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
+static int pd_check(int fmt, bool have_out) {
+    const int rc = check_value_rows(fmt, "partial dependence takes");
+    if (rc) return rc;
     if (!have_out) return set_err(B2F_EINVAL, "out is NULL");
     return B2F_OK;
 }
@@ -78,10 +77,7 @@ static int launch_dependence(b2f_model *m, cudaStream_t st, const void *rows_dev
         k_partial_dependence<true><<<grid, B2F_PD_WARPS * 32, 0, st>>>(pp, rows, (long long)n, out_dev);
     else
         k_partial_dependence<false><<<grid, B2F_PD_WARPS * 32, 0, st>>>(pp, rows, (long long)n, out_dev);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_partial_dependence launch failed: %s", cudaGetErrorString(e));
-    m->launches++;
-    return B2F_OK;
+    return launched(m, "k_partial_dependence");
 }
 
 /* the spec goes up once, before the chunks that read it; no earlier host call still reads it (each one synchronises) */
@@ -92,12 +88,10 @@ extern "C" int b2f_partial_dependence(b2f_model *m, const void *rows, int64_t n,
     int rc = pd_prepare(m, probes, n_probes, grid_words);
     if (rc) return rc;
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
-    if ((rc = pd_check(m, row_format, out || n == 0))) return rc;
+    if ((rc = pd_check(row_format, out || n == 0))) return rc;
     if (n > 0) {
         CUDA_TRY(cudaSetDevice(m->device));
-        const size_t bytes = m->pd.spec.size() * sizeof(uint32_t);
-        if ((rc = m->pd.host_spec.reserve(m->compute, bytes, bytes))) return rc;
-        CUDA_TRY(cudaMemcpy(m->pd.host_spec.p, m->pd.spec.data(), bytes, cudaMemcpyHostToDevice));
+        if ((rc = upload_spec(m, m->pd.host_spec, m->pd.spec, false, nullptr))) return rc;
     }
     const HostJob job{(size_t)m->pd.pp.points * sizeof(double), pd_chunk_rows(m), false, 0,
                       [](b2f_model *m, int, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, void *out_dev, int32_t *, DevBuf &) {
@@ -111,13 +105,11 @@ extern "C" int b2f_partial_dependence_device(b2f_model *m, const void *rows_dev,
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
     int rc = pd_prepare(m, probes, n_probes, grid_words);
-    if (rc == B2F_OK) rc = pd_check(m, row_format, out_dev != nullptr || n == 0);
+    if (rc == B2F_OK) rc = pd_check(row_format, out_dev != nullptr || n == 0);
     if (rc == B2F_OK) rc = check_row_format(m, row_format);
     if (rc) return rc;
     if (n == 0) return B2F_OK;
     CUDA_TRY(cudaSetDevice(m->device));
-    const size_t bytes = m->pd.spec.size() * sizeof(uint32_t);
-    if ((rc = m->pd.device_spec.reserve(m->compute, bytes, bytes))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(m->pd.device_spec.p, m->pd.spec.data(), bytes, cudaMemcpyHostToDevice, m->compute));
+    if ((rc = upload_spec(m, m->pd.device_spec, m->pd.spec, true, nullptr))) return rc;
     return launch_dependence(m, m->compute, rows_dev, n, row_format, out_dev, m->pd.device_spec.p);
 }

@@ -56,8 +56,8 @@ static size_t explain_row_bytes(const b2f_model *m, int v) {
 /* the checks of an explain call that follow the explainer's own (m->ex is set) */
 static int explain_check(const b2f_model *m, int fmt, int v, bool have_out) {
     if (v == SHAP_INTERVENTIONAL && !m->ex->bg.rows) return set_err(B2F_ESTATE, "no background attached (b2f_model_attach_background)");
-    if (fmt == B2F_ROWS_RANKED)
-        return set_err(B2F_EINVAL, "explanations take float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
+    const int rc = check_value_rows(fmt, "explanations take");
+    if (rc) return rc;
     if (!have_out) return set_err(B2F_EINVAL, v == SHAP_INTERACTIONS ? "phi2 is NULL" : "phi is NULL");
     return B2F_OK;
 }
@@ -102,10 +102,10 @@ static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, i
         return B2F_OK;
     }
     const int64_t ranges = explain_ranges(m, n, v);
+    int rc;
     if (ranges > 1) {
         const size_t bytes = (size_t)ranges * (size_t)n * values * sizeof(double);
-        int rc = scratch.reserve(st, bytes, bytes);
-        if (rc) return rc;
+        if ((rc = scratch.reserve(st, bytes, bytes))) return rc;
     }
     double *partials = static_cast<double *>(scratch.p);
     const uint32_t *rows = static_cast<const uint32_t *>(rows_dev);
@@ -114,9 +114,7 @@ static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, i
     /* a failed launch is also the thread's last error, taken (and cleared) below as after <<< >>> */
     cudaLaunchKernel(explain_kernel(v, ex.maxl, fmt == B2F_ROWS_PACKED64), dim3((unsigned)((n + 31) / 32), (unsigned)ranges),
                      dim3(B2F_SHAP_THREADS), args, (size_t)ex.kernels[v].smem_bytes, st);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_err(B2F_ECUDA, "%s launch failed: %s", name, cudaGetErrorString(e));
-    m->launches++;
+    if ((rc = launched(m, name))) return rc;
     if (ranges > 1) {
         if (inter) { /* one CTA per row, its triangle in shared memory */
             const unsigned blocks = (unsigned)std::min<int64_t>(n, (int64_t)m->sm_count * 8);
@@ -127,9 +125,7 @@ static int launch_explain(b2f_model *m, cudaStream_t st, const void *rows_dev, i
             const unsigned blocks = (unsigned)std::min<int64_t>((n_values + 255) / 256, (int64_t)m->sm_count * 8);
             k_tree_shap_finish<<<blocks, 256, 0, st>>>(partials, (int)ranges, (long long)n_values, denom, out_dev);
         }
-        e = cudaGetLastError();
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "%s_finish launch failed: %s", name, cudaGetErrorString(e));
-        m->launches++;
+        return launched(m, (std::string(name) + "_finish").c_str());
     }
     return B2F_OK;
 }
@@ -350,9 +346,8 @@ extern "C" int b2f_model_attach_background(b2f_model *m, const void *rows, int64
     if (!m->ex) return set_err(B2F_ESTATE, "no explainer attached (b2f_model_attach_explainer)");
     if (n <= 0) return set_err(B2F_EINVAL, "background needs at least one row (n = %lld)", (long long)n);
     if (!rows) return set_err(B2F_EINVAL, "rows is NULL");
-    if (row_format == B2F_ROWS_RANKED)
-        return set_err(B2F_EINVAL, "a background takes float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
-    int rc = check_row_format(m, row_format);
+    int rc = check_value_rows(row_format, "a background takes");
+    if (rc == B2F_OK) rc = check_row_format(m, row_format);
     if (rc) return rc;
     CUDA_TRY(cudaSetDevice(m->device));
     Explainer &ex = *m->ex;

@@ -21,13 +21,6 @@ static_assert(sizeof(struct b2f_perm_score) == 64 && offsetof(struct b2f_perm_sc
 static_assert(sizeof(PiScore) == sizeof(struct b2f_perm_score) && offsetof(PiScore, auc_u2) == offsetof(struct b2f_perm_score, auc_u2),
               "PiScore layout");
 
-/* reserve with the failure reported as B2F_ENOMEM and its byte count */
-static int pi_reserve(b2f_model *m, DevBuf &b, size_t bytes, const char *what) {
-    if (b.reserve(m->compute, bytes, bytes) == B2F_OK) return B2F_OK;
-    (void)cudaGetLastError();
-    return set_err(B2F_ENOMEM, "permutation scores: cannot allocate %zu device bytes for %s", bytes, what);
-}
-
 /* points of one group: the most whose keys, flags and their sort copies (18 bytes per row) fit the budget, at least one */
 static int64_t pi_group_points(int64_t n, int64_t points) {
     const int64_t fit = std::max<int64_t>(1, B2F_PERM_SCRATCH_BYTES / (18 * n));
@@ -40,9 +33,8 @@ extern "C" int b2f_permutation_scores(b2f_model *m, const void *rows, int64_t n,
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
     if (device_ms) *device_ms = 0.0f;
     const b2f_blob_header &h = m->hdr;
-    if (row_format == B2F_ROWS_RANKED)
-        return set_err(B2F_EINVAL, "permutation scores take float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
-    int rc = check_row_format(m, row_format);
+    int rc = check_value_rows(row_format, "permutation scores take");
+    if (rc == B2F_OK) rc = check_row_format(m, row_format);
     if (rc) return rc;
     if (n < 1 || n > (int64_t)INT_MAX) return set_err(B2F_EINVAL, "n = %lld: expected 1 .. 2^31 - 1 rows", (long long)n);
     if (!rows || !labels || !perm || !words || !out || !baseline) return set_err(B2F_EINVAL, "rows, labels, perm, words, out or baseline is NULL");
@@ -63,14 +55,16 @@ extern "C" int b2f_permutation_scores(b2f_model *m, const void *rows, int64_t n,
     CUDA_TRY(cudaSetDevice(m->device));
     Importance &pi = m->pi;
     const cudaStream_t st = m->compute;
-    const size_t row_bytes = row_format == B2F_ROWS_PACKED64 ? B2F_PACKED_ROW_WORDS * 4 : B2F_ROW_WORDS * 4;
+    const size_t row_bytes = row_bytes_of(m, row_format);
     const int64_t points = 1 + (int64_t)n_words * n_repeats, gp = pi_group_points(n, points);
-    if ((rc = pi_reserve(m, pi.rows, (size_t)n * row_bytes, "the rows")) || (rc = pi_reserve(m, pi.labels, (size_t)n, "the labels")) ||
-        (rc = pi_reserve(m, pi.perm, (size_t)perm_n * 4, "the permutations")) ||
-        (rc = pi_reserve(m, pi.keys, (size_t)gp * n * 16, "the ranking keys")) || (rc = pi_reserve(m, pi.flags, (size_t)gp * n * 2, "the flags")) ||
-        (rc = pi_reserve(m, pi.scores, (size_t)gp * sizeof(PiScore), "the records")) ||
-        (rc = pi_reserve(m, pi.offsets, (size_t)(gp + 1) * 4, "the segment offsets")) ||
-        (rc = pi_reserve(m, pi.segs, (size_t)(gp + 2) * sizeof(PiSeg), "the segments")))
+    const char *who = "permutation scores";
+    if ((rc = compute_reserve(m, pi.rows, (size_t)n * row_bytes, who, "the rows")) || (rc = compute_reserve(m, pi.labels, (size_t)n, who, "the labels")) ||
+        (rc = compute_reserve(m, pi.perm, (size_t)perm_n * 4, who, "the permutations")) ||
+        (rc = compute_reserve(m, pi.keys, (size_t)gp * n * 16, who, "the ranking keys")) ||
+        (rc = compute_reserve(m, pi.flags, (size_t)gp * n * 2, who, "the flags")) ||
+        (rc = compute_reserve(m, pi.scores, (size_t)gp * sizeof(PiScore), who, "the records")) ||
+        (rc = compute_reserve(m, pi.offsets, (size_t)(gp + 1) * 4, who, "the segment offsets")) ||
+        (rc = compute_reserve(m, pi.segs, (size_t)(gp + 2) * sizeof(PiSeg), who, "the segments")))
         return rc;
     uint8_t *d_labels = static_cast<uint8_t *>(pi.labels.p);
     unsigned long long *k0 = static_cast<unsigned long long *>(pi.keys.p), *k1 = k0 + gp * n;
@@ -80,16 +74,13 @@ extern "C" int b2f_permutation_scores(b2f_model *m, const void *rows, int64_t n,
     /* the sort's temporary storage for the largest group */
     size_t temp_bytes = 0;
     CUDA_TRY(pi_segmented_sort(nullptr, &temp_bytes, k0, k1, f0, f1, (int)(gp * n), (int)gp, d_off, st, nullptr));
-    if ((rc = pi_reserve(m, pi.temp, std::max<size_t>(temp_bytes, 1), "the sort's temporary storage"))) return rc;
+    if ((rc = compute_reserve(m, pi.temp, std::max<size_t>(temp_bytes, 1), who, "the sort's temporary storage"))) return rc;
     const size_t smem = pi_smem_bytes((int)h.max_depth);
     CUDA_TRY(cudaFuncSetAttribute(k_permutation_scores<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CUDA_TRY(cudaFuncSetAttribute(k_permutation_scores<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 
-    Events evs;
-    if (device_ms) {
-        if ((rc = evs.create(2))) return rc;
-        CUDA_TRY(cudaEventRecord(evs.e[0], st));
-    }
+    TimedRegion timed{m, device_ms};
+    if ((rc = timed.start())) return rc;
     CUDA_TRY(cudaMemcpyAsync(pi.rows.p, rows, (size_t)n * row_bytes, cudaMemcpyHostToDevice, st));
     std::vector<uint8_t> lab8((size_t)n);
     for (int64_t i = 0; i < n; ++i) lab8[i] = (uint8_t)labels[i];
@@ -128,26 +119,18 @@ extern "C" int b2f_permutation_scores(b2f_model *m, const void *rows, int64_t n,
                 k_permutation_scores<true><<<grid, B2F_PD_WARPS * 32, smem, st>>>(pp, d_segs + s, d_rows, d_labels, d_perm, (long long)n, k0, f0);
             else
                 k_permutation_scores<false><<<grid, B2F_PD_WARPS * 32, smem, st>>>(pp, d_segs + s, d_rows, d_labels, d_perm, (long long)n, k0, f0);
-            const cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_permutation_scores launch failed: %s", cudaGetErrorString(e));
-            m->launches++;
+            if ((rc = launched(m, "k_permutation_scores"))) return rc;
         }
         k_permutation_metrics<<<(unsigned)np, B2F_PI_METRIC_THREADS, 0, st>>>(pp, k0, f0, (long long)n, d_scores);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_permutation_metrics launch failed: %s", cudaGetErrorString(e));
-        m->launches++;
+        if ((rc = launched(m, "k_permutation_metrics"))) return rc;
         size_t tb = pi.temp.bytes;
         int cur = 0;
         CUDA_TRY(pi_segmented_sort(pi.temp.p, &tb, k0, k1, f0, f1, (int)(np * n), (int)np, d_off, st, &cur));
         k_permutation_auc<<<(unsigned)np, B2F_PI_METRIC_THREADS, 0, st>>>(cur ? k1 : k0, cur ? f1 : f0, (long long)n, d_scores);
-        e = cudaGetLastError();
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_permutation_auc launch failed: %s", cudaGetErrorString(e));
-        m->launches++;
+        if ((rc = launched(m, "k_permutation_auc"))) return rc;
         CUDA_TRY(cudaMemcpyAsync(res.data() + g0, d_scores, (size_t)np * sizeof(PiScore), cudaMemcpyDeviceToHost, st));
     }
-    if (device_ms) CUDA_TRY(cudaEventRecord(evs.e[1], st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (device_ms) CUDA_TRY(cudaEventElapsedTime(device_ms, evs.e[0], evs.e[1]));
+    if ((rc = timed.finish())) return rc;
     memcpy(baseline, res.data(), sizeof(PiScore));
     memcpy(out, res.data() + 1, (size_t)(points - 1) * sizeof(PiScore));
     return B2F_OK;

@@ -13,10 +13,9 @@
 
 static_assert(sizeof(b2f_pair_probe) == 16, "b2f_pair_probe layout");
 
-static int pp_check(const b2f_model *m, int fmt, bool have_out) {
-    (void)m;
-    if (fmt == B2F_ROWS_RANKED)
-        return set_err(B2F_EINVAL, "pair dependence takes float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values");
+static int pp_check(int fmt, bool have_out) {
+    const int rc = check_value_rows(fmt, "pair dependence takes");
+    if (rc) return rc;
     if (!have_out) return set_err(B2F_EINVAL, "out is NULL");
     return B2F_OK;
 }
@@ -110,18 +109,10 @@ static int pp_launch(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_
             if (packed) k_pair_dependence<true, false><<<grid, B2F_PD_WARPS * 32, 0, st>>>(p, segs + s, rows, (long long)n, out_dev, 0, 0);
             else k_pair_dependence<false, false><<<grid, B2F_PD_WARPS * 32, 0, st>>>(p, segs + s, rows, (long long)n, out_dev, 0, 0);
         }
-        const cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_pair_dependence launch failed: %s", cudaGetErrorString(e));
-        m->launches++;
+        const int rc = launched(m, "k_pair_dependence");
+        if (rc) return rc;
     }
     return B2F_OK;
-}
-
-/* reserve with the failure reported as B2F_ENOMEM and its byte count */
-static int pp_reserve(b2f_model *m, DevBuf &b, size_t bytes, const char *what) {
-    if (b.reserve(m->compute, bytes, bytes) == B2F_OK) return B2F_OK;
-    (void)cudaGetLastError();
-    return set_err(B2F_ENOMEM, "pair dependence: cannot allocate %zu device bytes for %s", bytes, what);
 }
 
 /* mean = 1 on the compute stream: n >= 1 device rows -> out_dev[P], the spec already at m->pair.spec_dev.  A group is a
@@ -131,7 +122,7 @@ static int pp_mean(b2f_model *m, const void *rows_dev, int64_t n, int fmt, doubl
     const cudaStream_t st = m->compute;
     const int64_t n_cta = (n + B2F_PD_WARPS * 32 - 1) / (B2F_PD_WARPS * 32);
     const int64_t gp = std::min<int64_t>(pp.points, std::max<int64_t>(B2F_PD_SEG, B2F_PERM_SCRATCH_BYTES / (n_cta * (int64_t)sizeof(double))));
-    int rc = pp_reserve(m, pp.partial, (size_t)(n_cta * gp) * sizeof(double), "the per-CTA partial sums");
+    int rc = compute_reserve(m, pp.partial, (size_t)(n_cta * gp) * sizeof(double), "pair dependence", "the per-CTA partial sums");
     if (rc) return rc;
     const PpSeg *segs = reinterpret_cast<const PpSeg *>(pp.spec.data());
     double *partial = static_cast<double *>(pp.partial.p);
@@ -142,22 +133,9 @@ static int pp_mean(b2f_model *m, const void *rows_dev, int64_t n, int fmt, doubl
         const int np = (int)(segs[s1 - 1].off + segs[s1 - 1].count - (uint32_t)point0);
         if ((rc = pp_launch(m, st, rows_dev, n, fmt, true, partial, pp.spec_dev.p, s0, s1, point0, np))) return rc;
         k_pair_dependence_finish<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(partial, (int)n_cta, np, (long long)n, out_dev + point0);
-        const cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return set_err(B2F_ECUDA, "k_pair_dependence_finish launch failed: %s", cudaGetErrorString(e));
-        m->launches++;
+        if ((rc = launched(m, "k_pair_dependence_finish"))) return rc;
         s0 = s1;
     }
-    return B2F_OK;
-}
-
-/* the spec goes to pp.spec_dev on the compute stream (the mean form and the device form), or to pp.host_spec before a
- * host job's chunks (each host call synchronises, so no earlier call still reads it) */
-static int pp_upload_spec(b2f_model *m, DevBuf &buf, bool async) {
-    const size_t bytes = m->pair.spec.size() * sizeof(uint32_t);
-    int rc = pp_reserve(m, buf, bytes, "the point table");
-    if (rc) return rc;
-    if (async) CUDA_TRY(cudaMemcpyAsync(buf.p, m->pair.spec.data(), bytes, cudaMemcpyHostToDevice, m->compute));
-    else CUDA_TRY(cudaMemcpy(buf.p, m->pair.spec.data(), bytes, cudaMemcpyHostToDevice));
     return B2F_OK;
 }
 
@@ -174,11 +152,11 @@ extern "C" int b2f_pair_dependence(b2f_model *m, const void *rows, int64_t n, in
     int rc = pp_prepare(m, probes, n_probes, point_words, mean);
     if (rc) return rc;
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
-    if ((rc = pp_check(m, row_format, out || (n == 0 && !mean)))) return rc;
+    if ((rc = pp_check(row_format, out || (n == 0 && !mean)))) return rc;
     if (!mean) {
         if (n > 0) {
             CUDA_TRY(cudaSetDevice(m->device));
-            if ((rc = pp_upload_spec(m, m->pair.host_spec, false))) return rc;
+            if ((rc = upload_spec(m, m->pair.host_spec, m->pair.spec, false, "pair dependence"))) return rc;
         }
         const HostJob job{(size_t)m->pair.points * sizeof(double), pp_chunk_rows(m), false, 0,
                           [](b2f_model *m, int, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, void *out_dev, int32_t *, DevBuf &) {
@@ -194,21 +172,16 @@ extern "C" int b2f_pair_dependence(b2f_model *m, const void *rows, int64_t n, in
     PairDependence &pp = m->pair;
     const cudaStream_t st = m->compute;
     const size_t row_bytes = row_bytes_of(m, row_format);
-    if ((rc = pp_reserve(m, pp.rows, (size_t)n * row_bytes, "the rows")) || (rc = pp_reserve(m, pp.out, (size_t)pp.points * sizeof(double), "the means")))
+    if ((rc = compute_reserve(m, pp.rows, (size_t)n * row_bytes, "pair dependence", "the rows")) ||
+        (rc = compute_reserve(m, pp.out, (size_t)pp.points * sizeof(double), "pair dependence", "the means")))
         return rc;
-    Events evs;
-    if (device_ms) {
-        if ((rc = evs.create(2))) return rc;
-        CUDA_TRY(cudaEventRecord(evs.e[0], st));
-    }
-    if ((rc = pp_upload_spec(m, pp.spec_dev, true))) return rc;
+    TimedRegion timed{m, device_ms};
+    if ((rc = timed.start())) return rc;
+    if ((rc = upload_spec(m, pp.spec_dev, pp.spec, true, "pair dependence"))) return rc;
     CUDA_TRY(cudaMemcpyAsync(pp.rows.p, rows, (size_t)n * row_bytes, cudaMemcpyHostToDevice, st));
     if ((rc = pp_mean(m, pp.rows.p, n, row_format, static_cast<double *>(pp.out.p)))) return rc;
     CUDA_TRY(cudaMemcpyAsync(out, pp.out.p, (size_t)pp.points * sizeof(double), cudaMemcpyDeviceToHost, st));
-    if (device_ms) CUDA_TRY(cudaEventRecord(evs.e[1], st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (device_ms) CUDA_TRY(cudaEventElapsedTime(device_ms, evs.e[0], evs.e[1]));
-    return B2F_OK;
+    return timed.finish();
 }
 
 extern "C" int b2f_pair_dependence_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const b2f_pair_probe *probes,
@@ -216,13 +189,13 @@ extern "C" int b2f_pair_dependence_device(b2f_model *m, const void *rows_dev, in
     if (!m) return set_err(B2F_EINVAL, "model is NULL");
     if (n < 0) return set_err(B2F_EINVAL, "negative row count");
     int rc = pp_prepare(m, probes, n_probes, point_words, mean);
-    if (rc == B2F_OK) rc = pp_check(m, row_format, out_dev != nullptr || (n == 0 && !mean));
+    if (rc == B2F_OK) rc = pp_check(row_format, out_dev != nullptr || (n == 0 && !mean));
     if (rc == B2F_OK) rc = check_row_format(m, row_format);
     if (rc) return rc;
     if (mean && (n < 1 || n > (int64_t)INT_MAX)) return set_err(B2F_EINVAL, "n = %lld: the mean needs 1 .. 2^31 - 1 rows", (long long)n);
     if (n == 0) return B2F_OK;
     CUDA_TRY(cudaSetDevice(m->device));
-    if ((rc = pp_upload_spec(m, m->pair.spec_dev, true))) return rc;
+    if ((rc = upload_spec(m, m->pair.spec_dev, m->pair.spec, true, "pair dependence"))) return rc;
     if (mean) return pp_mean(m, rows_dev, n, row_format, out_dev);
     return pp_launch(m, m->compute, rows_dev, n, row_format, false, out_dev, m->pair.spec_dev.p, 0, m->pair.n_segs, 0, 0);
 }

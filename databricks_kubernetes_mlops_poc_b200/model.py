@@ -518,6 +518,12 @@ class B200Model:
         out = {s: importance.result(s, rec, base, self.all_features, n_repeats, len(df)) for s in names}
         return out if multi else out[names[0]]
 
+    def _embedding_constants(self, rows: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
+        """Encoded reference rows -> the z-score (mean, scale) of the embedding MMD drift and trust scores share (``mmd.py``)."""
+        n_cat, n_num = len(self.categorical_features), len(self.numeric_features)
+        impute = parse_header(self.flat.blob)["impute"][n_cat:n_cat + n_num]
+        return mmd.standardization(mmd.numerics(rows, n_cat, n_num, impute))
+
     @property
     def mmd_reference_attached(self) -> bool:
         return self.mmd_reference_rows > 0
@@ -531,9 +537,7 @@ class B200Model:
         frame = frame if isinstance(frame, pd.DataFrame) else pd.DataFrame(frame)
         mmd.check_reference(len(frame))
         rows = self.encoder.encode_frame(frame)
-        n_cat, n_num = len(self.categorical_features), len(self.numeric_features)
-        impute = parse_header(self.flat.blob)["impute"][n_cat:n_cat + n_num]
-        mean, scale = mmd.standardization(mmd.numerics(rows, n_cat, n_num, impute))
+        mean, scale = self._embedding_constants(rows)
         self.mmd_reference_rows, self.mmd_sigma = 0, None
         with self.replicas[0].lock:
             try:
@@ -592,9 +596,7 @@ class B200Model:
         cls = trust.class_indices(labels, self.classes)
         trust.check_class_rows(cls, filter_type, k_filter)
         rows = self.encoder.encode_frame(frame)
-        n_cat, n_num = len(self.categorical_features), len(self.numeric_features)
-        impute = parse_header(self.flat.blob)["impute"][n_cat:n_cat + n_num]
-        mean, scale = mmd.standardization(mmd.numerics(rows, n_cat, n_num, impute))
+        mean, scale = self._embedding_constants(rows)
         positions = np.arange(len(frame))
         self.trust_reference_rows, self._trust_positions = None, None
         with self.replicas[0].lock:

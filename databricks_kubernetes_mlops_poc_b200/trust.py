@@ -20,7 +20,8 @@ from __future__ import annotations
 
 import numpy as np
 
-MAX_REFERENCE = 131072  # B2F_MMD_MAX_REF
+from .mmd import MAX_REFERENCE
+
 MAX_K = 64  # B2F_KNN_MAX_K
 MAX_K_FILTER = MAX_K - 1
 FILTER_TYPES = (None, "distance_knn")
