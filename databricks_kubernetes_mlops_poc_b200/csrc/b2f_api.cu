@@ -162,10 +162,9 @@ struct Slot {
 struct Explainer; /* an attached path table (explain_api.cuh) */
 static void explainer_free(Explainer *ex);
 
-/* partial dependence (b2f_partial_dependence; partial_dependence.cuh).  The forest fields of pp are set at model creation;
- * segs, grid and points are the current call's. */
+/* partial dependence (b2f_partial_dependence; partial_dependence.cuh): the current call's spec and point count */
 struct Dependence {
-    PdParams pp;
+    int32_t points = 0; /* doubles per output row */
     int n_segs = 0;
     std::vector<uint32_t> spec; /* the call's PdSeg table, then its grid words */
     DevBuf host_spec;           /* a host call's spec on the device */
@@ -184,7 +183,7 @@ struct PairDependence {
 };
 
 /* nearest single-field counterfactuals (b2f_counterfactual; counterfactual.cuh).  The split-value table is built on the
- * first call; the forest fields of cp are set at model creation, the probe fields are the current call's. */
+ * first call; cp.pd is the model's walk parameters, set at model creation, the probe fields are the current call's. */
 struct Counterfactual {
     CfParams cp;
     bool built = false;
@@ -275,6 +274,7 @@ struct b2f_model {
     void *d_blob = nullptr;
     int64_t forest_bytes = 0;
     Explainer *ex = nullptr; /* attached TreeSHAP path table (b2f_model_attach_explainer) */
+    PdParams walk; /* the forest fields every mask-walk kernel reads (K6, K7, K8, K10); segs, grid and points are a call's */
     Dependence pd;
     PairDependence pair;
     Counterfactual cf;
@@ -794,7 +794,7 @@ static int warp_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
         kp.g[g].n_leaf_slots = gt[g].n_leaf_slots;
         kp.g[g].depth = gt[g].depth;
     }
-    PdParams &pp = m->pd.pp;
+    PdParams &pp = m->walk;
     memset(&pp, 0, sizeof(pp));
     pp.chunks = kp.chunks;
     pp.n_groups = kp.n_groups;
@@ -1422,6 +1422,21 @@ static int check_value_rows(int fmt, const char *subject) {
     if (fmt == B2F_ROWS_RANKED)
         return set_err(B2F_EINVAL, "%s float32 rows (B2F_ROWS_WORDS24 / B2F_ROWS_PACKED64): ranked rows carry no values", subject);
     return B2F_OK;
+}
+
+/* a mask walk holds at most one stack entry per level of the tree; subject: the caller with its verb ("counterfactuals walk") */
+static int check_walk_depth(const b2f_model *m, const char *subject) {
+    const b2f_blob_header &h = m->hdr;
+    if (h.max_depth > B2F_PD_STACK) return set_err(B2F_EINVAL, "%s trees of depth <= %d; this forest has depth %u", subject, B2F_PD_STACK, h.max_depth);
+    return B2F_OK;
+}
+
+/* a mask-walk spec: the segment table, then the point words */
+template <typename Seg>
+static void pack_spec(std::vector<uint32_t> &spec, const std::vector<Seg> &segs, const std::vector<uint32_t> &words) {
+    spec.assign(segs.size() * (sizeof(Seg) / sizeof(uint32_t)), 0u);
+    memcpy(spec.data(), segs.data(), segs.size() * sizeof(Seg));
+    spec.insert(spec.end(), words.begin(), words.end());
 }
 
 /* a call's spec into buf: synchronously, before a host job's chunks (each host call synchronises, so no earlier call still

@@ -10,9 +10,9 @@
  *     upper = t'_{k-1}          for the least k > j that flips  (the smallest float32 above x that flips)
  *     lower = nextdown(t'_k)    for the greatest k < j that flips (the largest float32 below x that flips)
  *
- * k_counterfactual scores every piece of every probed word with K6's mask walk (partial_dependence.cuh pd_mask_walk, the
- * same device function): thread = row, warp = 32-row tile, CTA = B2F_PD_WARPS tiles x one segment (blockIdx.y) of up to
- * 32 consecutive pieces of one word.  A piece's point is its representative, t'_{k-1} (nextdown(t'_0) for piece 0), read
+ * k_counterfactual scores every piece of every probed word with the mask walk of the what-if kernels (partial_dependence.cuh
+ * pd_mask_walk): thread = row, warp = 32-row tile, CTA = B2F_PD_WARPS tiles x one segment (blockIdx.y) of up to 32
+ * consecutive pieces of one word.  A piece's point is its representative, t'_{k-1} (nextdown(t'_0) for piece 0), read
  * from the model's split-value table in HBM.  Each thread finds its own j by binary search in the same table.  The
  * epilogue turns the 32 accumulators into p1 with aggregate() -- the tile kernel's order, so each p1 is bit for bit the
  * tile kernel's score of the row with the word set to the representative -- and writes one 32-byte CfCand per (row,

@@ -78,8 +78,7 @@ static int cf_prepare(b2f_model *m, int64_t n, int fmt, const int32_t *words, in
                            "(score its categories with b2f_partial_dependence)",
                            i, words[i], h.n_cat, h.n_cat + h.n_num - 1);
     if (!std::isfinite(cutoff) || cutoff < 0.0 || cutoff > 1.0) return set_err(B2F_EINVAL, "cutoff %g: expected a number in [0, 1]", cutoff);
-    if (h.max_depth > B2F_PD_STACK) return set_err(B2F_EINVAL, "counterfactuals walk trees of depth <= %d; this forest has depth %u", B2F_PD_STACK, h.max_depth);
-    if ((rc = cf_build_table(m))) return rc;
+    if ((rc = check_walk_depth(m, "counterfactuals walk")) || (rc = cf_build_table(m))) return rc;
     CfParams &cp = m->cf.cp;
     cp.cutoff = cutoff;
     cp.n_words = n_words;

@@ -9,7 +9,7 @@
 /* device bytes of one chunk's partial-dependence curves: the chunk's rows are this over the row's bytes, 1 024 to 16 384 */
 #define B2F_PD_CHUNK_BYTES (64ll << 20)
 static int64_t pd_chunk_rows(const b2f_model *m) {
-    const int64_t rows = B2F_PD_CHUNK_BYTES / ((int64_t)m->pd.pp.points * (int64_t)sizeof(double));
+    const int64_t rows = B2F_PD_CHUNK_BYTES / ((int64_t)m->pd.points * (int64_t)sizeof(double));
     return std::max<int64_t>(1024, std::min<int64_t>(B2F_CHUNK_ROWS, rows / 32 * 32));
 }
 
@@ -28,7 +28,8 @@ static int pd_prepare(b2f_model *m, const b2f_pd_probe *probes, int n_probes, co
     const b2f_blob_header &h = m->hdr;
     if (!probes || !grid_words) return set_err(B2F_EINVAL, "probes or grid_words is NULL");
     if (n_probes < 1 || n_probes > B2F_PD_MAX_PROBES) return set_err(B2F_EINVAL, "n_probes = %d: expected 1..%d", n_probes, B2F_PD_MAX_PROBES);
-    if (h.max_depth > B2F_PD_STACK) return set_err(B2F_EINVAL, "partial dependence walks trees of depth <= %d; this forest has depth %u", B2F_PD_STACK, h.max_depth);
+    const int rc = check_walk_depth(m, "partial dependence walks");
+    if (rc) return rc;
     const int fields = (int)(h.n_cat + h.n_num);
     std::vector<PdSeg> segs;
     std::vector<uint32_t> words;
@@ -58,19 +59,18 @@ static int pd_prepare(b2f_model *m, const b2f_pd_probe *probes, int n_probes, co
     }
     Dependence &pd = m->pd;
     pd.n_segs = (int)segs.size();
-    pd.pp.points = (int32_t)words.size();
-    pd.spec.assign(segs.size() * (sizeof(PdSeg) / sizeof(uint32_t)), 0u);
-    memcpy(pd.spec.data(), segs.data(), segs.size() * sizeof(PdSeg));
-    pd.spec.insert(pd.spec.end(), words.begin(), words.end());
+    pd.points = (int32_t)words.size();
+    pack_spec(pd.spec, segs, words);
     return B2F_OK;
 }
 
 /* out_dev[n][points] for n device rows of format fmt on stream st; spec_dev holds the call's spec */
 static int launch_dependence(b2f_model *m, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, double *out_dev, const void *spec_dev) {
     if (n <= 0) return B2F_OK;
-    PdParams pp = m->pd.pp;
+    PdParams pp = m->walk;
     pp.segs = static_cast<const PdSeg *>(spec_dev);
     pp.grid = reinterpret_cast<const uint32_t *>(pp.segs + m->pd.n_segs);
+    pp.points = m->pd.points;
     const dim3 grid((unsigned)((n + B2F_PD_WARPS * 32 - 1) / (B2F_PD_WARPS * 32)), (unsigned)m->pd.n_segs);
     const uint32_t *rows = static_cast<const uint32_t *>(rows_dev);
     if (fmt == B2F_ROWS_PACKED64)
@@ -93,7 +93,7 @@ extern "C" int b2f_partial_dependence(b2f_model *m, const void *rows, int64_t n,
         CUDA_TRY(cudaSetDevice(m->device));
         if ((rc = upload_spec(m, m->pd.host_spec, m->pd.spec, false, nullptr))) return rc;
     }
-    const HostJob job{(size_t)m->pd.pp.points * sizeof(double), pd_chunk_rows(m), false, 0,
+    const HostJob job{(size_t)m->pd.points * sizeof(double), pd_chunk_rows(m), false, 0,
                       [](b2f_model *m, int, cudaStream_t st, const void *rows_dev, int64_t n, int fmt, void *out_dev, int32_t *, DevBuf &) {
                           return launch_dependence(m, st, rows_dev, n, fmt, static_cast<double *>(out_dev), m->pd.host_spec.p);
                       }};

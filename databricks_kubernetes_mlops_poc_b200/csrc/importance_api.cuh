@@ -43,8 +43,7 @@ extern "C" int b2f_permutation_scores(b2f_model *m, const void *rows, int64_t n,
     if (n_words < 1 || n_words > fields) return set_err(B2F_EINVAL, "n_words = %d: expected 1..%d", n_words, fields);
     for (int i = 0; i < n_words; ++i)
         if (words[i] < 0 || words[i] >= fields) return set_err(B2F_EINVAL, "words[%d] = %d: outside the %d fields", i, words[i], fields);
-    if (h.max_depth > B2F_PD_STACK)
-        return set_err(B2F_EINVAL, "permutation scores walk trees of depth <= %d; this forest has depth %u", B2F_PD_STACK, h.max_depth);
+    if ((rc = check_walk_depth(m, "permutation scores walk"))) return rc;
     for (int64_t i = 0; i < n; ++i)
         if (labels[i] != 0 && labels[i] != 1) return set_err(B2F_EINVAL, "labels[%lld] = %d: expected 0 or 1", (long long)i, labels[i]);
     const int64_t perm_n = (int64_t)n_repeats * n;
@@ -91,7 +90,7 @@ extern "C" int b2f_permutation_scores(b2f_model *m, const void *rows, int64_t n,
     CUDA_TRY(cudaMemcpyAsync(d_off, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice, st));
 
     std::vector<PiScore> res((size_t)points);
-    const PdParams &pp = m->pd.pp; /* the forest fields (segs, grid and points unused) */
+    const PdParams &pp = m->walk;
     const uint32_t *d_rows = static_cast<const uint32_t *>(pi.rows.p);
     const int32_t *d_perm = static_cast<const int32_t *>(pi.perm.p);
     const unsigned bx = (unsigned)((n + B2F_PD_WARPS * 32 - 1) / (B2F_PD_WARPS * 32));

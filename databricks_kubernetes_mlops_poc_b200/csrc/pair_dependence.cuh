@@ -3,8 +3,9 @@
  *
  * For every row i and every point (u, v) of a probed pair of request fields (a, b), the kernel returns the prediction of
  * row i with row word a replaced by u and row word b by v -- sklearn's two-way `partial_dependence(..., [a, b],
- * method="brute")` `individual` curves.  It is K6's mask walk (partial_dependence.cuh) over two probed words: each (row,
- * tree, segment of up to 32 points) is one walk with an explicit stack of (node, point mask) that
+ * method="brute")` `individual` curves.  It is K6's mask walk over two probed words (partial_dependence.cuh pd_mask_walk
+ * with TWO = true): each (row, tree, segment of up to 32 points) is one walk with an explicit stack of (node, point
+ * mask) that
  *
  *   split on word a       : splits the mask on take_second(u_k)
  *   split on word b       : splits the mask on take_second(v_k)
@@ -41,55 +42,6 @@ struct PpSeg {
     uint32_t off;    /* first point: its column in an output row, and its index in the point table (2 words per point) */
 };
 
-/* The two-word mask walk: pd_mask_walk (partial_dependence.cuh) with a second probed word.  gva[k] / gvb[k] (shared) are
- * the words point k puts at word_a / word_b; the rest as pd_mask_walk. */
-__device__ __forceinline__ void pd_mask_walk(const PdParams &p, uint32_t word_a, uint32_t word_b, uint32_t full, const uint32_t *gva,
-                                             const uint32_t *gvb, const uint32_t (*xw)[32], int lane,
-                                             unsigned long long (*stk)[B2F_PD_WARPS * 32], double (&acc)[B2F_PD_SEG]) {
-    for (int g = 0; g < p.n_groups; ++g) {
-        const uint8_t *chunk = p.chunks + p.g_off[g];
-        const size_t leaf_area = (size_t)p.g_slots[g] * B2F_NODE_STRIDE;
-        const int n_trees = (int)p.g_trees[g];
-        for (int l = 0; l < n_trees; ++l) { /* tree 32 g + l: tree order */
-            const uint8_t *nodes = chunk + l * 8;
-            uint32_t node = 0, mask = full;
-            int sp = 0;
-            while (true) {
-                const uint2 tm = __ldg(reinterpret_cast<const uint2 *>(nodes + (size_t)node * B2F_NODE_STRIDE));
-                const uint32_t first = tm.y & B2F_META_SLOT_MASK;
-                if (first == node) { /* a leaf is the only node that is its own first child */
-                    const double v = __ldg(reinterpret_cast<const double *>(nodes + leaf_area + (size_t)tm.x * B2F_NODE_STRIDE));
-#pragma unroll
-                    for (int k = 0; k < B2F_PD_SEG; ++k)
-                        if ((mask >> k) & 1u) acc[k] += v;
-                    if (sp == 0) break;
-                    const unsigned long long e = stk[--sp][threadIdx.x];
-                    node = (uint32_t)e;
-                    mask = (uint32_t)(e >> 32);
-                    continue;
-                }
-                const uint32_t feat = tm.y >> B2F_META_FEAT_SHIFT;
-                if (feat == word_a || feat == word_b) {
-                    const uint32_t *gv = feat == word_a ? gva : gvb;
-                    uint32_t sec = 0;
-#pragma unroll
-                    for (int k = 0; k < B2F_PD_SEG; ++k) sec |= (take_second(gv[k], tm.x, tm.y) ? 1u : 0u) << k;
-                    const uint32_t m2 = mask & sec, m1 = mask & ~sec;
-                    if (m1 && m2) { /* fork: the second child waits on the stack */
-                        stk[sp++][threadIdx.x] = ((unsigned long long)m2 << 32) | (first + 1u);
-                        node = first;
-                        mask = m1;
-                    } else {
-                        node = first + (m2 ? 1u : 0u);
-                    }
-                } else {
-                    node = first + (take_second(xw[feat][lane], tm.x, tm.y) ? 1u : 0u);
-                }
-            }
-        }
-    }
-}
-
 /* p.grid: the call's point table, (a word, b word) per point, numerics imputed; p.points: doubles per output row (MEAN =
  * false).  segs: this launch's segments (blockIdx.y).  MEAN = false: out[row * p.points + point]; MEAN = true:
  * out[blockIdx.x * group_points + point - point0], the CTA's partial sums of the launch's group of points. */
@@ -118,7 +70,7 @@ __global__ void __launch_bounds__(B2F_PD_WARPS * 32)
     double acc[B2F_PD_SEG];
 #pragma unroll
     for (int k = 0; k < B2F_PD_SEG; ++k) acc[k] = p.agg_mode == B2F_AGG_GBDT_LOGISTIC ? p.init_raw : 0.0;
-    if (live) pd_mask_walk(p, sg.word_a, sg.word_b, full, gv[0], gv[1], xs[warp], lane, stk, acc);
+    if (live) pd_mask_walk<1, true>(p, sg.word_a, full, gv[0], xs[warp], lane, stk, acc, sg.word_b, gv[1]);
 
 #pragma unroll
     for (int k = 0; k < B2F_PD_SEG; ++k) {

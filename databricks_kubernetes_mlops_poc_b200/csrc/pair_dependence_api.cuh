@@ -40,7 +40,8 @@ static int pp_prepare(b2f_model *m, const b2f_pair_probe *probes, int n_probes, 
     if (!probes || !point_words) return set_err(B2F_EINVAL, "probes or point_words is NULL");
     if (mean != 0 && mean != 1) return set_err(B2F_EINVAL, "mean = %d: expected 0 or 1", mean);
     if (n_probes < 1 || n_probes > B2F_PAIR_MAX_PROBES) return set_err(B2F_EINVAL, "n_probes = %d: expected 1..%d", n_probes, B2F_PAIR_MAX_PROBES);
-    if (h.max_depth > B2F_PD_STACK) return set_err(B2F_EINVAL, "pair dependence walks trees of depth <= %d; this forest has depth %u", B2F_PD_STACK, h.max_depth);
+    int rc = check_walk_depth(m, "pair dependence walks");
+    if (rc) return rc;
     const int fields = (int)(h.n_cat + h.n_num);
     int64_t total = 0;
     for (int i = 0; i < n_probes; ++i) {
@@ -63,8 +64,7 @@ static int pp_prepare(b2f_model *m, const b2f_pair_probe *probes, int n_probes, 
         const b2f_pair_probe pr = probes[i];
         for (int k = 0; k < pr.count; ++k) {
             uint32_t a = point_words[2 * ((size_t)pr.point_offset + k)], b = point_words[2 * ((size_t)pr.point_offset + k) + 1];
-            int rc = pp_point_word(h, i, k, pr.word_a, a);
-            if (rc) return rc;
+            if ((rc = pp_point_word(h, i, k, pr.word_a, a))) return rc;
             if (pr.word_b >= 0 && (rc = pp_point_word(h, i, k, pr.word_b, b))) return rc;
             if (pr.word_b < 0) b = 0u;
             if (k % B2F_PD_SEG == 0)
@@ -76,17 +76,14 @@ static int pp_prepare(b2f_model *m, const b2f_pair_probe *probes, int n_probes, 
     }
     pp.n_segs = (int)segs.size();
     pp.points = total;
-    pp.spec.assign(segs.size() * (sizeof(PpSeg) / sizeof(uint32_t)), 0u);
-    memcpy(pp.spec.data(), segs.data(), segs.size() * sizeof(PpSeg));
-    pp.spec.insert(pp.spec.end(), words.begin(), words.end());
+    pack_spec(pp.spec, segs, words);
     return B2F_OK;
 }
 
-/* the forest fields of K6's parameters with this call's point table at spec_dev */
+/* the model's walk parameters with this call's point table at spec_dev */
 static PdParams pp_params(const b2f_model *m, const void *spec_dev, const PpSeg **segs) {
-    PdParams p = m->pd.pp;
+    PdParams p = m->walk;
     *segs = static_cast<const PpSeg *>(spec_dev);
-    p.segs = nullptr;
     p.grid = reinterpret_cast<const uint32_t *>(*segs + m->pair.n_segs);
     p.points = (int32_t)std::min<int64_t>(m->pair.points, INT_MAX);
     return p;

@@ -22,7 +22,8 @@
  * tile kernel's order -- so a point equals, bit for bit, k_forest_predict_tile on the row with the word replaced.  No
  * atomics; a row's outputs depend on nothing but the row, the forest and the grid.
  *
- * The mask walk is pd_mask_walk, which K7 (counterfactual.cuh) calls as well.
+ * The mask walk is pd_mask_walk, which K7 (counterfactual.cuh), K8 (permutation_importance.cuh) and K10
+ * (pair_dependence.cuh, with a second probed word) call as well.
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -63,7 +64,8 @@ struct PdParams {
 
 /* Stage this lane's row into xw[word][lane] (its warp's tile): decode, impute the numerics, sentinel above the fields
  * (k_forest_predict_tile's staging).  A dead lane stages sentinels.  k_partial_dependence keeps its own inline copy of
- * these lines: through this function its SASS would change (same work, another instruction schedule). */
+ * these lines: through this function its PACKED instance takes 96 registers instead of 100, so 5 CTAs per SM instead of 4,
+ * which is faster on large grids and slower on small ones (DESIGN.md, K6). */
 template <bool PACKED>
 __device__ __forceinline__ void pd_stage_row(const PdParams &p, const uint32_t *__restrict__ rows, long long row, bool live,
                                              uint32_t (*xw)[32], int lane) {
@@ -103,12 +105,15 @@ __device__ __forceinline__ void pd_stage_row(const PdParams &p, const uint32_t *
 }
 
 /* The mask walk: acc[k] += every leaf payload that point k of a segment reaches, tree by tree in tree order.  One walk per
- * (row, tree) forks only at splits on row word `word`, with gv[k * PSTRIDE] (shared) the word point k puts there and `full`
+ * (row, tree) forks only at splits on row word `word`, with gva[k * PSTRIDE] (shared) the word point k puts there and `full`
  * the mask of the segment's points; xw = the warp's staged rows; stk = the block's walk stacks, column threadIdx.x this
- * thread's.  PSTRIDE = 1: one point table for the block (K6, K7); K8 passes its thread's column of a per-thread table. */
-template <int PSTRIDE = 1>
-__device__ __forceinline__ void pd_mask_walk(const PdParams &p, uint32_t word, uint32_t full, const uint32_t *gv, const uint32_t (*xw)[32],
-                                             int lane, unsigned long long (*stk)[B2F_PD_WARPS * 32], double (&acc)[B2F_PD_SEG]) {
+ * thread's.  PSTRIDE = 1: one point table for the block (K6, K7, K10); K8 passes its thread's column of a per-thread table.
+ * TWO = true (K10) also forks at splits on word_b, with gvb[k * PSTRIDE] point k's word there; TWO = false ignores word_b
+ * and gvb, so the one-word walk carries no second compare. */
+template <int PSTRIDE = 1, bool TWO = false>
+__device__ __forceinline__ void pd_mask_walk(const PdParams &p, uint32_t word, uint32_t full, const uint32_t *gva, const uint32_t (*xw)[32],
+                                             int lane, unsigned long long (*stk)[B2F_PD_WARPS * 32], double (&acc)[B2F_PD_SEG],
+                                             uint32_t word_b = 0u, const uint32_t *gvb = nullptr) {
     for (int g = 0; g < p.n_groups; ++g) {
         const uint8_t *chunk = p.chunks + p.g_off[g];
         const size_t leaf_area = (size_t)p.g_slots[g] * B2F_NODE_STRIDE;
@@ -132,7 +137,8 @@ __device__ __forceinline__ void pd_mask_walk(const PdParams &p, uint32_t word, u
                     continue;
                 }
                 const uint32_t feat = tm.y >> B2F_META_FEAT_SHIFT;
-                if (feat == word) {
+                if (feat == word || (TWO && feat == word_b)) {
+                    const uint32_t *gv = (!TWO || feat == word) ? gva : gvb;
                     uint32_t sec = 0;
 #pragma unroll
                     for (int k = 0; k < B2F_PD_SEG; ++k) sec |= (take_second(gv[k * PSTRIDE], tm.x, tm.y) ? 1u : 0u) << k;

@@ -3,9 +3,9 @@
  *
  * sklearn's permutation_importance shuffles one column at a time, rescores every row and reports the drop in a metric.
  * Row i with field f taken from row sigma_r(i) differs from row i in one row word, so all repeats r of a (row, tree,
- * field) are one mask walk that forks only at splits on that word -- K6's pd_mask_walk (partial_dependence.cuh), except that
- * the points differ per lane: lane t's point k is word f of row sigma_{r0+k}(t's row), gathered from the device copy of
- * every row (pd_mask_walk<T> reads column threadIdx.x of a per-thread point table).
+ * field) are one mask walk that forks only at splits on that word -- the what-if kernels' pd_mask_walk
+ * (partial_dependence.cuh), except that the points differ per lane: lane t's point k is word f of row sigma_{r0+k}(t's
+ * row), gathered from the device copy of every row (pd_mask_walk<T> reads column threadIdx.x of a per-thread point table).
  *
  * k_permutation_scores: thread = row, warp = 32-row tile, CTA = B2F_PD_WARPS tiles x one segment (blockIdx.y) = one
  * probed word and up to 32 consecutive repeats.  The baseline is a segment with no probed word (one point: the row as it

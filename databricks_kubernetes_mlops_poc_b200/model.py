@@ -168,10 +168,7 @@ class B200Model:
 
     def predict(self, model_input) -> dict:
         """Mirror of ``CustomModel.predict(context, model_input)`` (02-register-model.ipynb:330-353)."""
-        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)  # never mutated here
-        if len(df.columns) == 0:
-            # the reference dies in df[self.all_features] on an empty request (-> HTTP 500)
-            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        df = self._frame(model_input)
         # the drift sweep takes milliseconds of device time on its own stream (2.2 ms for 1 000 rows on an H100): start it
         # first, score the rows meanwhile
         pending = self._pool.submit(self.drift.score, df) if self.drift is not None else None
@@ -185,6 +182,13 @@ class B200Model:
             "feature_drift_batch": dict(zip(self.all_features, drift_scores)),
         }
 
+    def _frame(self, model_input) -> pd.DataFrame:
+        """A request as a frame (never mutated here); KeyError when it has no columns, as the reference raises from
+        ``df[self.all_features]`` on an empty request (-> HTTP 500)."""
+        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
+        if len(df.columns) == 0:
+            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        return df
 
     def _predictions(self, df: pd.DataFrame):
         """-> (predictions list, outlier-flag list): what ``predict`` returns for these rows, without the drift scores."""
@@ -289,23 +293,13 @@ class B200Model:
         ``grid_frame``, or of ``model_input`` without one; missing values never enter a default grid.  At most 256 points per
         feature and 23 features per call.  Every model has it, with or without an explainer.  Rows with NaN numerics are
         accepted (the classifier alone is scored).  It runs on the first GPU's handle only, like ``explain``."""
-        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
-        if len(df.columns) == 0:
-            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        df = self._frame(model_input)
         features = dependence.check_request(features, self.all_features, kind)
-        custom_values = dict(custom_values or {})
-        unknown = [f for f in custom_values if f not in self.all_features]
-        if unknown:
-            raise ValueError(f"custom_values for unknown feature(s) {unknown}")
+        grid_of = self._grid_rule(custom_values, grid_resolution, percentiles, dependence.MAX_POINTS)
         source = df if grid_frame is None else grid_frame
         grids, words, probes, off = [], [], [], 0
         for name in features:
-            if name in custom_values:
-                grid = list(custom_values[name])
-            else:
-                grid = dependence.grid_from_column(source[name], name in self.categorical_features, grid_resolution, percentiles).tolist()
-            if not 1 <= len(grid) <= dependence.MAX_POINTS:
-                raise ValueError(f"feature {name!r}: {len(grid)} grid points, expected 1..{dependence.MAX_POINTS}")
+            grid = grid_of(name, source)
             grids.append(grid)
             words.append(dependence.encode_grid(self.encoder, name, grid))
             probes.append((dependence.word_of(self.encoder, name), off, len(grid)))
@@ -323,26 +317,36 @@ class B200Model:
         ``dependence.grid_from_column`` over ``grid_frame``'s column, or ``model_input``'s.  ValueError for an unknown field,
         a pair of one field, or an axis outside 1..256 points."""
         pairs = interaction.check_pairs(pairs, self.all_features)
-        custom_values = dict(custom_values or {})
-        unknown = [f for f in custom_values if f not in self.all_features]
-        if unknown:
-            raise ValueError(f"custom_values for unknown feature(s) {unknown}")
+        grid_of = self._grid_rule(custom_values, grid_resolution, percentiles, interaction.MAX_AXIS_POINTS)
         source = model_input if grid_frame is None else grid_frame
         source = source if isinstance(source, pd.DataFrame) else pd.DataFrame(source)
         cache, out = {}, []
         for pair in pairs:
             for name in pair:
-                if name in cache:
-                    continue
-                if name in custom_values:
-                    grid = list(custom_values[name])
-                else:
-                    grid = dependence.grid_from_column(source[name], name in self.categorical_features, grid_resolution, percentiles).tolist()
-                if not 1 <= len(grid) <= interaction.MAX_AXIS_POINTS:
-                    raise ValueError(f"feature {name!r}: {len(grid)} grid points, expected 1..{interaction.MAX_AXIS_POINTS}")
-                cache[name] = grid
+                if name not in cache:
+                    cache[name] = grid_of(name, source)
             out.append([cache[pair[0]], cache[pair[1]]])
         return out
+
+    def _grid_rule(self, custom_values: dict | None, grid_resolution: int, percentiles, max_points: int):
+        """-> grid_of(name, source): the grid of a probed field, ``custom_values[name]`` when given, else the default rule of
+        ``dependence.grid_from_column`` over ``source[name]``.  ValueError for custom values of an unknown field (here) or a
+        grid outside 1..max_points points (from grid_of)."""
+        custom_values = dict(custom_values or {})
+        unknown = [f for f in custom_values if f not in self.all_features]
+        if unknown:
+            raise ValueError(f"custom_values for unknown feature(s) {unknown}")
+
+        def grid_of(name: str, source) -> list:
+            if name in custom_values:
+                grid = list(custom_values[name])
+            else:
+                grid = dependence.grid_from_column(source[name], name in self.categorical_features, grid_resolution, percentiles).tolist()
+            if not 1 <= len(grid) <= max_points:
+                raise ValueError(f"feature {name!r}: {len(grid)} grid points, expected 1..{max_points}")
+            return grid
+
+        return grid_of
 
     def pair_dependence(self, model_input, pairs, *, kind: str = "average", grid_resolution: int = 100, percentiles=(0.05, 0.95),
                         custom_values: dict | None = None, grid_frame: pd.DataFrame | None = None) -> dict:
@@ -356,9 +360,7 @@ class B200Model:
         copying the curves), ``individual`` is there for "individual" and "both".  Grids follow ``pair_grids``: at most 256
         points per axis.  ``pairs``: one pair or a list of them.  Every model has it; rows with NaN numerics are accepted
         (the classifier alone is scored).  It runs on the first GPU's handle only, under ``replicas[0].lock``."""
-        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
-        if len(df.columns) == 0:
-            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        df = self._frame(model_input)
         if kind not in dependence.KINDS:
             raise ValueError(f"kind={kind!r}: expected one of {dependence.KINDS}")
         pairs = interaction.check_pairs(pairs, self.all_features)
@@ -397,9 +399,7 @@ class B200Model:
         sums are float64 numpy in a fixed order.  ValueError for an unknown or repeated field, fewer than two fields, a
         sample outside 2..10 000, a bad seed or fewer than two rows.  It runs on the first GPU's handle only, under
         ``replicas[0].lock``."""
-        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
-        if len(df.columns) == 0:
-            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        df = self._frame(model_input)
         features = interaction.check_features(features, self.all_features)
         sample, random_state = interaction.check_sample(sample, random_state)
         S = interaction.sample_rows(len(df), sample, random_state)
@@ -430,9 +430,7 @@ class B200Model:
         where P(class 1) rounds to exactly 0.5.  ``features=None`` probes every field; unknown or repeated names raise
         ValueError, as does a cutoff outside [0, 1].  Every model has it, with or without an explainer; rows with NaN
         numerics are accepted.  It runs on the first GPU's handle only, like ``partial_dependence``."""
-        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
-        if len(df.columns) == 0:
-            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        df = self._frame(model_input)
         features = list(self.all_features) if features is None else ([features] if isinstance(features, str) else list(features))
         if not features:
             raise ValueError("at least one feature is needed")
@@ -503,9 +501,7 @@ class B200Model:
         ValueError there, as sklearn does.  It runs on the first GPU's handle only, under ``replicas[0].lock``."""
         names, multi = importance.check_scoring(scoring)
         n_repeats = importance.check_n_repeats(n_repeats)
-        df = df if isinstance(df, pd.DataFrame) else pd.DataFrame(df)
-        if len(df.columns) == 0:
-            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        df = self._frame(df)
         labels = importance.check_labels(y, len(df))
         if len(df) == 0:
             raise ValueError("permutation importance needs at least one row")
@@ -560,9 +556,7 @@ class B200Model:
         if not self.mmd_reference_attached:
             raise RuntimeError("this model has no MMD reference: attach_mmd_reference(frame), from_pipeline(..., mmd_reference=frame) "
                                f"or a model directory that holds {MMD_FILE} (save_model_dir(..., mmd_reference=frame))")
-        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
-        if len(df.columns) == 0:
-            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        df = self._frame(model_input)
         n_ref = self.mmd_reference_rows
         n_permutations, p_val, random_state = mmd.check_request(len(df), n_ref, n_permutations, p_val, random_state)
         rows = self.encoder.encode_frame(df)
@@ -626,9 +620,7 @@ class B200Model:
         if not self.trust_reference_attached:
             raise RuntimeError("this model has no trust reference: attach_trust_reference(frame), from_pipeline(..., trust_reference=frame) "
                                f"or a model directory that holds {TRUST_FILE} (save_model_dir(..., trust_reference=frame))")
-        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
-        if len(df.columns) == 0:
-            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        df = self._frame(model_input)
         k, dist_type = trust.check_score(k, dist_type, self.trust_reference_rows)
         if len(df) == 0:
             raise ValueError("trust scores need at least one row")
@@ -662,9 +654,7 @@ class B200Model:
         if self.explain_blob is None:
             raise RuntimeError("this model has no explainer: build it with from_pipeline(..., explain=True) or load a model directory "
                                f"that holds {EXPLAIN_FILE} (save_model_dir(..., explain_blob=flatten_explainer(pipeline)))")
-        df = model_input if isinstance(model_input, pd.DataFrame) else pd.DataFrame(model_input)
-        if len(df.columns) == 0:
-            raise KeyError(f"None of {self.all_features} are in the [columns]")
+        df = self._frame(model_input)
         rows = self.encoder.encode_frame(df)
         with self.replicas[0].lock:
             values, base = getattr(self.engine, method)(rows)

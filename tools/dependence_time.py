@@ -10,10 +10,12 @@ Per model and workload:
   field), host clock, one run;
 * sklearn_1000_ms: sklearn's partial_dependence(method="brute") on 1 000 of the rows on the host CPUs (workload (b) for
   rf100d6 only), once.
-Requests are the benchmark's synthetic rows."""
+Requests are the benchmark's synthetic rows, as 24-word rows, or with B2F_TOOL_ROWS=packed as 64-byte packed rows
+(ROWS_PACKED64, written to dependence_time_packed.json); the expanded predict path takes the 24-word rows either way."""
 import json, os, sys, time
 
 OUT = os.environ.get("B2F_TOOL_OUT", "tools_out")  # where the result file goes
+PACKED = os.environ.get("B2F_TOOL_ROWS", "words24") == "packed"  # the row format K6 reads
 import numpy as np
 import pandas as pd
 
@@ -21,6 +23,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402  (its GBDT recipe and the card record)
 from databricks_kubernetes_mlops_poc_b200 import dependence, training  # noqa: E402
+from databricks_kubernetes_mlops_poc_b200._cabi import ROWS_PACKED64, ROWS_WORDS24  # noqa: E402
 from databricks_kubernetes_mlops_poc_b200.encode import RowEncoder  # noqa: E402
 from databricks_kubernetes_mlops_poc_b200.engine import ForestEngine  # noqa: E402
 from databricks_kubernetes_mlops_poc_b200.flatten import flatten_pipeline  # noqa: E402
@@ -58,11 +61,15 @@ def main():
     grids = {f: dependence.grid_from_column(curated[f], f in rp.CATEGORICAL_FEATURES) for f in rp.FEATURES}
     workloads = {"a_credit_limit_x100": ["credit_limit"], "b_all_23_fields": list(rp.FEATURES)}
     res = {"device": bench.device_record(0), "rows": N, "models": {}}
+    if PACKED:
+        res["row_format"] = "packed64"
+    fmt = ROWS_PACKED64 if PACKED else ROWS_WORDS24
     for name, pipe in models.items():
         flat = flatten_pipeline(pipe)
         enc = RowEncoder(flat)
         eng = ForestEngine(flat, 0)
-        rows = enc.encode_arrays(codes, nums)
+        words24 = enc.encode_arrays(codes, nums)
+        rows = enc.pack_rows(words24) if PACKED else words24
         d_rows = eng.device_alloc(rows.nbytes)
         eng.h2d(d_rows, rows)
         per = {}
@@ -76,7 +83,7 @@ def main():
             d_out = eng.device_alloc(N * off * 8)
 
             def kernel():
-                eng.partial_dependence_device(d_rows, N, probes, grid, d_out)
+                eng.partial_dependence_device(d_rows, N, probes, grid, d_out, fmt)
                 eng.sync()
 
             k_ms = median_ms(kernel)
@@ -86,7 +93,7 @@ def main():
 
             def expanded():
                 for (word, _, g), w in zip(probes, words):
-                    big = np.repeat(rows, g, axis=0)
+                    big = np.repeat(words24, g, axis=0)
                     big[:, word] = np.tile(w, N)
                     eng.predict_rows(big, np.float64)
 
@@ -105,7 +112,7 @@ def main():
         eng.close()
         res["models"][name] = per
     os.makedirs(OUT, exist_ok=True)
-    with open(os.path.join(OUT, "dependence_time.json"), "w") as f:
+    with open(os.path.join(OUT, "dependence_time_packed.json" if PACKED else "dependence_time.json"), "w") as f:
         json.dump(res, f, indent=1)
     print(json.dumps(res["device"]))
 
