@@ -475,8 +475,11 @@ static RankKernel<OutT> rank_kernel(const b2f_model *m) {
     }
 }
 /* The dynamic shared-memory limit belongs to the kernel function on the current device, not to a model: every model of the
- * process that launches `kernel` shares it.  So it only ever rises -- a later model with a smaller forest (an attached
- * outlier forest, a second engine) must not lower it under an earlier model's launches, which would then fail. */
+ * process that launches `kernel` shares it.  So it only ever rises -- a later model with a smaller need (an attached
+ * outlier forest, a second engine, an explainer of fewer fields, a shallower forest's permutation scores, a smaller k)
+ * must not lower it under an earlier model's launches, which would then fail.  Every kernel with dynamic shared memory
+ * sets its limit here, at attach or per call, and never through cudaFuncSetAttribute directly
+ * (tests/test_models_together_cpu.py). */
 template <typename K>
 static cudaError_t set_smem_limit(K kernel, int bytes) {
     if (!kernel) return cudaErrorInvalidValue;
@@ -904,7 +907,7 @@ static int tile_init(b2f_model *m, const uint8_t *blob, const EnvHooks &env) {
 static int streams_init(b2f_model *m) {
     for (int s = 0; s < B2F_STREAMS; ++s) CUDA_TRY(cudaStreamCreateWithFlags(&m->slots[s].stream, cudaStreamNonBlocking));
     CUDA_TRY(cudaStreamCreateWithFlags(&m->compute, cudaStreamNonBlocking));
-    CUDA_TRY(cudaFuncSetAttribute(k_feature_moments, cudaFuncAttributeMaxDynamicSharedMemorySize, B2F_MOM_SMEM));
+    CUDA_TRY(set_smem_limit(k_feature_moments, B2F_MOM_SMEM));
     m->mom_blocks = m->sm_count * 3; /* one full wave: 3 CTAs (3-stage 72 KB ring each) per SM */
     CUDA_TRY(cudaMalloc(&m->d_mom_partials, (size_t)m->mom_blocks * B2F_MOM_PARTIAL_VALUES * sizeof(double)));
     CUDA_TRY(cudaMalloc(&m->d_mom_ticket, sizeof(unsigned int)));

@@ -100,7 +100,7 @@ static int drift_init(b2f_drift *d, const double *ref_sorted, const int32_t *cat
     if (const char *rs = getenv("B2F_DRIFT_ROWSCAN_SMEM")) d->rowscan_smem_max_n = std::max(0, std::min(B2F_DRIFT_ROWSCAN_SMEM_LIMIT, atoi(rs)));
     d->finish_smem = 2 * B2F_DRIFT_RING_MAX * sizeof(double);
     if (d->rowscan_smem_max_n > 0) d->finish_smem = std::max(d->finish_smem, (size_t)B2F_DRIFT_ROWSCAN_CAP * sizeof(double));
-    CUDA_TRY(cudaFuncSetAttribute(k_drift_finish, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(d->finish_smem, (size_t)B2F_DRIFT_ROWSCAN_CAP * sizeof(double))));
+    CUDA_TRY(set_smem_limit(k_drift_finish, (int)std::max<size_t>(d->finish_smem, (size_t)B2F_DRIFT_ROWSCAN_CAP * sizeof(double))));
     return B2F_OK;
 }
 

@@ -286,7 +286,7 @@ extern "C" int b2f_model_attach_explainer(b2f_model *m, const void *paths, size_
         const int F = sp.n_cat + sp.n_num;
         k.smem_bytes = v == SHAP_INTERACTIONS ? inter_smem_bytes(F) : (v == SHAP_INTERVENTIONAL ? interv_smem_bytes(F) : shap_smem_bytes(F));
         for (bool pk : {false, true})
-            if (e == cudaSuccess) e = cudaFuncSetAttribute(explain_kernel(v, ex->maxl, pk), cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem_bytes);
+            if (e == cudaSuccess) e = set_smem_limit(explain_kernel(v, ex->maxl, pk), k.smem_bytes);
         if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k.ctas_per_sm, explain_kernel(v, ex->maxl, false), B2F_SHAP_THREADS, k.smem_bytes);
         k.ctas_per_sm = std::max(1, k.ctas_per_sm);
     }

@@ -75,8 +75,8 @@ extern "C" int b2f_permutation_scores(b2f_model *m, const void *rows, int64_t n,
     CUDA_TRY(pi_segmented_sort(nullptr, &temp_bytes, k0, k1, f0, f1, (int)(gp * n), (int)gp, d_off, st, nullptr));
     if ((rc = compute_reserve(m, pi.temp, std::max<size_t>(temp_bytes, 1), who, "the sort's temporary storage"))) return rc;
     const size_t smem = pi_smem_bytes((int)h.max_depth);
-    CUDA_TRY(cudaFuncSetAttribute(k_permutation_scores<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CUDA_TRY(cudaFuncSetAttribute(k_permutation_scores<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CUDA_TRY(set_smem_limit(k_permutation_scores<true>, (int)smem));
+    CUDA_TRY(set_smem_limit(k_permutation_scores<false>, (int)smem));
 
     TimedRegion timed{m, device_ms};
     if ((rc = timed.start())) return rc;

@@ -84,7 +84,7 @@ extern "C" int b2f_knn(b2f_model *m, const void *rows, int64_t n, int row_format
 
     CUDA_TRY(cudaSetDevice(m->device));
     const int smem = (int)knn_smem_bytes(kn.ref.mp.n_cat, kn.ref.mp.n_num, k);
-    CUDA_TRY(cudaFuncSetAttribute(k_knn_chunk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CUDA_TRY(set_smem_limit(k_knn_chunk, smem));
     const cudaStream_t st = m->compute;
     /* the piece size: at most B2F_KNN_PIECE_ROWS queries, halved until the candidate scratch fits the budget */
     int64_t piece = std::min<int64_t>(n, B2F_KNN_PIECE_ROWS);

@@ -65,9 +65,9 @@ static MmdPool ref_pool(const EmbeddedRef &ref, int64_t n_ref) {
 /* the pair kernels' dynamic shared memory (up to 47 KB, beside the select's static histogram) */
 static int mmd_smem_attr(const Mmd &md) {
     const int smem = (int)mmd_smem_bytes(md.ref.mp.n_cat, md.ref.mp.n_num);
-    CUDA_TRY(cudaFuncSetAttribute(k_mmd_select_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CUDA_TRY(cudaFuncSetAttribute(k_mmd_row_sums, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CUDA_TRY(cudaFuncSetAttribute(k_mmd_subset_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CUDA_TRY(set_smem_limit(k_mmd_select_hist, smem));
+    CUDA_TRY(set_smem_limit(k_mmd_row_sums, smem));
+    CUDA_TRY(set_smem_limit(k_mmd_subset_pairs, smem));
     return B2F_OK;
 }
 
