@@ -34,6 +34,7 @@ SCORED_FULL_DTYPE = np.dtype(  # b2f_scored_full, 24 bytes
 MOMENT_VALUES = ROW_WORDS * 3
 PD_PROBE_DTYPE = np.dtype([("word", np.int32), ("grid_offset", np.int32), ("count", np.int32)])  # b2f_pd_probe
 PAIR_PROBE_DTYPE = np.dtype([("word_a", np.int32), ("word_b", np.int32), ("point_offset", np.int32), ("count", np.int32)])  # b2f_pair_probe
+ALE_PROBE_DTYPE = np.dtype([("word", np.int32), ("edge_offset", np.int32), ("bins", np.int32)])  # b2f_ale_probe
 COUNTERFACTUAL_DTYPE = np.dtype(  # struct b2f_counterfactual, 32 bytes
     [("lower_p1", np.float64), ("upper_p1", np.float64), ("lower", np.float32), ("upper", np.float32), ("value", np.float32), ("reserved", np.int32)]
 )
@@ -193,6 +194,11 @@ SIGNATURES = {
         C.c_int,
         [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p],
     ),
+    "b2f_ale": (
+        C.c_int,
+        [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)],
+    ),
+    "b2f_ale_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b2f_counterfactual": (
         C.c_int,
         [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)],

@@ -38,6 +38,7 @@
 #include "counterfactual.cuh"
 #include "permutation_importance.cuh"
 #include "pair_dependence.cuh"
+#include "ale.cuh"
 #include "mmd_drift.cuh"
 #include "knn.cuh"
 #include "tree_shap.cuh"
@@ -182,6 +183,15 @@ struct PairDependence {
     DevBuf rows, partial, out;
 };
 
+/* accumulated local effects (b2f_ale; ale.cuh): the current call's spec (AleSeg table, then the edges) and bins; the
+ * rows of the host form, the per-CTA partials of a piece and the per-bin results, on the compute stream, grown on demand */
+struct Ale {
+    int n_segs = 0;
+    int bins = 0;
+    std::vector<uint32_t> spec;
+    DevBuf spec_dev, rows, psum, pcnt, sums, counts;
+};
+
 /* nearest single-field counterfactuals (b2f_counterfactual; counterfactual.cuh).  The split-value table is built on the
  * first call; cp.pd is the model's walk parameters, set at model creation, the probe fields are the current call's. */
 struct Counterfactual {
@@ -274,9 +284,10 @@ struct b2f_model {
     void *d_blob = nullptr;
     int64_t forest_bytes = 0;
     Explainer *ex = nullptr; /* attached TreeSHAP path table (b2f_model_attach_explainer) */
-    PdParams walk; /* the forest fields every mask-walk kernel reads (K6, K7, K8, K10); segs, grid and points are a call's */
+    PdParams walk; /* the forest fields every mask-walk kernel reads (K6, K7, K8, K10, K12); segs, grid and points are a call's */
     Dependence pd;
     PairDependence pair;
+    Ale ale;
     Counterfactual cf;
     Importance pi;
     Mmd mmd;
@@ -972,6 +983,7 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
     }
     for (DevBuf *b : {&m->scratch, &m->pd.host_spec, &m->pd.device_spec, &m->cf.dev, &m->mom_rows, &m->gather, &m->flush}) b->release();
     for (DevBuf *b : {&m->pair.host_spec, &m->pair.spec_dev, &m->pair.rows, &m->pair.partial, &m->pair.out}) b->release();
+    for (DevBuf *b : {&m->ale.spec_dev, &m->ale.rows, &m->ale.psum, &m->ale.pcnt, &m->ale.sums, &m->ale.counts}) b->release();
     for (DevBuf *b : {&m->pi.rows, &m->pi.labels, &m->pi.perm, &m->pi.keys, &m->pi.flags, &m->pi.temp, &m->pi.offsets, &m->pi.segs, &m->pi.scores}) b->release();
     for (EmbeddedRef *e : {&m->mmd.ref, &m->knn.ref})
         for (DevBuf *b : {&e->ref_z, &e->ref_c, &e->rows, &e->z, &e->c}) b->release();
@@ -1907,6 +1919,9 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
 
 /* ------------------------------------------------------------------ two-way partial dependence (K10) */
 #include "pair_dependence_api.cuh"
+
+/* ------------------------------------------------------------------ accumulated local effects (K12) */
+#include "ale_api.cuh"
 
 /* ------------------------------------------------------------------ counterfactuals (K7) */
 #include "counterfactual_api.cuh"

@@ -288,6 +288,28 @@ class ForestEngine:
         check(self._lib.b2f_pair_dependence_device(self._h, rows_dev, n, fmt, ptr(pr), len(pr), ptr(words), int(bool(mean)), out_dev),
               "b2f_pair_dependence_device")
 
+    # ------------------------------------------------------------------ accumulated local effects (csrc/ale.cuh)
+    def ale_rows(self, rows: np.ndarray, probes, edges: np.ndarray, device_ms: bool = False):
+        """Encoded rows (N, 24) or packed (N, 16), probes [(numeric row word, edge offset, bins K)] and float32 edges ->
+        (float64 bin sums, int64 bin row counts[, device ms]), each (sum of K,) in probe order: per bin of a probe, the sum
+        over the rows whose value of the word lies in it of f(upper edge) - f(lower edge), and the number of those rows."""
+        rows = np.ascontiguousarray(rows)
+        pr = _ale_probe_table(probes)
+        z = np.ascontiguousarray(edges, dtype=np.float32)
+        K = int(pr["bins"].sum()) if len(pr) else 0
+        sums, counts = np.empty(K, dtype=np.float64), np.empty(K, dtype=np.int64)
+        ms = C.c_float(0.0)
+        check(self._lib.b2f_ale(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(pr), len(pr), ptr(z), ptr(sums), ptr(counts),
+                                C.byref(ms)), "b2f_ale")
+        return (sums, counts, ms.value) if device_ms else (sums, counts)
+
+    def ale_device(self, rows_dev: int, n: int, probes, edges: np.ndarray, sums_dev: int, counts_dev: int, fmt: int = ROWS_WORDS24) -> None:
+        """Enqueue the per-bin sums (doubles) and row counts (int64) of device-resident rows into device buffers; probes and
+        edges are host arrays, as for ``ale_rows``; ``sync`` waits."""
+        pr = _ale_probe_table(probes)
+        z = np.ascontiguousarray(edges, dtype=np.float32)
+        check(self._lib.b2f_ale_device(self._h, rows_dev, n, fmt, ptr(pr), len(pr), ptr(z), sums_dev, counts_dev), "b2f_ale_device")
+
     # ------------------------------------------------------------------ counterfactuals (csrc/counterfactual.cuh)
     def counterfactual_rows(self, rows: np.ndarray, words, cutoff: float = 0.5, device_ms: bool = False):
         """Encoded rows (N, 24) or packed (N, 16) and numeric row words -> (proba float64 (N,), records (N, len(words)) of
@@ -597,6 +619,11 @@ def _probe_table(probes) -> np.ndarray:
 def _pair_probe_table(probes) -> np.ndarray:
     """[(word a, word b or -1, point offset, count)] -> b2f_pair_probe records."""
     return np.array([tuple(int(v) for v in p) for p in probes], dtype=_cabi.PAIR_PROBE_DTYPE)
+
+
+def _ale_probe_table(probes) -> np.ndarray:
+    """[(row word, edge offset, bins)] -> b2f_ale_probe records."""
+    return np.array([tuple(int(v) for v in p) for p in probes], dtype=_cabi.ALE_PROBE_DTYPE)
 
 
 def moments_merge(parts: np.ndarray) -> np.ndarray:

@@ -29,7 +29,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pandas as pd
 
-from . import dependence, importance, interaction, mmd, trust
+from . import ale, dependence, importance, interaction, mmd, trust
 from ._cabi import OUT_F64, OUT_FULL, ROWS_PACKED64, ROWS_WORDS24, B2FError
 from ._pylists import ListBuilder
 from .encode import RowEncoder
@@ -412,6 +412,55 @@ class B200Model:
             means = self.engine.pair_dependence_rows(rows, probes, points, mean=True)
         res = interaction.strength_result(means, maps, features)
         res["rows"] = len(S)
+        return res
+
+    def accumulated_local_effects(self, model_input, features=None, *, bins: int = ale.DEFAULT_BINS, min_bin_points: int = ale.DEFAULT_MIN_BIN_POINTS,
+                                  custom_edges: dict | None = None, grid_frame: pd.DataFrame | None = None) -> dict:
+        """How P(class 1) moves with each numeric request field where the applicants actually are: accumulated local
+        effects (Apley & Zhu), which score each row only at the two edges of the bin its own value lies in, so correlated
+        fields are never pushed to combinations no applicant has (partial dependence's weakness).  The formulas and the
+        default edge rule are in ``ale.py``; f = P(class 1) as ``partial_dependence`` scores it, each substituted row bit
+        for bit the tile kernel's score.
+
+        ``features``: numeric fields (default: every numeric field, in field order).  Edges: ``custom_edges[f]`` (2..257
+        finite numbers, strictly increasing as float32; rows outside [z_0, z_K] go to the end bins), else the edge rule over
+        the present values of ``grid_frame[f]``, or of ``model_input[f]`` without one.  A row whose field is missing takes
+        no part in that field.  -> ``{"feature_names", "output": "probability", "feature_values": [edges (K + 1)],
+        "ale_values": [(K + 1)], "bin_effects": [d_k (K)], "bin_rows": [n_k (K)], "ale0": [float], "constant_value": mean
+        P(class 1) over the rows, "rows"}``; a field with one distinct value has one edge and ``ale_values == [0.0]``.
+        ValueError for an unknown, categorical or repeated field, bins outside 1..256, min_bin_points < 1, bad custom edges,
+        zero rows, or a field with no present value to build edges from.  Every model has it.  It runs on the first GPU's
+        handle only, under ``replicas[0].lock``."""
+        df = self._frame(model_input)
+        features = ale.check_features(features, self.numeric_features, self.categorical_features)
+        bins, min_bin_points = ale.check_params(bins, min_bin_points)
+        custom_edges = dict(custom_edges or {})
+        extra = [f for f in custom_edges if f not in features]
+        if extra:
+            raise ValueError(f"custom_edges for feature(s) {extra} that are not probed")
+        if len(df) == 0:
+            raise ValueError("accumulated local effects need at least one row")
+        source = df if grid_frame is None else grid_frame
+        edges = []
+        for f in features:
+            if f in custom_edges:
+                edges.append(ale.check_custom_edges(f, custom_edges[f]))
+            else:
+                try:
+                    edges.append(ale.default_edges(ale.present_float32(self.encoder, f, source[f]), bins, min_bin_points))
+                except ValueError as e:
+                    raise ValueError(f"feature {f!r}: {e}") from None
+        probes, flat_edges, which = ale.probe_plan([dependence.word_of(self.encoder, f) for f in features], edges)
+        rows = self.encoder.encode_frame(df)
+        with self.replicas[0].lock:
+            if probes:
+                sums, counts = self.engine.ale_rows(rows, probes, flat_edges)
+            else:
+                sums, counts = np.zeros(0), np.zeros(0, np.int64)
+            proba, _ = self.engine.predict_rows(rows, np.float64)
+        res = ale.result(features, edges, sums, counts, probes, which)
+        res["constant_value"] = float(np.mean(proba))
+        res["rows"] = len(df)
         return res
 
     def counterfactuals(self, model_input, features=None, *, cutoff: float = 0.5) -> dict:

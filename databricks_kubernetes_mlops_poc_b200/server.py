@@ -43,9 +43,9 @@ from fastapi import FastAPI, Request, Response
 from fastapi.exceptions import RequestValidationError
 from pydantic import ValidationError
 
-from . import dependence, importance, interaction, mmd, trust
+from . import ale, dependence, importance, interaction, mmd, trust
 from .ingest import NativeRequestParser, parse_rows, rows_to_frame  # noqa: F401  (rows_to_frame re-exported)
-from .schema import ALL_FEATURES, LABELLED_ROWS, TARGET, LabelledApplicant, LoanApplicant, ModelOutput
+from .schema import ALL_FEATURES, CATEGORICAL_FEATURES, LABELLED_ROWS, NUMERIC_FEATURES, TARGET, LabelledApplicant, LoanApplicant, ModelOutput
 
 ml_models: dict = {}
 
@@ -366,6 +366,37 @@ def _dependence_problem(features, values, kind, grid_resolution) -> str | None:
     return None
 
 
+_ALE_PARAMETERS = [
+    {"name": "feature", "in": "query", "required": False,
+     "description": "numeric request field; repeat for several, each at most once; none = every numeric field",
+     "schema": {"type": "array", "items": {"type": "string", "enum": list(NUMERIC_FEATURES)}}, "style": "form", "explode": True},
+    {"name": "bins", "in": "query", "required": False, "description": "most bins per field of the default (quantile) edges",
+     "schema": {"type": "integer", "minimum": 1, "maximum": ale.MAX_BINS, "default": ale.DEFAULT_BINS}},
+    {"name": "min_bin_points", "in": "query", "required": False, "description": "fewest request rows per bin of the default edges",
+     "schema": {"type": "integer", "minimum": 1, "default": ale.DEFAULT_MIN_BIN_POINTS}},
+    {"name": "value", "in": "query", "required": False,
+     "description": "explicit bin edge of the one probed field; repeat for 2..257 strictly increasing numbers",
+     "schema": {"type": "array", "items": {"type": "number"}}, "style": "form", "explode": True},
+]
+
+
+def _ale_problem(features, values, bins: str, min_bin_points: str) -> str | None:
+    """Why a /explain/ale query is unprocessable, or None (edges the rows cannot give are the model's ValueError)."""
+    try:
+        ale.check_features(features or None, NUMERIC_FEATURES, CATEGORICAL_FEATURES)
+        ale.check_params(int(bins), int(min_bin_points))
+    except ValueError as e:
+        return str(e) if "invalid literal" not in str(e) else "bins and min_bin_points must be integers"
+    if values:
+        if len(features) != 1:
+            return "explicit values need exactly one feature"
+        try:
+            ale.check_custom_edges(features[0], values)
+        except ValueError as e:
+            return str(e)
+    return None
+
+
 _MMD_PARAMETERS = [
     {"name": "n_permutations", "in": "query", "required": False,
      "schema": {"type": "integer", "minimum": 1, "maximum": mmd.MAX_PERMUTATIONS, "default": 100}},
@@ -612,6 +643,43 @@ def create_app(model=None, loader=None) -> FastAPI:
             return {"feature_names": list(out["feature_names"]), "rows": int(out["rows"]), "pairs": [list(p) for p in out["pairs"]],
                     "h_squared": _nullable(out["h_squared"]), "numerator": _nullable(out["numerator"]),
                     "denominator": _nullable(out["denominator"]), "matrix": [_nullable(r) for r in out["matrix"]]}
+
+        return await answered(request, call)
+
+    @app.post("/explain/ale", openapi_extra={"requestBody": _REQUEST_SCHEMA, "parameters": _ALE_PARAMETERS})
+    async def explain_ale(request: Request):
+        """How the default probability moves with each numeric field where the applicants actually are: accumulated local
+        effects.  Each applicant is scored only at the two edges of the bin its own value lies in; a bin's effect is the
+        mean change over its applicants, and `ale_values` (one per edge in `feature_values`) are the effects summed along
+        the field and centred on the applicants (`ale0` is what was taken off).  Unlike /explain/dependence, no applicant is
+        moved to values far from its own, so correlated fields (the six bill amounts) are not scored at combinations no one
+        has.  The edges are the repeated `value` parameters (one field only), else quantiles of the request rows with at
+        least `min_bin_points` rows per bin, at most `bins` bins (every distinct value when there are few).  An applicant
+        missing the field takes no part in it.  `bin_effects` and `bin_rows` give each bin's effect and size;
+        `constant_value` is the mean probability.  422 for an unknown, categorical or repeated field, a bad bins or
+        min_bin_points, bad values, or a field no request row has a value for."""
+        q = request.query_params
+        features, values = q.getlist("feature"), q.getlist("value")
+        bins, min_bin_points = q.get("bins", str(ale.DEFAULT_BINS)), q.get("min_bin_points", str(ale.DEFAULT_MIN_BIN_POINTS))
+        problem = _ale_problem(features, values, bins, min_bin_points)
+        if problem:
+            return _unprocessable(problem)
+
+        def call(m, input_df):
+            kw = {"bins": int(bins), "min_bin_points": int(min_bin_points)}
+            if values:
+                kw["custom_edges"] = {features[0]: [float(v) for v in values]}
+            try:
+                out = m.accumulated_local_effects(input_df, features or None, **kw)
+            except ValueError as e:
+                return _unprocessable(str(e))
+            return {"feature_names": list(out["feature_names"]), "output": out["output"], "rows": int(out["rows"]),
+                    "constant_value": float(out["constant_value"]),
+                    "feature_values": [np.asarray(v, dtype=np.float64).tolist() for v in out["feature_values"]],
+                    "ale_values": [np.asarray(v, dtype=np.float64).tolist() for v in out["ale_values"]],
+                    "bin_effects": [np.asarray(v, dtype=np.float64).tolist() for v in out["bin_effects"]],
+                    "bin_rows": [np.asarray(v, dtype=np.int64).tolist() for v in out["bin_rows"]],
+                    "ale0": [float(v) for v in out["ale0"]]}
 
         return await answered(request, call)
 

@@ -417,6 +417,38 @@ int b2f_pair_dependence(b2f_model *m, const void *rows, int64_t n, int row_forma
 int b2f_pair_dependence_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const b2f_pair_probe *probes, int n_probes,
                                const uint32_t *point_words, int mean, double *out_dev);
 
+/* ---- accumulated local effects (csrc/ale.cuh) ----
+ * The device half of ALE (Apley & Zhu): for each probe (a numeric row word with float32 edges z_0 < ... < z_K,
+ * edges[edge_offset .. edge_offset + K]) and each row i whose value x of that word is present (not NaN as given, before
+ * imputation), the row's bin k = clamp(#{j : z_j < x}, 1, K) and its delta f(x_i with the word = z_k) - f(x_i with the word
+ * = z_{k-1}), f = b2f_predict_f64's proba1 (each score bit for bit the tile kernel's score of the substituted row; the row's
+ * other missing numerics imputed).  A row whose word is missing takes no part in that probe.  Out, per probe in probe order
+ * and per bin k = 1..K (index boff + k - 1, boff = the bins of the earlier probes): bin_sums, the sum of the bin's deltas,
+ * and bin_rows, the bin's row count.
+ * Summation order (no atomics): rows are taken in CTAs of 128 consecutive rows; a CTA's partial of a bin is its rows'
+ * deltas in row order added to 0.0; a bin's result is its CTA partials in CTA order added to 0.0.  So results are
+ * bit-identical from run to run and across row formats, and a probe's results do not depend on the other probes of the
+ * call.  One walk per (row, tree) carries the two points of up to 16 probes.  The host form copies the rows to the device
+ * once, on the compute stream, into a buffer the model keeps; the per-CTA partials stay under B2F_PERM_SCRATCH_BYTES (the
+ * rows are taken in pieces of whole CTAs).  Errors: B2F_EINVAL for ranked rows, n < 1, a NULL pointer, n_probes outside
+ * 1..n_num, a word that is not numeric or is probed twice, bins outside 1..B2F_ALE_MAX_BINS, an edge range past
+ * B2F_ALE_MAX_EDGES, edges that are not strictly increasing, or a forest deeper than 32 levels; B2F_ERANGE for a
+ * non-finite edge; B2F_ENOMEM (with the byte count) when a device buffer cannot be allocated.  device_ms (may be NULL): from
+ * the first upload to the last copy back, CUDA events on the compute stream. */
+#define B2F_ALE_MAX_BINS 256
+#define B2F_ALE_MAX_EDGES (23 * (B2F_ALE_MAX_BINS + 1))
+typedef struct b2f_ale_probe {
+    int32_t word;        /* numeric row word: n_cat .. n_cat + n_num - 1 */
+    int32_t edge_offset; /* first edge in edges */
+    int32_t bins;        /* K: 1 .. B2F_ALE_MAX_BINS (K + 1 edges) */
+} b2f_ale_probe;
+int b2f_ale(b2f_model *m, const void *rows, int64_t n, int row_format, const b2f_ale_probe *probes, int n_probes, const float *edges,
+            double *bin_sums, int64_t *bin_rows, float *device_ms);
+/* device-resident form: rows_dev, bin_sums_dev and bin_rows_dev in device memory, probes and edges in host memory;
+ * enqueued on the compute stream (asynchronous, like b2f_partial_dependence_device; b2f_sync waits) */
+int b2f_ale_device(b2f_model *m, const void *rows_dev, int64_t n, int row_format, const b2f_ale_probe *probes, int n_probes,
+                   const float *edges, double *bin_sums_dev, int64_t *bin_rows_dev);
+
 /* ---- nearest single-field counterfactuals (csrc/counterfactual.cuh) ----
  * "What is the smallest change to this one field that changes the decision?"  For row i and probed numeric row word w with
  * the forest's split values t'_0 < ... < t'_{m-1} (b2f_blob_split_values), every float32 value of a piece [t'_{k-1}, t'_k)
