@@ -220,6 +220,16 @@ SIGNATURES = {
         C.c_int,
         [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_double), C.c_void_p, C.POINTER(C.c_float)],
     ),
+    "b2f_mmd_online_bootstrap": (
+        C.c_int,
+        [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)],
+    ),
+    "b2f_mmd_online_configure": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_float)]),
+    "b2f_mmd_online_push": (
+        C.c_int,
+        [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_float)],
+    ),
+    "b2f_mmd_online_reset": (C.c_int, [C.c_void_p]),
     "b2f_model_attach_knn_reference": (
         C.c_int,
         [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p],

@@ -40,6 +40,7 @@
 #include "pair_dependence.cuh"
 #include "ale.cuh"
 #include "mmd_drift.cuh"
+#include "mmd_online.cuh"
 #include "knn.cuh"
 #include "tree_shap.cuh"
 #include "tree_shap_interactions.cuh"
@@ -222,6 +223,21 @@ struct EmbeddedRef {
     DevBuf rows, z, c;   /* a call's rows and their embedding */
 };
 
+/* the online MMD detector (b2f_mmd_online_*; mmd_online.cuh): its configuration, the window state carried between pushes
+ * (the stream's last W - 1 rows: embedding and c) and its copy at configure for reset, and a call's buffers; all on the
+ * compute stream, grown on demand */
+struct MmdOnline {
+    int window = 0; /* 0: not configured */
+    int64_t rw = 0, t = 0;
+    double k_rr = 0.0;
+    DevBuf total;                          /* T = sum of r_ref */
+    DevBuf rz, rc;                         /* the sub-reference's embedding, compacted */
+    DevBuf carry_z, carry_c, carry_cv;     /* the window state */
+    DevBuf init_z, init_c, init_cv;        /* the window state at configure */
+    DevBuf pos, band, qsum, cv, stats, krr; /* a bootstrap slice's or a push piece's scratch */
+    DevBuf seq_z, seq_c, out;              /* a piece's sequence: the carried rows, then its own */
+};
+
 /* the MMD drift test (b2f_model_attach_mmd_reference / b2f_mmd_drift; mmd_drift.cuh): the reference and its kernel row
  * sums, kept between calls, and a call's buffers; all on the compute stream, grown on demand */
 struct Mmd {
@@ -229,6 +245,7 @@ struct Mmd {
     double sigma = 0.0, coef = 0.0;
     DevBuf r_ref; /* sum_{j != i} k(i, j) over the reference */
     DevBuf r, partial, sub, pairs, out, hist;
+    MmdOnline online; /* configured against this reference: attaching another drops it */
 };
 
 /* the k-nearest reference search of trust scores (b2f_model_attach_knn_reference / b2f_knn; knn.cuh): the class-sorted
@@ -988,6 +1005,12 @@ extern "C" void b2f_model_destroy(b2f_model *m) {
     for (EmbeddedRef *e : {&m->mmd.ref, &m->knn.ref})
         for (DevBuf *b : {&e->ref_z, &e->ref_c, &e->rows, &e->z, &e->c}) b->release();
     for (DevBuf *b : {&m->mmd.r_ref, &m->mmd.r, &m->mmd.partial, &m->mmd.sub, &m->mmd.pairs, &m->mmd.out, &m->mmd.hist}) b->release();
+    {
+        MmdOnline &o = m->mmd.online;
+        for (DevBuf *b : {&o.total, &o.rz, &o.rc, &o.carry_z, &o.carry_c, &o.carry_cv, &o.init_z, &o.init_c, &o.init_cv, &o.pos, &o.band,
+                          &o.qsum, &o.cv, &o.stats, &o.krr, &o.seq_z, &o.seq_c, &o.out})
+            b->release();
+    }
     for (DevBuf *b : {&m->knn.orig, &m->knn.cand_d, &m->knn.cand_i, &m->knn.dist, &m->knn.index}) b->release();
     for (auto &t : m->tickets)
         for (auto &e : t.ev)
@@ -1931,6 +1954,9 @@ extern "C" int b2f_moments_multi(b2f_model **models, int n_models, const void *r
 
 /* ------------------------------------------------------------------ MMD drift test (K9) */
 #include "mmd_api.cuh"
+
+/* ------------------------------------------------------------------ online MMD drift detector (K13) */
+#include "mmd_online_api.cuh"
 
 /* ------------------------------------------------------------------ k-nearest reference rows of trust scores (K11) */
 #include "knn_api.cuh"

@@ -121,6 +121,7 @@ extern "C" int b2f_model_attach_mmd_reference(b2f_model *m, const void *rows, in
     if (device_ms) *device_ms = 0.0f;
     Mmd &md = m->mmd;
     md.ref.n_ref = 0; /* replaced: no reference until this one is complete */
+    md.online.window = 0; /* the online detector was configured against the old one */
     int rc = ref_check_rows(m, rows, n, row_format, 2, B2F_MMD_MAX_REF, "MMD drift takes", "MMD reference");
     if (rc == B2F_OK) rc = ref_constants(m, md.ref, num_mean, num_scale, "MMD reference");
     if (rc) return rc;

@@ -383,6 +383,42 @@ class ForestEngine:
                                       C.byref(ms)), "b2f_mmd_drift")
         return (obs.value, perm, ms.value) if device_ms else (obs.value, perm)
 
+    # ------------------------------------------------------------------ online MMD drift detector (csrc/mmd_online.cuh)
+    def mmd_online_bootstrap(self, etw: np.ndarray, window: int, device_ms: bool = False):
+        """(n_boot, 2W - 1) reference positions -> (float64 (n_boot, W) window statistics, float64 (n_boot,) K_RR[, device
+        ms]) against the attached MMD reference (``mmd_online.py`` draws the positions)."""
+        p = np.ascontiguousarray(etw, dtype=np.int32)
+        if p.ndim != 2 or p.shape[1] != 2 * int(window) - 1:
+            raise ValueError(f"etw must be (n_boot, {2 * int(window) - 1}), not {p.shape}")
+        stats = np.empty((p.shape[0], int(window)), dtype=np.float64)
+        k_rr = np.empty(p.shape[0], dtype=np.float64)
+        ms = C.c_float(0.0)
+        check(self._lib.b2f_mmd_online_bootstrap(self._h, ptr(p), p.shape[0], int(window), ptr(stats), ptr(k_rr), C.byref(ms)),
+              "b2f_mmd_online_bootstrap")
+        return (stats, k_rr, ms.value) if device_ms else (stats, k_rr)
+
+    def mmd_online_configure(self, perm: np.ndarray, window: int, device_ms: bool = False):
+        """A permutation of the reference's rows: sub-reference perm[:rw], initial window perm[-W:]; t = 0[, -> device ms]."""
+        p = np.ascontiguousarray(perm, dtype=np.int32)
+        if p.shape != (self.mmd_reference_rows,):
+            raise ValueError(f"perm must be ({self.mmd_reference_rows},), not {p.shape}")
+        ms = C.c_float(0.0)
+        check(self._lib.b2f_mmd_online_configure(self._h, ptr(p), int(window), C.byref(ms)), "b2f_mmd_online_configure")
+        return ms.value if device_ms else None
+
+    def mmd_online_push(self, rows: np.ndarray, device_ms: bool = False):
+        """Encoded rows (M, 24) or packed (M, 16), pushed in row order -> (float64 (M,) window statistics, time of row 0[,
+        device ms])."""
+        rows = np.ascontiguousarray(rows)
+        stat = np.empty(rows.shape[0], dtype=np.float64)
+        t0, ms = C.c_int64(0), C.c_float(0.0)
+        check(self._lib.b2f_mmd_online_push(self._h, ptr(rows), rows.shape[0], self._fmt(rows), ptr(stat), C.byref(t0), C.byref(ms)),
+              "b2f_mmd_online_push")
+        return (stat, t0.value, ms.value) if device_ms else (stat, t0.value)
+
+    def mmd_online_reset(self) -> None:
+        check(self._lib.b2f_mmd_online_reset(self._h), "b2f_mmd_online_reset")
+
     # ------------------------------------------------------------------ k-nearest reference rows of trust scores (csrc/knn.cuh)
     def attach_knn_reference(self, rows: np.ndarray, classes, num_mean, num_scale) -> None:
         """Encoded reference rows (N, 24) or packed (N, 16), 2 <= N <= 131 072, their classes (0 / 1, each present) and the

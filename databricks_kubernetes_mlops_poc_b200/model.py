@@ -20,6 +20,7 @@ when a reference table is supplied; without one every score is 0.0.
 from __future__ import annotations
 
 import contextlib
+import json
 import math
 import os
 import threading
@@ -29,7 +30,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pandas as pd
 
-from . import ale, dependence, importance, interaction, mmd, trust
+from . import ale, dependence, importance, interaction, mmd, mmd_online, trust
 from ._cabi import OUT_F64, OUT_FULL, ROWS_PACKED64, ROWS_WORDS24, B2FError
 from ._pylists import ListBuilder
 from .encode import RowEncoder
@@ -42,6 +43,7 @@ DRIFT_FILE = "drift_reference.npz"
 EXPLAIN_FILE = "explain.b2f"  # TreeSHAP path table (flatten_explainer); optional
 BACKGROUND_FILE = "explain_background.npz"  # background rows of interventional explanations (raw columns); optional
 MMD_FILE = "mmd_reference.npz"  # reference rows of the MMD drift test (raw columns, and its sigma); optional
+ONLINE_DRIFT_FILE = "online_drift.json"  # configure_online_drift keywords, configured at load after the MMD reference; optional
 TRUST_FILE = "trust_reference.npz"  # labelled reference rows of trust scores (raw columns, labels, fit options); optional
 TRUST_TARGET = "default_payment_next_month"  # the label column a trust reference frame carries by default
 OUTLIER_PICKLE = os.path.join("artifacts", "outlier.pkl")  # joblib.dump(outlier, ".../outlier.pkl"), 02-register-model.ipynb:264,326-328
@@ -52,7 +54,7 @@ class B200Model:
     def __init__(self, flat: FlatForest, devices=None, drift=None, outlier_blob: bytes | None = None, host_threads: int = 0,
                  explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None,
                  mmd_reference: pd.DataFrame | None = None, mmd_sigma: float | None = None,
-                 trust_reference: pd.DataFrame | None = None, trust_options: dict | None = None):
+                 trust_reference: pd.DataFrame | None = None, trust_options: dict | None = None, online_drift: dict | None = None):
         self.flat = flat
         self.all_features = flat.all_features
         self.categorical_features = list(flat.cat_features)
@@ -88,8 +90,12 @@ class B200Model:
             self.attach_background(explain_background)
         self.mmd_reference_rows = 0
         self.mmd_sigma = None  # the attached MMD reference's kernel width
+        self._online = None  # the online detector's configuration (configure_online_drift), its thresholds and keywords
+        self._online_time = 0  # rows pushed since configure or reset
         if mmd_reference is not None:
             self.attach_mmd_reference(mmd_reference, sigma=mmd_sigma)
+        if online_drift is not None:
+            self.configure_online_drift(**online_drift)
         self.trust_reference_rows = None  # rows kept per class of the attached trust reference
         self._trust_positions = None  # attached reference row -> its position in the fitted frame
         if trust_reference is not None:
@@ -105,7 +111,8 @@ class B200Model:
         ``IsolationForest`` plus ``outlier_threshold=``), flattened into a second forest over the same rows.
         ``explain``: also build the TreeSHAP path table, so that ``explain()`` works.  ``background``: a frame of raw rows
         (e.g. the training table) to attach for ``explain_interventional()``; it needs ``explain``.  ``mmd_reference=frame``
-        (and ``mmd_sigma=``): the reference table of ``mmd_drift()``.  ``trust_reference=frame`` (and ``trust_options=``, the
+        (and ``mmd_sigma=``): the reference table of ``mmd_drift()``; ``online_drift=dict(ert=..., window_size=..., ...)``: the
+        keywords of ``configure_online_drift``, which needs it.  ``trust_reference=frame`` (and ``trust_options=``, the
         keywords of ``attach_trust_reference``): the labelled reference of ``trust_score()``."""
         if background is not None and not explain:
             raise ValueError("a background is for interventional explanations: pass explain=True with it")
@@ -584,6 +591,7 @@ class B200Model:
         rows = self.encoder.encode_frame(frame)
         mean, scale = self._embedding_constants(rows)
         self.mmd_reference_rows, self.mmd_sigma = 0, None
+        self._online = None  # the device drops its online detector with the old reference
         with self.replicas[0].lock:
             try:
                 got = self.engine.attach_mmd_reference(rows, mean, scale, sigma)
@@ -613,6 +621,72 @@ class B200Model:
         with self.replicas[0].lock:
             obs, perm = self.engine.mmd_statistics(rows, subsets)
         return mmd.result(obs, perm, p_val, self.mmd_sigma, n_ref, len(df))
+
+    @property
+    def online_drift_configured(self) -> bool:
+        return self._online is not None
+
+    def configure_online_drift(self, *, ert: float, window_size: int, n_bootstraps: int = 1000, random_state: int = 0) -> dict:
+        """Configure the online drift detector, alibi-detect's ``MMDDriftOnline(x_ref, ert, window_size,
+        n_bootstraps=n_bootstraps)`` on the attached MMD reference (``mmd_online.py``): thresholds from ``n_bootstraps``
+        bootstrap streams of the reference, so that with no drift the expected run time between false alarms is about
+        ``ert`` rows, then the split of the reference into a sub-reference and an initial window that is not in detection.
+        Replaces an earlier configuration; t starts at 0.  -> ``{"thresholds": float64 (window_size,),
+        "sub_reference_rows", "split_attempts", "ert", "window_size", "n_bootstraps", "random_state"}``.  It runs on the first
+        GPU's handle only, under ``replicas[0].lock``.  RuntimeError without an MMD reference; ValueError for a bad argument,
+        a window position no bootstrap survives, or no split out of detection in ``mmd_online.SPLIT_ATTEMPTS`` draws."""
+        if not self.mmd_reference_attached:
+            raise RuntimeError("online drift needs an MMD reference: attach_mmd_reference(frame) first")
+        n_ref = self.mmd_reference_rows
+        ert, W, n_boot, random_state = mmd_online.check_config(n_ref, ert, window_size, n_bootstraps, random_state)
+        rng = np.random.default_rng(random_state)
+        etw = mmd_online.draw_bootstraps(rng, n_ref, W, n_boot)
+        self._online = None
+        with self.replicas[0].lock:
+            stats, _ = self.engine.mmd_online_bootstrap(etw, W)
+            thr = mmd_online.thresholds(stats, ert)
+            perm, attempts = mmd_online.split(rng, n_ref, W, thr, lambda y: self.engine.mmd_online_bootstrap(y[None, :], W)[0][0, W - 1])
+            self.engine.mmd_online_configure(perm, W)
+            self._online_time = 0
+        self._online = {"thresholds": thr, "sub_reference_rows": n_ref - (2 * W - 1), "split_attempts": attempts, "ert": ert,
+                        "window_size": W, "n_bootstraps": n_boot, "random_state": random_state}
+        return dict(self._online)
+
+    def _online_required(self) -> dict:
+        if self._online is None:
+            raise RuntimeError("online drift is not configured: configure_online_drift(ert=..., window_size=...), "
+                               f"from_pipeline(..., online_drift=dict(...)) or a model directory that holds {ONLINE_DRIFT_FILE}")
+        return self._online
+
+    def online_drift(self, model_input) -> dict:
+        """Push the request's rows, in row order, into the online detector's window: per row ``time`` (rows since configure
+        or reset, from 1), ``test_stat`` (the window's MMD^2 against the sub-reference), ``threshold`` and ``is_drift``
+        (0/1), then ``first_drift`` (the first time of this call in detection, else None), ``ert`` and ``window_size``.  A
+        detection resets nothing (``reset_online_drift``).  The statistics do not depend on how the stream is cut into
+        calls.  Calls are ordered by ``replicas[0].lock``.  RuntimeError when not configured; ValueError for no rows or a
+        push above ``mmd_online.KERNEL_BUDGET`` kernel values."""
+        cfg = self._online_required()
+        df = self._frame(model_input)
+        W = cfg["window_size"]
+        mmd_online.check_push(len(df), self.mmd_reference_rows, W)
+        rows = self.encoder.encode_frame(df)
+        with self.replicas[0].lock:
+            stat, t_first = self.engine.mmd_online_push(rows)
+            self._online_time = t_first + len(rows) - 1
+        return mmd_online.result(stat, t_first, cfg["thresholds"], cfg["ert"], W)
+
+    def reset_online_drift(self) -> None:
+        """Back to the window of configure: t = 0, the initial window."""
+        self._online_required()
+        with self.replicas[0].lock:
+            self.engine.mmd_online_reset()
+            self._online_time = 0
+
+    def online_drift_state(self) -> dict | None:
+        """The configuration (``configure_online_drift``'s answer) and ``time``, the rows pushed since configure or reset;
+        None when not configured."""
+        cfg = self._online
+        return None if cfg is None else {**cfg, "time": self._online_time}
 
     @property
     def trust_reference_attached(self) -> bool:
@@ -813,13 +887,21 @@ class _Replica:
 def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | None = None, outlier_blob: bytes | None = None,
                    explain_blob: bytes | None = None, explain_background: pd.DataFrame | None = None,
                    mmd_reference: pd.DataFrame | None = None, mmd_sigma: float | None = None,
-                   trust_reference: pd.DataFrame | None = None, trust_options: dict | None = None) -> None:
+                   trust_reference: pd.DataFrame | None = None, trust_options: dict | None = None,
+                   online_drift: dict | None = None) -> None:
     """Write the GPU-side artefact next to (or instead of) the MLflow pickles.  ``explain_blob``: the TreeSHAP path table
     (``flatten_explainer``), written as ``explain.b2f`` so that ``load_model`` attaches it.  ``explain_background``: raw
     rows written as ``explain_background.npz``, attached by ``load_model`` with the explainer.  ``mmd_reference``: raw rows
     written as ``mmd_reference.npz`` with ``mmd_sigma`` (None: the median heuristic at load), attached by ``load_model``.
     ``trust_reference``: raw rows written as ``trust_reference.npz`` with their labels (``trust_options["labels"]``, else the
-    frame's ``default_payment_next_month``) and the other ``attach_trust_reference`` options, fitted by ``load_model``."""
+    frame's ``default_payment_next_month``) and the other ``attach_trust_reference`` options, fitted by ``load_model``.
+    ``online_drift``: the keywords of ``configure_online_drift`` (it needs ``mmd_reference``), written as
+    ``online_drift.json``; ``load_model`` configures the detector from them after the MMD reference.  The window state is
+    not saved: a loaded model starts at t = 0."""
+    if online_drift is not None:
+        if mmd_reference is None:
+            raise ValueError("online_drift needs mmd_reference: the detector runs on the MMD reference")
+        online_drift = _online_keywords(online_drift, len(mmd_reference))
     os.makedirs(path, exist_ok=True)
     flat.save(os.path.join(path, BLOB_FILE))
     if explain_blob is not None:
@@ -830,6 +912,9 @@ def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | 
     if mmd_reference is not None:
         sigma = mmd.check_sigma(mmd_sigma)
         _save_background(os.path.join(path, MMD_FILE), flat, mmd_reference, mmd_sigma=np.float64(np.nan if sigma is None else sigma))
+    if online_drift is not None:
+        with open(os.path.join(path, ONLINE_DRIFT_FILE), "w") as f:
+            json.dump(online_drift, f, indent=1)
     if trust_reference is not None:
         opts = dict(trust_options or {})
         labels = opts.pop("labels", None)
@@ -850,6 +935,15 @@ def save_model_dir(path: str, flat: FlatForest, reference_frame: pd.DataFrame | 
         from .drift import TabularDrift
 
         TabularDrift(reference_frame[flat.all_features], flat.cat_features, device=None).save(os.path.join(path, DRIFT_FILE))
+
+
+def _online_keywords(kw: dict, n_ref: int) -> dict:
+    """The checked keywords of configure_online_drift, as JSON values."""
+    unknown = set(kw) - {"ert", "window_size", "n_bootstraps", "random_state"}
+    if unknown or "ert" not in kw or "window_size" not in kw:
+        raise ValueError(f"online_drift takes ert, window_size, n_bootstraps and random_state, not {sorted(kw)}")
+    ert, W, n_boot, rs = mmd_online.check_config(n_ref, kw["ert"], kw["window_size"], kw.get("n_bootstraps", 1000), kw.get("random_state", 0))
+    return {"ert": ert, "window_size": W, "n_bootstraps": n_boot, "random_state": rs}
 
 
 def _save_background(path: str, flat: FlatForest, frame: pd.DataFrame, **extra) -> None:
@@ -959,6 +1053,11 @@ def load_model(path: str, devices=None, **kw) -> B200Model:
         with np.load(mmd_path, allow_pickle=False) as z:
             sigma = float(z["mmd_sigma"])
         kw["mmd_sigma"] = None if math.isnan(sigma) else sigma
+    online_path = os.path.join(path, ONLINE_DRIFT_FILE)
+    if ("online_drift" not in kw and "mmd_reference" in kw and os.path.exists(online_path)
+            and os.environ.get("B200_ONLINE_DRIFT", "gpu") != "off"):
+        with open(online_path) as f:
+            kw["online_drift"] = json.load(f)
     trust_path = os.path.join(path, TRUST_FILE)
     if "trust_reference" not in kw and os.path.exists(trust_path) and os.environ.get("B200_TRUST", "gpu") != "off":
         kw["trust_reference"] = _load_background(trust_path, flat)

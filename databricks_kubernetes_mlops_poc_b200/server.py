@@ -43,7 +43,7 @@ from fastapi import FastAPI, Request, Response
 from fastapi.exceptions import RequestValidationError
 from pydantic import ValidationError
 
-from . import ale, dependence, importance, interaction, mmd, trust
+from . import ale, dependence, importance, interaction, mmd, mmd_online, trust
 from .ingest import NativeRequestParser, parse_rows, rows_to_frame  # noqa: F401  (rows_to_frame re-exported)
 from .schema import ALL_FEATURES, CATEGORICAL_FEATURES, LABELLED_ROWS, NUMERIC_FEATURES, TARGET, LabelledApplicant, LoanApplicant, ModelOutput
 
@@ -804,7 +804,60 @@ def create_app(model=None, loader=None) -> FastAPI:
             None, lambda: m.mmd_drift(input_df, n_permutations=n_permutations, p_val=p_val, random_state=random_state))
         return Response(content=json.dumps(out, allow_nan=False, separators=(",", ":")).encode("utf-8"), media_type="application/json")
 
-    @app.post("/predict", response_model=ModelOutput, openapi_extra={"requestBody": _REQUEST_SCHEMA})
+    def _online_not_configured():
+        return Response(content=json.dumps({"detail": "this model has no online drift detector (configure_online_drift)"}), status_code=501,
+                        media_type="application/json")
+
+    def _online_state(m) -> Response:
+        st = m.online_drift_state()
+        body = {**st, "thresholds": np.asarray(st["thresholds"], dtype=np.float64).tolist()}
+        return Response(content=json.dumps(body, separators=(",", ":")).encode("utf-8"), media_type="application/json")
+
+    @app.post("/drift/online", openapi_extra={"requestBody": _REQUEST_SCHEMA})
+    async def drift_online(request: Request):
+        """Has the applicant stream moved away from the reference, and when?  Pushes the request's applicants, in order, into
+        the online MMD detector's sliding window (alibi-detect's MMDDriftOnline, configured with an expected run time
+        `ert` between false alarms): per applicant `time` (applicants pushed since configure or reset), `test_stat` (the
+        window's MMD^2 against the sub-reference), `threshold` and `is_drift`, then `first_drift` (the first time of this
+        request in detection, else null).  The detector keeps its window across requests; concurrent requests are pushed
+        whole, one after another, in the order they take the model's lock.  A detection resets nothing: POST
+        /drift/online/reset does.  501 when no detector is configured; 422 for no applicants or a request above 2^36
+        kernel values."""
+        m = ml_models["credit_default"]
+        if not getattr(m, "online_drift_configured", False):
+            return _online_not_configured()
+        input_df = parser.frame(await request.body())
+        try:
+            mmd_online.check_push(len(input_df), m.mmd_reference_rows, m.online_drift_state()["window_size"])
+        except ValueError as e:
+            return _unprocessable(str(e))
+        out = await asyncio.get_running_loop().run_in_executor(None, lambda: m.online_drift(input_df))
+        body = {"time": np.asarray(out["time"]).tolist(), "test_stat": np.asarray(out["test_stat"], dtype=np.float64).tolist(),
+                "threshold": np.asarray(out["threshold"], dtype=np.float64).tolist(), "is_drift": np.asarray(out["is_drift"]).tolist(),
+                "first_drift": out["first_drift"], "ert": out["ert"], "window_size": out["window_size"]}
+        return Response(content=json.dumps(body, separators=(",", ":")).encode("utf-8"), media_type="application/json")
+
+    @app.post("/drift/online/reset")
+    async def drift_online_reset():
+        """Start the online detector's stream again: the window of its configuration, time 0.  -> the state as GET
+        /drift/online gives it.  501 when no detector is configured."""
+        m = ml_models["credit_default"]
+        if not getattr(m, "online_drift_configured", False):
+            return _online_not_configured()
+        await asyncio.get_running_loop().run_in_executor(None, m.reset_online_drift)
+        return _online_state(m)
+
+    @app.get("/drift/online")
+    async def drift_online_get():
+        """The online detector's configuration (`ert`, `window_size`, `n_bootstraps`, `random_state`, `thresholds`,
+        `sub_reference_rows`, `split_attempts`) and `time`, the applicants pushed since configure or reset.  501 when no
+        detector is configured."""
+        m = ml_models["credit_default"]
+        if not getattr(m, "online_drift_configured", False):
+            return _online_not_configured()
+        return _online_state(m)
+
+    @app.post("/predict",response_model=ModelOutput, openapi_extra={"requestBody": _REQUEST_SCHEMA})
     async def predict(request: Request):
         """Score a list of loan applicants: default probability, outlier flag, per-feature batch drift."""
         # list[LoanApplicant] semantics (422 on a type error, defaults filled): native one-pass parser for bodies of the

@@ -545,6 +545,37 @@ int b2f_model_attach_mmd_reference(b2f_model *m, const void *rows, int64_t n, in
 int b2f_mmd_drift(b2f_model *m, const void *rows, int64_t n, int row_format, const int32_t *subsets, int n_perm, double *mmd2_obs,
                   double *mmd2_perm, float *device_ms);
 
+/* ---- online MMD drift detector (csrc/mmd_online.cuh) ----
+ * alibi-detect's MMDDriftOnline on the attached MMD reference (its embedding, sigma and kernel; n_ref rows): a sliding
+ * window of W rows over a stream, compared with a sub-reference R of rw = n_ref - E rows, E = 2W - 1.  With
+ * r_i = sum_{j != i} k(i, j) over the reference, T = sum r, c_s = sum_{i in R} k(i, x_s) and S_WW the sum of k over the
+ * ordered pairs of a window:  stat = K_RR / (rw (rw - 1)) + S_WW / (W (W - 1)) - 2 sum_{s in window} c_s / (rw W).
+ *
+ * b2f_mmd_online_bootstrap: etw holds n_boot sequences y of E reference positions (distinct within a sequence); R is the
+ * other rw rows.  stats[b * W + w] gets the statistic of the window y_w .. y_{w+W-1} and k_rr[b] the pair sum over R,
+ * K_RR = T - 2 sum_{j in y} r_j + (the pair sum inside y).  The host sets the thresholds from them.
+ * b2f_mmd_online_configure: perm is a permutation of the reference; R = perm[0 .. rw), the initial window is the last W
+ * rows of perm.  It keeps R's embedding, K_RR and the window state (a copy too, for reset) and sets t = 0.
+ * b2f_mmd_online_push: pushes n rows (B2F_ROWS_WORDS24 or B2F_ROWS_PACKED64, host memory) in row order; stat[i] gets the
+ * statistic of the window that ends at row i, and *t_first (may be NULL) the time of row 0 (t counts the rows pushed since
+ * configure or reset, from 1).  The rows go in pieces whose scratch stays under 256 MiB, the window state carried across.
+ * b2f_mmd_online_reset: back to the window state of configure, t = 0.
+ *
+ * Float64, no float atomics: every statistic depends only on the reference, the configuration and the stream's rows, not on
+ * how the stream is cut into pushes, the row format or the run.  Attaching an MMD reference drops the configuration.
+ *
+ * Limits and errors: 2 <= W <= B2F_MMD_ONLINE_MAX_WINDOW, n_ref >= 2W + 1, 1 <= n_boot <= B2F_MMD_ONLINE_MAX_BOOT, n >= 1.
+ * B2F_ESTATE without an MMD reference, or (push, reset) before configure; B2F_EINVAL for a window or count out of range, a
+ * position outside [0, n_ref) or repeated within a sequence, ranked rows or a NULL pointer; B2F_ENOMEM with the byte count
+ * when a device buffer cannot be allocated.  device_ms (may be NULL): from the first upload to the last copy back, CUDA
+ * events on the compute stream. */
+#define B2F_MMD_ONLINE_MAX_WINDOW 256
+#define B2F_MMD_ONLINE_MAX_BOOT 100000
+int b2f_mmd_online_bootstrap(b2f_model *m, const int32_t *etw, int n_boot, int window, double *stats, double *k_rr, float *device_ms);
+int b2f_mmd_online_configure(b2f_model *m, const int32_t *perm, int window, float *device_ms);
+int b2f_mmd_online_push(b2f_model *m, const void *rows, int64_t n, int row_format, double *stat, int64_t *t_first, float *device_ms);
+int b2f_mmd_online_reset(b2f_model *m);
+
 /* ---- k-nearest reference rows of trust scores (csrc/knn.cuh) ----
  * The exact k nearest rows of each class of a labelled reference, the half of alibi's TrustScore that needs the GPU.  The
  * space is the MMD test's: a row is embedded as its category codes (one-hot; -1 = the all-zero block) and its numerics as
